@@ -23,6 +23,7 @@ COMMON = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "-Xcompiler",
 # persistent kernel and the 5-launch path differ in the last bit).  The GEMM-side hot loops use explicit fmaf.
 UNITS = {  # translation unit -> extra flags
     "api.cu": [],
+    "cbfqp.cu": ["-fmad=false"],
     "geometry.cu": ["-fmad=false"],
     "gnn.cu": ["-fmad=false"],
     "rollout_persist.cu": ["-fmad=false"],

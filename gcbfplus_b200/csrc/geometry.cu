@@ -478,14 +478,14 @@ env_step_kernel(const gcbf_env_desc d, const float* __restrict__ agent, const fl
         float sq = 0.f;
 #pragma unroll
         for (int c = 0; c < NU; ++c) {
-            // mode 0: a = 2 pi + u_ref (gcbf_plus.py:182-186); 1: given action; 2: a = u_ref (test.py --u-ref)
-            act[c] = (mode == 0) ? (2.f * pi[a * NU + c] + ur[c]) : ((mode == 1) ? action[a * NU + c] : ur[c]);
+            // mode 0: a = 2 pi + u_ref (gcbf_plus.py:182-186); 1 / 3: given action; 2: a = u_ref (test.py --u-ref)
+            act[c] = (mode == 0) ? (2.f * pi[a * NU + c] + ur[c]) : ((mode == 1 || mode == 3) ? action[a * NU + c] : ur[c]);
             u[c] = isnan(act[c]) ? act[c] : fminf(fmaxf(act[c], -d.u_lim), d.u_lim);  // clip_action
             const float df = u[c] - ur[c];
             sq = (c == 0) ? df * df : sq + df * df;
-            if (mode != 1) action[a * NU + c] = act[c];
+            if (mode == 0 || mode == 2) action[a * NU + c] = act[c];
         }
-        euler_dev<KIND>(d, x, gl, u, xn);
+        euler_dev<KIND>(d, x, gl, u, xn, mode != 3);   // mode 3: DubinsCar stop mask off
 #pragma unroll
         for (int c = 0; c < SD; ++c) next_agent[a * SD + c] = xn[c];
         const float nr = sqrtf(sq);
@@ -986,7 +986,7 @@ extern "C" __attribute__((visibility("default"))) int32_t gcbf_env_step(const gc
     GCBF_REQUIRE(agent && goal && row_start && row_deg && edge_src && action && next_agent && reward && cost,
                  "NULL pointer argument");
     GCBF_REQUIRE(desc->n_obs == 0 || obstacles, "obstacles is NULL but n_obs > 0");
-    GCBF_REQUIRE(mode >= 0 && mode <= 2 && (mode != 0 || pi), "bad mode %d (mode 0 needs pi)", mode);
+    GCBF_REQUIRE(mode >= 0 && mode <= 3 && (mode != 0 || pi), "bad mode %d (mode 0 needs pi)", mode);
     const int obw = env_pd(desc->env_kind) == 2 ? 16 : 4;
     const size_t smem = sizeof(float) * (size_t)desc->n_obs * obw;
     GCBF_REQUIRE(smem <= 40 * 1024, "too many obstacles for env_step");

@@ -189,9 +189,10 @@ __device__ __forceinline__ void u_ref_dev(const gcbf_env_desc& d, const float* x
 }
 
 // agent_step_euler (double_integrator.py:128-143; SI :104-109; Dubins :104-122; LD :123-134)
+// stop = false: the DubinsCar stop mask is off (env.enable_stop = False, dubins_car.py:138-142)
 template <int KIND>
 __device__ __forceinline__ void euler_dev(const gcbf_env_desc& d, const float* x, const float* gl, const float* u,
-                                          float* xn) {
+                                          float* xn, const bool stop_mask = true) {
     using T = EnvTraits<KIND>;
     constexpr int SD = T::SD, NU = T::NU;
     float xd[SD];
@@ -205,7 +206,7 @@ __device__ __forceinline__ void euler_dev(const gcbf_env_desc& d, const float* x
         xd[3] = u[1] / d.mass;
     } else if (KIND == GCBF_ENV_DUBINS_CAR) {
         const float ddx = x[0] - gl[0], ddy = x[1] - gl[1];
-        const float stop = (sqrtf(ddx * ddx + ddy * ddy) < d.half_r) ? 1.f : 0.f;
+        const float stop = (stop_mask && sqrtf(ddx * ddx + ddy * ddy) < d.half_r) ? 1.f : 0.f;
         const float keep = 1.f - stop;
         xd[0] = (cosf(x[2]) * x[3]) * keep;
         xd[1] = (sinf(x[2]) * x[3]) * keep;

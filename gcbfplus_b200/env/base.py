@@ -493,14 +493,20 @@ class MultiAgentEnv(ABC):
         return action, nxt, reward, cost
 
     def step(self, graph: SwarmGraph, action: torch.Tensor, get_eval_info: bool = False) -> StepResult:
-        """env.step (double_integrator.py:145-181)."""
+        """env.step (double_integrator.py:145-181).  enable_stop = False (DubinsCar under DecShareCBF) steps without
+        the stop mask (dubins_car.py:138-142)."""
         self._t += 1
-        _, nxt, reward, cost = self._dynamics(graph, action, None, 1)
+        _, nxt, reward, cost = self._dynamics(graph, action, None, self.action_step_mode)
         done = torch.zeros(graph.n_graphs, dtype=torch.bool, device=graph.agent.device)
         info = {}
         if get_eval_info:
             info["inside_obstacles"] = self.inside_obstacles(graph)
         return StepResult(self.get_graph(nxt, graph.goal, graph.obstacle), reward, cost, done, info)
+
+    @property
+    def action_step_mode(self) -> int:
+        """gcbf_env_step mode of a step with a given action: 1, or 3 when the DubinsCar stop mask is off."""
+        return 1 if getattr(self, "enable_stop", True) else 3
 
     def forward_graph(self, graph: SwarmGraph, action: torch.Tensor) -> SwarmGraph:
         """env.forward_graph (double_integrator.py:340-354): next agent states on the same

@@ -12,7 +12,7 @@ class DubinsCar(MultiAgentEnv):
     PARAMS = {"car_radius": 0.05, "comm_radius": 0.5, "n_rays": 16, "obs_len_range": [0.1, 0.6], "n_obs": 8}
 
     def _setup_dynamics(self) -> None:
-        self.enable_stop = True  # dubins_car.py:54 (the CUDA step always applies the stop mask)
+        self.enable_stop = True  # dubins_car.py:54; False (DecShareCBF) turns the stop mask of step() off
 
     def _thresholds(self) -> dict:
         r = self.radius  # dubins_car.py:398-440

@@ -7,6 +7,8 @@ Two device paths with the same arithmetic (bit-identical results, tests/test_gpu
 * 5-launch env-step (gcbf_rollout_step), the whole T-step loop captured in one CUDA graph: LinearDrone, n > 512,
   GCBF_PERSISTENT=0, the u_ref policy.
 No host sync inside the loop on either path.
+The CBF-QP baselines (algo/cbf_qp.py) run on the CUDA-graph path: per step the pairwise CBFs + QP solve (2 launches),
+env.step with the QP action as input, and the graph build of the next state.
 """
 from __future__ import annotations
 
@@ -17,6 +19,7 @@ from typing import Optional
 import torch
 
 from .. import _lib
+from ..algo.cbf_qp import BASELINES, iter_stats
 from ..algo.params import NetParams
 from ..utils.graph import SwarmGraph
 from .data import Rollout
@@ -44,13 +47,20 @@ class _Chain:
         n_ws = env.lib.gcbf_rollout_workspace_floats(C.byref(self.desc))
         self.ws = torch.empty(int(n_ws), dtype=f32, device=dev)
         self.stream = None
+        if eng.controller is not None:
+            # CBF-QP baseline: pairwise-CBF workspace, relaxations (scratch) and the per-step iteration record
+            n_qp = env.lib.gcbf_cbfqp_workspace_floats(C.byref(self.desc))
+            self.qp_ws = torch.empty(int(n_qp), dtype=f32, device=dev)
+            self.qp_r = torch.empty(E, N, 3, dtype=f32, device=dev)
+            self.qp_iters = torch.zeros(eng.T, eng.controller._n_solves(E, N), dtype=i32, device=dev)
 
 
 class RolloutEngine:
     def __init__(self, env, n_envs: int, T: Optional[int] = None, n_obs: Optional[int] = None,
                  use_cuda_graph: bool = True, policy: str = "actor", n_chains: Optional[int] = None,
                  persistent: Optional[bool] = None):
-        """policy: 'actor' (a = 2 pi + u_ref, algo.step) or 'u_ref' (test.py --u-ref).
+        """policy: 'actor' (a = 2 pi + u_ref, algo.step), 'u_ref' (test.py --u-ref), or a CBF-QP baseline: a
+        DecShareCBF / CentralizedCBF object, or its name ('dec_share_cbf' / 'centralized_cbf': built with alpha = 1).
         n_chains: the environments are split into independent chains that run as parallel branches of
         the CUDA graph (each per-step kernel is latency-bound and fills a fraction of the 132 SMs, so
         concurrent chains overlap their launch / tail latencies).  Results do not depend on it."""
@@ -58,6 +68,17 @@ class RolloutEngine:
         self.E = n_envs
         self.T = T or env.max_episode_steps
         self.O = env.params["n_obs"] if n_obs is None else n_obs
+        self.controller = None
+        if not isinstance(policy, str):
+            self.controller, policy = policy, policy.NAME
+        elif policy in BASELINES:
+            self.controller = BASELINES[policy](env, env.node_dim, env.edge_dim, env.state_dim, env.action_dim,
+                                                env.num_agents)
+        elif policy not in ("actor", "u_ref"):
+            raise ValueError(f"unknown rollout policy {policy!r}")
+        if self.controller is None and not getattr(env, "enable_stop", True):
+            raise ValueError("the actor / u_ref rollouts apply the DubinsCar stop mask; env.enable_stop is False "
+                             "(set by DecShareCBF)")
         self.policy = policy
         self.use_cuda_graph = use_cuda_graph
         dev = env.device
@@ -151,10 +172,19 @@ class RolloutEngine:
                 stream)
             _lib.check(rc, "gcbf_rollout_step")
             return
+        mode = 2                        # u_ref policy
+        if self.controller is not None:  # CBF-QP action, then env.step with it as input
+            c = self.controller
+            rc = getattr(env.lib, c._ENTRY)(C.byref(d), c.alpha, c.max_iter, c.tol, self.agent[t, ch.e0].data_ptr(),
+                                            self.goal[ch.e0].data_ptr(), self.hits[t, ch.e0].data_ptr(),
+                                            self.actions[t, ch.e0].data_ptr(), ch.qp_r.data_ptr(),
+                                            ch.qp_iters[t].data_ptr(), ch.qp_ws.data_ptr(), ch.qp_ws.numel(), stream)
+            _lib.check(rc, c._ENTRY)
+            mode = env.action_step_mode
         rc = env.lib.gcbf_env_step(C.byref(d), self.agent[t, ch.e0].data_ptr(), self.goal[ch.e0].data_ptr(), obs,
                                    None, ch.row_start[b].data_ptr(), ch.row_deg[b].data_ptr(), ch.edge_src[b].data_ptr(),
                                    self.actions[t, ch.e0].data_ptr(), self.agent[t + 1, ch.e0].data_ptr(),
-                                   self.rewards[t, ch.e0:].data_ptr(), self.costs[t, ch.e0:].data_ptr(), 2, stream)
+                                   self.rewards[t, ch.e0:].data_ptr(), self.costs[t, ch.e0:].data_ptr(), mode, stream)
         _lib.check(rc, "gcbf_env_step")
         self._build(ch, t + 1, stream)
 
@@ -238,6 +268,13 @@ class RolloutEngine:
             self.launches_per_run = int(lib.gcbf_launch_count() - n0)
         if check:
             self.check_overflow()
+
+    def qp_stats(self) -> dict:
+        """CBF-QP baselines: median / max iterations and capped solves over every solve of the last run() (reads the
+        device record once; call after run())."""
+        if self.controller is None:
+            raise RuntimeError("qp_stats() needs a CBF-QP baseline policy")
+        return iter_stats(torch.cat([ch.qp_iters.reshape(-1) for ch in self.chains]))
 
     def check_overflow(self) -> None:
         c = self.counters.cpu()

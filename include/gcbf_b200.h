@@ -153,7 +153,8 @@ int32_t gcbf_gnn_infer(const gcbf_env_desc* desc, int32_t net_kind, int32_t out_
  * env.step minus get_graph (env/double_integrator.py:145-198: clip_action,
  * agent_step_euler, reward, get_cost).
  * mode 0: action <- 2*pi + u_ref (output);  mode 1: `action` is an INPUT (env.step(graph, action));
- * mode 2: action <- u_ref (test.py --u-ref).
+ * mode 2: action <- u_ref (test.py --u-ref);  mode 3: as mode 1 with the DubinsCar stop mask off
+ * (env.enable_stop = False, env/dubins_car.py:138-142, which DecShareCBF sets; other envs: same as mode 1).
  * Outputs: action [A,nu] (unclipped a, what the rollout records), next_agent [A,sd],
  * reward [G], cost [G]. */
 int32_t gcbf_env_step(const gcbf_env_desc* desc, const float* agent, const float* goal,
@@ -330,6 +331,41 @@ int32_t gcbf_qp_labels(const gcbf_env_desc* desc, float alpha, int32_t use_tenso
                        const int32_t* edge_recv, const int32_t* edge_src, const int32_t* counters,
                        float* u_qp, float* aux, int32_t* iters, float* workspace, int64_t workspace_floats,
                        void* stream);
+
+/* ---------------------------------------------------------------- CBF-QP baseline controllers
+ * Replace the reference's hand-written baselines for a batch of G graphs: the pairwise CBFs
+ * (gcbfplus/algo/utils.py:44-349, get_pwise_cbf_fn :413-439, k = 3), DecShareCBF.get_qp_action
+ * (algo/dec_share_cbf.py:61-150) and CentralizedCBF.get_qp_action (algo/centralized_cbf.py:64-117).
+ * Candidates of agent i: [the N agents of its graph | its own R hit nodes], squared distance with the self entry at
+ * 100, the 3 nearest in stable order.  Inputs: agent / goal [G,N,sd], hits [G,N,R,pd].
+ *
+ * gcbf_cbf_pairwise (get_cbf + the Lie terms of its jax.jacfwd):
+ *   k_idx [G,N,3] int32: candidate index (j < N: agent j of the graph; N + k: hit node k of this agent);
+ *   k_isobs [G,N,3] uint8 (k_idx >= N);  k_h, k_lf_h [G,N,3];  k_lg_self [G,N,3,nu] = dh/dx_i g(x_i);
+ *   k_lg_other [G,N,3,nu] = dh/dx_j g(x_j) for an agent pick j != i, else 0 (NULL: not written).
+ *   k_lf_h includes the picked agent's drift: dh/dx_i f(x_i) + dh/dx_j f(x_j).
+ * gcbf_cbfqp_dec_share: one QP per agent, x = [u (nu) | r (3)],
+ *   min 1/2|u|^2 - u_ref.u + 5|r|^2 + 1000 sum r  s.t.  -Lg_self u - r <= resp (Lf_h + alpha h),  |u| <= u_lim,  r >= 0,
+ *   resp = 1 for an obstacle pick, 0.5 for an agent pick.  u [G,N,nu]; r [G,N,3] or NULL;
+ *   iters [G,N] or NULL (solves: one per agent).
+ * gcbf_cbfqp_centralized: one QP per graph, x = [u (N nu) | r (3N)], rows (i, k) with Lg blocks of agent i and of
+ *   the picked agent, b = Lf_h + alpha h.  n_agents <= GCBF_CBFQP_CENTRAL_MAX_AGENTS, LinearDrone <= 999 (the
+ *   graph's QP lives in shared memory; larger is rejected with status -1).  u [G,N,nu]; r [G,N,3] or NULL; iters [G] or NULL (solves: one per graph).
+ * Both solve the dual exactly in fp64 (unique minimiser): max_iter caps the iterations, tol is the stopping threshold
+ * on the projected dual-gradient residual.  iters[s] = iterations of solve s, with bit 30 set when the cap was hit
+ * before the stopping test passed (the iterate at the cap is returned).
+ *   workspace: gcbf_cbfqp_workspace_floats(desc) floats (holds the pairwise terms). */
+#define GCBF_CBFQP_CENTRAL_MAX_AGENTS 1024
+int32_t gcbf_cbf_pairwise(const gcbf_env_desc* desc, const float* agent, const float* hits, int32_t* k_idx,
+                          uint8_t* k_isobs, float* k_h, float* k_lf_h, float* k_lg_self, float* k_lg_other,
+                          void* stream);
+int64_t gcbf_cbfqp_workspace_floats(const gcbf_env_desc* desc);
+int32_t gcbf_cbfqp_dec_share(const gcbf_env_desc* desc, float alpha, int32_t max_iter, float tol, const float* agent,
+                             const float* goal, const float* hits, float* u, float* r, int32_t* iters,
+                             float* workspace, int64_t workspace_floats, void* stream);
+int32_t gcbf_cbfqp_centralized(const gcbf_env_desc* desc, float alpha, int32_t max_iter, float tol,
+                               const float* agent, const float* goal, const float* hits, float* u, float* r,
+                               int32_t* iters, float* workspace, int64_t workspace_floats, void* stream);
 
 /* ---------------------------------------------------------------- dense-layer building blocks
  * The fp32 GEMM family the MLPs are made of (flax nn.Dense, gcbfplus/nn/mlp.py:19-21, and its

@@ -3,7 +3,9 @@
 Video rendering is out of scope (SURVEY 2 row 17) -> --no-video is implied; --cbf <agent id> computes the CBF
 contour grids the reference hands to its renderer (test.py:125-131, trainer/utils.py:149-168) and saves them as
 <path>/cbf_contours/epi<k>_agent<id>.npz (b_xs, b_ys, bb_h per time step).  --nojit-rollout is accepted: the
-reference needs it to survive n >= 512 with dense graphs (env/base.py:191-259); the sparse rollout engine has no such limit."""
+reference needs it to survive n >= 512 with dense graphs (env/base.py:191-259); the sparse rollout engine has no such limit.
+--algo centralized_cbf | dec_share_cbf without --path runs the CBF-QP baseline controllers (test.py:88-103) with
+alpha = --alpha and writes to ./logs/<env>/<algo>."""
 import argparse
 import os
 
@@ -11,6 +13,7 @@ import numpy as np
 import yaml
 
 from gcbfplus_b200.algo import make_algo
+from gcbfplus_b200.algo.cbf_qp import BASELINES
 from gcbfplus_b200.env import make_env
 from gcbfplus_b200.trainer.rollout import RolloutEngine
 from gcbfplus_b200.trainer.utils import cbf_contours, test_rates
@@ -30,7 +33,18 @@ def test(args):
                    area_size=args.area_size, max_step=args.max_step, max_travel=args.max_travel)
     policy = "u_ref"
     algo = None
-    if not args.u_ref:
+    baseline = args.algo in BASELINES and args.path is None and not args.u_ref
+    if baseline:
+        if args.cbf is not None:
+            raise SystemExit(f"--cbf: the CBF contours are not available for the {args.algo} baseline (the reference's "
+                             "contour path only works with a trained GCBF+ CBF)")
+        assert args.env is not None, "--env required for a baseline"
+        algo = make_algo(algo=args.algo, env=env, node_dim=env.node_dim, edge_dim=env.edge_dim,
+                         state_dim=env.state_dim, action_dim=env.action_dim, n_agents=env.num_agents, alpha=args.alpha)
+        policy = algo
+        path = os.path.join(f"./logs/{args.env}/{args.algo}")
+        os.makedirs(path, exist_ok=True)
+    elif not args.u_ref:
         assert args.path is not None, "--path or --u-ref required"
         model_path = os.path.join(args.path, "models")
         step = max(int(m) for m in os.listdir(model_path) if m.isdigit()) if args.step is None else args.step
@@ -52,7 +66,7 @@ def test(args):
         os.makedirs(path, exist_ok=True)
     n_epi = args.epi - args.offset
     eng = RolloutEngine(env, n_epi, T=env.max_episode_steps, policy=policy)
-    if algo is not None:
+    if algo is not None and not baseline:
         eng.set_params(algo.actor_params)
     # test.py:117-119,158: test_keys = split(PRNGKey(seed), 1000)[:epi][offset:]; episode i resets with
     # split(test_keys[i])[0].  All episodes run as one batch here.
@@ -75,6 +89,13 @@ def test(args):
           f"cost: {np.mean(costs):.3f}, min/max cost: {np.min(costs):.3f}/{np.max(costs):.3f}, "
           f"safe_rate: {safe_mean * 100:.3f}%, finish_rate: {finish_mean * 100:.3f}%, "
           f"success_rate: {succ.mean() * 100:.3f}%")
+    if baseline:
+        st = eng.qp_stats()
+        print(f"QP iterations: median {st['iters_median']:.0f}, max {st['iters_max']}, "
+              f"capped {st['capped']} of {st['solves']} solves")
+        if st["capped"]:
+            print(f"WARNING: {st['capped']} QP solve(s) hit the iteration cap ({algo.max_iter}); their actions are the "
+                  "capped iterates, not the exact QP minimisers")
     if args.log:
         with open(os.path.join(path, "test_log.csv"), "a") as f:
             f.write(f"{env.num_agents},{args.epi},{env.max_episode_steps},{env.area_size},{env.params['n_obs']},"
