@@ -38,6 +38,11 @@ constexpr int WG_ROWS_BYTES = 64 * 128;   // the 64 rows of one warpgroup inside
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
+// The dynamic shared-memory window rounded up to the 1024-byte alignment SWIZZLE_128B needs.  The result is the
+// __shared__ array plus a byte offset: a round trip through uintptr_t would erase its address space, and every access
+// through it would become a generic 64-bit LD / ST instead of LDS / STS.
+__device__ __forceinline__ uint8_t* smem_align1024(uint8_t* raw) { return raw + ((1024u - (smem_u32(raw) & 1023u)) & 1023u); }
+
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
 }
@@ -232,7 +237,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                const int32_t* __restrict__ m_ptr, const int m_fixed, const int m_cap, const int K, const int N,
                const int ndot) {
     extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+    uint8_t* smem = smem_align1024(smem_raw);
     uint64_t* full = reinterpret_cast<uint64_t*>(smem + STAGES * STG);   // [STAGES] TMA bytes landed
     uint64_t* empty = full + STAGES;                                      // [STAGES] MMAs of the stage retired
 
@@ -462,7 +467,7 @@ gemm_tn_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant
     using CF = TnCfg<BNT>;
     constexpr int MR = 32 * BNT / 256;                       // m rows of dY converted per thread
     extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+    uint8_t* smem = smem_align1024(smem_raw);
     uint8_t* planes = smem + TN_RAWS * CF::RAW;
     uint64_t* full = reinterpret_cast<uint64_t*>(planes + CF::PB * CF::PLANES);
     uint64_t* empty = full + TN_RAWS;

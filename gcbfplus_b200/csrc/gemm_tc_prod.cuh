@@ -153,7 +153,7 @@ gemm_tc_prod_kernel(const __grid_constant__ CUtensorMap tmBh, const __grid_const
                     const int32_t* __restrict__ m_ptr, const int m_fixed, const int m_cap) {
     constexpr int ED = EnvTraits<KIND>::ED;
     extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+    uint8_t* smem = smem_align1024(smem_raw);
     uint64_t* full = reinterpret_cast<uint64_t*>(smem + STAGES * STG);
     uint64_t* empty = full + STAGES;
     float* sW = reinterpret_cast<float*>(smem + STAGES * STG + 256);
@@ -220,7 +220,7 @@ edge_chain_kernel(const __grid_constant__ CUtensorMap tmBh, const __grid_constan
                   const int32_t* __restrict__ m_ptr, const int m_cap, const ChainArgs ch) {
     constexpr int ED = EnvTraits<KIND>::ED;
     extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+    uint8_t* smem = smem_align1024(smem_raw);
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * STG);
     uint64_t* full = bars;                 // [3]
     uint64_t* empty = bars + 3;            // [3]

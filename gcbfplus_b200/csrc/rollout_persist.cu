@@ -44,6 +44,23 @@ constexpr int MAX_OBS = 32;
 // B_MAIN: both consumer warpgroups' main-loop MMAs of an edge tile retired; B_T2F: its chained gate GEMM retired
 enum { B_FULL = 0, B_EMPTY = 3, B_B2F = 6, B_B2E = 8, B_MAIN = 10, B_T2F = 11, B_COUNT = 12 };
 
+// Rollout constants staged in shared memory once per rollout (float offsets).  The epilogues and the tail read them
+// per element, and every cluster barrier invalidates L1, so from global memory each phase would refetch them from L2.
+// NU = 2 in every 2-D environment.
+constexpr int PNU = 2;
+enum {
+    K_B23 = 0,          // [128] message bias (folded W23 layer)
+    K_BIAS_G = 128,     // [128] gate hidden-layer bias
+    K_AVEC = 256,       // [128] folded gate vector
+    K_BU1 = 384,        // [256] update-layer bias
+    K_BU1ROW = 640,     // [256] update-layer agent one-hot row
+    K_BUH = 896,        // [256] folded update / head bias
+    K_HO = 1152,        // [256][NU] folded output layer
+    K_BHO = K_HO + 256 * PNU,   // [NU] output bias
+    K_CST = K_BHO + PNU,        // [1] folded gate constant
+    K_FLOATS = K_CST + 1
+};
+
 struct PArgs {
     gcbf_env_desc d;
     int T, cap_env, C;
@@ -106,11 +123,11 @@ rollout_persist_kernel(const __grid_constant__ PArgs P, const __grid_constant__ 
                        const __grid_constant__ CUtensorMap tmV1) {
     using TR = EnvTraits<KIND>;
     constexpr int SD = TR::SD, ED = TR::ED, NU = TR::NU, PD = TR::PD;
-    static_assert(PD == 2, "persistent rollout kernel: 2-D environments");
+    static_assert(PD == 2 && NU == PNU, "persistent rollout kernel: 2-D environments");
     constexpr int OBW = 16, OBS2 = 24;
     constexpr int A_BYTES = 16384, B_BYTES = 16384;
     extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+    uint8_t* smem = smem_align1024(smem_raw);
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + 3 * STG);
     int* s_tot = reinterpret_cast<int*>(smem + 3 * STG + 256 + 16);       // [8] CTA edge totals of the cluster
     float* sW = reinterpret_cast<float*>(smem + 3 * STG + 512);            // [(ED + 3)][256]
@@ -121,6 +138,7 @@ rollout_persist_kernel(const __grid_constant__ PArgs P, const __grid_constant__ 
     int* s_off = reinterpret_cast<int*>(sbits + 64 * 16);                  // [APC + 1]
     unsigned* s_hb = reinterpret_cast<unsigned*>(s_off + 72);              // [APC]
     float* s_red = reinterpret_cast<float*>(s_hb + 64);                    // [3][PW]
+    float* sk = s_red + 3 * PW;                                            // [K_FLOATS] rollout constants
 
     const gcbf_env_desc& d = P.d;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -177,6 +195,18 @@ rollout_persist_kernel(const __grid_constant__ PArgs P, const __grid_constant__ 
         const int t = i / 256, c = i % 256;
         sW[(ED + t) * 256 + c] = P.W1[(ED + t) * 256 + c] + P.W1[(ED + 3 + 2) * 256 + c] + P.b1[c];
     }
+    auto stage = [&](int off, const float* src, int n) {
+        for (int i = tid; i < n; i += PT) sk[off + i] = src[i];
+    };
+    stage(K_B23, P.b23, 128);
+    stage(K_BIAS_G, P.bias_g, 128);
+    stage(K_AVEC, P.avec, 128);
+    stage(K_BU1, P.b_u1, 256);
+    stage(K_BU1ROW, P.b_u1row, 256);
+    stage(K_BUH, P.buh, 256);
+    stage(K_HO, P.ho, 256 * NU);
+    stage(K_BHO, P.bho, NU);
+    stage(K_CST, P.cst, 1);
     // obstacles of this environment (+ derived far-skip fields) and the ray table stay resident for the whole rollout
     if (O > 0) {
         const float* ob = P.obstacles + (d.obs_per_graph ? (size_t)env * O * OBW : 0);
@@ -273,7 +303,7 @@ rollout_persist_kernel(const __grid_constant__ PArgs P, const __grid_constant__ 
                     edge_tile_mainloop<ED>(dacc, smem, &bars[B_FULL], &bars[B_EMPTY], it_l, g, r, half, row_ok, sW, f, stype);
                     mbar_arrive(&bars[B_MAIN]);
                     bar_consumers();               // both main loops retired: the hand-over may overwrite stages 0-1
-                    drain_msg(dacc, smem, g, wt, P.b23, P.msg + (seg_e0 + (size_t)tile * BM) * 128, M_cur - tile * BM);
+                    drain_msg(dacc, smem, g, wt, sk + K_B23, P.msg + (seg_e0 + (size_t)tile * BM) * 128, M_cur - tile * BM);
                     fence_async_smem();
                     bar_wg(g);
                     float d2[64];
@@ -289,11 +319,11 @@ rollout_persist_kernel(const __grid_constant__ PArgs P, const __grid_constant__ 
                         mbar_arrive(&bars[B_B2E + slot]);
                     }
                     float q[2][1];
-                    frag_relu_dot<1>(d2, P.bias_g, P.avec, 1, 1, wt, q);
+                    frag_relu_dot<1>(d2, sk + K_BIAS_G, sk + K_AVEC, 1, 1, wt, q);
                     if ((lane & 3) == 0) {
                         const int rr = tile * BM + 64 * g + frag_row0(wt);
-                        if (rr < M_cur) P.logit[seg_e0 + rr] = q[0][0] + P.cst[0];
-                        if (rr + 8 < M_cur) P.logit[seg_e0 + rr + 8] = q[1][0] + P.cst[0];
+                        if (rr < M_cur) P.logit[seg_e0 + rr] = q[0][0] + sk[K_CST];
+                        if (rr + 8 < M_cur) P.logit[seg_e0 + rr + 8] = q[1][0] + sk[K_CST];
                     }
                     mbar_arrive(&bars[B_T2F]);
                     bar_consumers();               // the gate slots (stage 2) are drained before the next tile's A rows land
@@ -405,16 +435,16 @@ rollout_persist_kernel(const __grid_constant__ PArgs P, const __grid_constant__ 
                                 if (ml >= ga_hi) continue;
                                 const int n = nc0 + frag_col(wt, i);
                                 float2 o = make_float2(dacc[i], dacc[i + 1]);
-                                const float2 bb = *reinterpret_cast<const float2*>(P.b_u1 + n);
+                                const float2 bb = *reinterpret_cast<const float2*>(sk + K_BU1 + n);
                                 o.x += bb.x; o.y += bb.y;
-                                const float2 b2 = *reinterpret_cast<const float2*>(P.b_u1row + n);
+                                const float2 b2 = *reinterpret_cast<const float2*>(sk + K_BU1ROW + n);
                                 o.x += b2.x; o.y += b2.y;
                                 o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f);
                                 *reinterpret_cast<float2*>(P.v1 + (size_t)(env_a0 + ml) * 256 + n) = o;
                             }
                         } else {
                             float q[2][4];
-                            frag_relu_dot<4>(dacc, P.buh + nc0, P.ho + (size_t)nc0 * NU, NU, NU, wt, q);
+                            frag_relu_dot<4>(dacc, sk + K_BUH + nc0, sk + K_HO + nc0 * NU, NU, NU, wt, q);
                             if ((lane & 3) == 0)
 #pragma unroll
                                 for (int h = 0; h < 2; ++h)
@@ -472,7 +502,7 @@ rollout_persist_kernel(const __grid_constant__ PArgs P, const __grid_constant__ 
                     float sq = 0.f;
 #pragma unroll
                     for (int c = 0; c < NU; ++c) {
-                        const float act = 2.f * tanhf(zz[c] + P.bho[c]) + ur[c];
+                        const float act = 2.f * tanhf(zz[c] + sk[K_BHO + c]) + ur[c];
                         if (rec) act_t[a * NU + c] = act;
                         u[c] = isnan(act) ? act : fminf(fmaxf(act, -d.u_lim), d.u_lim);
                         const float df = u[c] - ur[c];
@@ -794,7 +824,7 @@ extern "C" __attribute__((visibility("default"))) int32_t gcbf_rollout_persisten
 
 static int persist_smem_bytes() {
     return 3 * rp::STG + 512 + 7 * 256 * 4 + rp::MAX_N * 4 * 4 + rp::MAX_OBS * 24 * 4 + 64 * 4 + 64 * 16 * 4 + 72 * 4 + 64 * 4 +
-           3 * rp::PW * 4 + 1024;
+           3 * rp::PW * 4 + rp::K_FLOATS * 4 + 1024;
 }
 
 /* Co-resident clusters of `cluster_size` CTAs of the persistent rollout kernel on the current device
