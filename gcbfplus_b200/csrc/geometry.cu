@@ -31,7 +31,7 @@ graph_build_kernel(const gcbf_env_desc d, const float* __restrict__ agent, const
     constexpr int OBW = (PD == 2) ? 16 : 4;
     extern __shared__ float smem[];
     const int N = d.n_agents, O = d.n_obs, R = d.n_hits;
-    constexpr int OBS2 = (PD == 2) ? 24 : 4;    // 2-D: packed rectangle + derived [14] reach^2, [15..18] edge dx, [19..22] edge dy
+    constexpr int OBS2 = (PD == 2) ? OBS2D : 4; // 2-D: packed rectangle + the derived fields of derive_far_fields
     float* spos = smem;                         // [N, PD]
     float* sobs = spos + N * PD;                // [O, OBS2]
     float* stab = sobs + O * OBS2;              // [n_rays, PD]
@@ -65,7 +65,6 @@ graph_build_kernel(const gcbf_env_desc d, const float* __restrict__ agent, const
         // into the other half of the caller's double buffer).
         __shared__ float s_red[3][GB_WARPS];
         const bool rec = blockIdx.x == 0;
-        const int A_tot = d.n_graphs * N;
         float acc[3] = {0.f, 0.f, 0.f};
         for (int i = tid; i < N; i += blockDim.x) {
             const size_t a = (size_t)g * N + i;
@@ -74,42 +73,25 @@ graph_build_kernel(const gcbf_env_desc d, const float* __restrict__ agent, const
                 const float4 v = *reinterpret_cast<const float4*>(tl.z + ((size_t)p * tl.z_cap + a) * 4);
                 zz[0] += v.x; zz[1] += v.y; zz[2] += v.z; zz[3] += v.w;
             }
-            float x[SD], gl[SD], ur[NU], u[NU], xn[SD];
+            float x[SD], gl[SD], ur[NU], act[NU], xn[SD];
 #pragma unroll
             for (int c = 0; c < SD; ++c) {
                 x[c] = tl.agent_prev[a * SD + c];
                 gl[c] = tl.goal[a * SD + c];
             }
-            u_ref_dev<KIND>(d, x, gl, ur);
-            float sq = 0.f;
+            policy_action<KIND>(d, x, gl, zz, tl.bHO, ur, act);
+            if (rec)
 #pragma unroll
-            for (int c = 0; c < NU; ++c) {
-                const float act = 2.f * tanhf(zz[c] + tl.bHO[c]) + ur[c];
-                if (rec) tl.action[a * NU + c] = act;
-                u[c] = isnan(act) ? act : fminf(fmaxf(act, -d.u_lim), d.u_lim);
-                const float df = u[c] - ur[c];
-                sq = (c == 0) ? df * df : sq + df * df;
-            }
-            euler_dev<KIND>(d, x, gl, u, xn);
+                for (int c = 0; c < NU; ++c) tl.action[a * NU + c] = act[c];
+            const float sq = step_agent<KIND>(d, x, gl, act, ur, true, xn);
 #pragma unroll
             for (int c = 0; c < PD; ++c) spos[i * PD + c] = xn[c];
             if (rec) {
 #pragma unroll
                 for (int c = 0; c < SD; ++c) tl.next_agent[a * SD + c] = xn[c];
                 const float nr = sqrtf(sq);
-                bool col = false;
-                const int rs = tl.row_start_prev[a], rd = tl.row_deg_prev[a];
-                for (int e = rs + 1; e < rs + rd; ++e) {
-                    const int sidx = tl.edge_src_prev[e];
-                    if (sidx < 0) break;
-                    float dd = 0.f;
-#pragma unroll
-                    for (int c = 0; c < PD; ++c) {
-                        const float dlt = x[c] - tl.agent_prev[(size_t)sidx * SD + c];
-                        dd = (c == 0) ? dlt * dlt : dd + dlt * dlt;
-                    }
-                    col = col || (d.two_r > sqrtf(dd));
-                }
+                const bool col = collides_prev<PD, SD>(x, tl.row_start_prev[a], tl.row_deg_prev[a], tl.edge_src_prev,
+                                                       tl.agent_prev, d.two_r);
                 bool in_obs = false;
                 if (O > 0) {
                     const float* ob = obstacles + (d.obs_per_graph ? (size_t)g * O * OBW : 0);
@@ -120,39 +102,11 @@ graph_build_kernel(const gcbf_env_desc d, const float* __restrict__ agent, const
                 acc[2] += in_obs ? 1.f : 0.f;
             }
         }
-        (void)A_tot;
-        if (rec) {
-#pragma unroll
-            for (int q = 0; q < 3; ++q) {
-                const float v = warp_sum(acc[q]);
-                if (lane == 0) s_red[q][warp] = v;
-            }
-            __syncthreads();
-            if (tid == 0) {
-                float t[3] = {0.f, 0.f, 0.f};
-                for (int w = 0; w < GB_WARPS; ++w) {
-                    t[0] += s_red[0][w];
-                    t[1] += s_red[1][w];
-                    t[2] += s_red[2][w];
-                }
-                reward[g] = -(t[0] / (float)N);
-                cost[g] = t[1] / (float)N + t[2] / (float)N;
-            }
-        }
+        if (rec) reduce_reward_cost<GB_WARPS>(acc, &s_red[0][0], N, reward + g, cost + g);
     }
     __syncthreads();
     if (PD == 2) {   // derived fields for the (conservative, exactness-preserving) far-obstacle skip
-        for (int o = tid; o < O; o += blockDim.x) {
-            float* ob = sobs + OBS2 * o;
-            const float reach = d.comm_radius + sqrtf(ob[2] * ob[2] + ob[3] * ob[3]) + 2e-3f;
-            ob[14] = reach * reach;
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-                const int kp = (k + 3) & 3;
-                ob[15 + k] = ob[6 + 2 * kp] - ob[6 + 2 * k];   // x4 - x3
-                ob[19 + k] = ob[7 + 2 * kp] - ob[7 + 2 * k];   // y4 - y3
-            }
-        }
+        derive_far_fields(sobs, O, d.comm_radius, tid, blockDim.x);
         __syncthreads();
     }
 
@@ -171,55 +125,7 @@ graph_build_kernel(const gcbf_env_desc d, const float* __restrict__ agent, const
     // ---------------- LiDAR (env/utils.py:49-131)
     if (do_cast && valid) {
         if (PD == 2) {
-            const bool ray_ok = lane < d.n_rays;
-            const int rl = ray_ok ? lane : 0;
-            const float x1 = p[0], y1 = p[1];
-            const float x2 = x1 + stab[rl * 2 + 0], y2 = y1 + stab[rl * 2 + 1];
-            const float rdx = x1 - x2, rdy = y1 - y2;
-            float alpha;
-            if (O == 0) {
-                alpha = 1.f * NO_HIT;
-            } else {
-                // A rectangle whose bounding circle is out of the ray's reach cannot be hit or contain the agent:
-                // every edge test gives valid = 0 and alpha = 0 * alpha + 1e6 = 1e6 exactly -- unless an edge is
-                // exactly parallel to the ray (det == 0 -> alpha = x/0 -> NaN in the reference, obstacle.py:88-94).
-                // The skip is taken only when it is bit-identical to the full evaluation (agent-uniform branch).
-                alpha = NO_HIT;
-                bool is_in = false;
-                for (int o = 0; o < O; ++o) {
-                    const float* ob = sobs + OBS2 * o;
-                    const float cx = x1 - ob[0], cy = y1 - ob[1];
-                    const bool far = (cx * cx + cy * cy) > ob[14];
-                    bool degenerate = false;
-                    if (far) {
-#pragma unroll
-                        for (int k = 0; k < 4; ++k) {
-                            const float det = rdx * ob[19 + k] - rdy * ob[15 + k];
-                            degenerate = degenerate || !(det != 0.f);   // det == 0 or NaN
-                        }
-                    }
-                    if (!far) is_in = is_in || rect_inside(ob, x1, y1, 0.f);
-                    if (!far || __any_sync(0xffffffffu, degenerate))
-                        alpha = nanmin(alpha, rect_raytrace(ob, x1, y1, x2, y2));
-                }
-                alpha = alpha * (1.f - (is_in ? 1.f : 0.f));
-            }
-            const float hx = x1 + (x2 - x1) * alpha;
-            const float hy = y1 + (y2 - y1) * alpha;
-            SortKey k;
-            k.flag = ray_ok ? (isnan(alpha) ? 1 : 0) : 2;
-            k.alpha = alpha;
-            k.idx = lane;
-            // argsort is stable: when no ray of this agent hit anything (every alpha == 1e6) the order is the
-            // identity and the 15-stage warp sort can be skipped (warp-uniform, the common case in open space)
-            const bool all_miss = __all_sync(0xffffffffu, !ray_ok || alpha == NO_HIT);
-            if (!all_miss) k = warp_sort32(k, lane);
-            const float shx = __shfl_sync(0xffffffffu, hx, k.idx);
-            const float shy = __shfl_sync(0xffffffffu, hy, k.idx);
-            if (lane < R) {
-                my_hits[lane * 2 + 0] = shx;
-                my_hits[lane * 2 + 1] = shy;
-            }
+            lidar2d_warp(p, stab, sobs, O, d.n_rays, R, lane, my_hits);
         } else {
             const bool is_in = (O > 0) ? inside_any<PD>(sobs, O, p, 0.f) : false;
             const float keep = 1.f - (is_in ? 1.f : 0.f);
@@ -332,68 +238,11 @@ graph_build_kernel(const gcbf_env_desc d, const float* __restrict__ agent, const
     }
     __syncwarp();
 
-    // ---------------- active hit nodes: ||p - hit|| < comm_radius - 0.1 (double_integrator.py:254-257)
-    unsigned hit_bits = 0u;
-    {
-        bool act = false;
-        if (valid && lane < R) {
-            float acc = 0.f;
-#pragma unroll
-            for (int c = 0; c < PD; ++c) {
-                const float dlt = p[c] - my_hits[lane * PD + c];
-                acc = (c == 0) ? dlt * dlt : acc + dlt * dlt;
-            }
-            act = acc < d.lidar_sq_thr;   // == (sqrtf(acc) < lidar_radius), threshold precomputed exactly on the host
-        }
-        hit_bits = __ballot_sync(0xffffffffu, act);
-    }
-    // ---------------- neighbours: ||p_i - p_j|| < comm_radius, j != i (double_integrator.py:227-232).
-    // sqrtf(acc) < Rc  <=>  acc < comm_sq_thr (smallest fp32 whose correctly rounded sqrt is >= Rc; host-computed),
-    // so the scan needs no sqrt; the ballots are kept in shared memory for the fill pass.
+    // ---------------- active hit nodes and neighbours; the ballots are kept in shared memory for the fill pass
+    const unsigned hit_bits = active_hit_bits<PD>(d, p, my_hits, lane, valid);
     int cnt = 0;
     unsigned* my_bits = sbits + warp * n_words;
-    if (valid) {   // warp-uniform.  40 % of the kernel's instructions were in this scan: full 32-candidate words run
-                   // without the per-lane range / self tests (the self bit is cleared after the ballot), unrolled x4
-        const int n_full = N >> 5;
-#pragma unroll 4
-        for (int w = 0; w < n_full; ++w) {
-            const int j = (w << 5) + lane;
-            float acc;
-            if (PD == 2) {
-                const float2 q = *reinterpret_cast<const float2*>(spos + j * 2);
-                const float dx = p[0] - q.x, dy = p[1] - q.y;
-                acc = dx * dx;
-                acc = acc + dy * dy;
-            } else {
-                acc = 0.f;
-#pragma unroll
-                for (int c = 0; c < PD; ++c) {
-                    const float dlt = p[c] - spos[j * PD + c];
-                    acc = (c == 0) ? dlt * dlt : acc + dlt * dlt;
-                }
-            }
-            unsigned bits = __ballot_sync(0xffffffffu, acc < d.comm_sq_thr);
-            if (w == (i >> 5)) bits &= ~(1u << (i & 31));
-            if (lane == 0) my_bits[w] = bits;
-            cnt += __popc(bits);
-        }
-        if (N & 31) {
-            const int j = (n_full << 5) + lane;
-            bool ok = false;
-            if (j < N && j != i) {
-                float acc = 0.f;
-#pragma unroll
-                for (int c = 0; c < PD; ++c) {
-                    const float dlt = p[c] - spos[j * PD + c];
-                    acc = (c == 0) ? dlt * dlt : acc + dlt * dlt;
-                }
-                ok = acc < d.comm_sq_thr;
-            }
-            const unsigned bits = __ballot_sync(0xffffffffu, ok);
-            if (lane == 0) my_bits[n_full] = bits;
-            cnt += __popc(bits);
-        }
-    }
+    if (valid) cnt = neighbour_bits<PD, PD>(d, p, i, spos, lane, my_bits);
     const int deg = valid ? (1 + cnt + __popc(hit_bits)) : 0;
     if (lane == 0) s_off[warp + 1] = deg;
     __syncthreads();
@@ -415,27 +264,8 @@ graph_build_kernel(const gcbf_env_desc d, const float* __restrict__ agent, const
         if (lane == 0) {
             row_start[a_id] = base;
             row_deg[a_id] = deg;
-            edge_recv[base] = a_id;
-            edge_src[base] = -1;
         }
-        int pos = base + 1;
-        const unsigned lt = (1u << lane) - 1u;
-        __syncwarp();
-        for (int w = 0; w < n_words; ++w) {
-            const unsigned bits = my_bits[w];
-            if (bits == 0u) continue;            // warp-uniform: most words of a sparse neighbourhood are empty
-            if ((bits >> lane) & 1u) {
-                const int e = pos + __popc(bits & lt);
-                edge_recv[e] = a_id;
-                edge_src[e] = g * N + (w << 5) + lane;
-            }
-            pos += __popc(bits);
-        }
-        if ((hit_bits >> lane) & 1u) {
-            const int e = pos + __popc(hit_bits & lt);
-            edge_recv[e] = a_id;
-            edge_src[e] = -2 - lane;
-        }
+        fill_row(edge_recv, edge_src, base, a_id, g * N, my_bits, n_words, hit_bits, lane);
     }
     __syncthreads();   // s_off / s_base / the per-warp scratch are reused by the next round
     }
@@ -468,42 +298,25 @@ env_step_kernel(const gcbf_env_desc d, const float* __restrict__ agent, const fl
     float r_acc = 0.f, c_acc = 0.f, o_acc = 0.f;
     for (int i = threadIdx.x; i < N; i += blockDim.x) {
         const size_t a = (size_t)g * N + i;
-        float x[SD], gl[SD], ur[NU], act[NU], u[NU], xn[SD];
+        float x[SD], gl[SD], ur[NU], act[NU], xn[SD];
 #pragma unroll
         for (int c = 0; c < SD; ++c) {
             x[c] = agent[a * SD + c];
             gl[c] = goal[a * SD + c];
         }
         u_ref_dev<KIND>(d, x, gl, ur);
-        float sq = 0.f;
 #pragma unroll
         for (int c = 0; c < NU; ++c) {
             // mode 0: a = 2 pi + u_ref (gcbf_plus.py:182-186); 1 / 3: given action; 2: a = u_ref (test.py --u-ref)
             act[c] = (mode == 0) ? (2.f * pi[a * NU + c] + ur[c]) : ((mode == 1 || mode == 3) ? action[a * NU + c] : ur[c]);
-            u[c] = isnan(act[c]) ? act[c] : fminf(fmaxf(act[c], -d.u_lim), d.u_lim);  // clip_action
-            const float df = u[c] - ur[c];
-            sq = (c == 0) ? df * df : sq + df * df;
             if (mode == 0 || mode == 2) action[a * NU + c] = act[c];
         }
-        euler_dev<KIND>(d, x, gl, u, xn, mode != 3);   // mode 3: DubinsCar stop mask off
+        const float sq = step_agent<KIND>(d, x, gl, act, ur, mode != 3, xn);   // mode 3: DubinsCar stop mask off
 #pragma unroll
         for (int c = 0; c < SD; ++c) next_agent[a * SD + c] = xn[c];
         const float nr = sqrtf(sq);
         r_acc += nr * nr;  // (jnp.linalg.norm(...) ** 2)
-        // get_cost (double_integrator.py:183-198): any_j (2r > dist_ij), via the neighbour list
-        bool col = false;
-        const int rs = row_start[a], rd = row_deg[a];
-        for (int e = rs + 1; e < rs + rd; ++e) {
-            const int s = edge_src[e];
-            if (s < 0) break;
-            float acc = 0.f;
-#pragma unroll
-            for (int c = 0; c < PD; ++c) {
-                const float dlt = x[c] - agent[(size_t)s * SD + c];
-                acc = (c == 0) ? dlt * dlt : acc + dlt * dlt;
-            }
-            col = col || (d.two_r > sqrtf(acc));
-        }
+        const bool col = collides_prev<PD, SD>(x, row_start[a], row_deg[a], edge_src, agent, d.two_r);
         c_acc += col ? 1.f : 0.f;
         o_acc += (O > 0 && inside_any<PD>(sobs, O, x, d.radius)) ? 1.f : 0.f;
     }

@@ -1,6 +1,9 @@
-// geometry_dev.cuh -- device functions shared by geometry.cu and rollout_persist.cu: obstacle primitives
-// (Rectangle / Sphere inside + ray cast), the stable 32-key warp sort of the LiDAR returns, u_ref and the Euler step.
-// Both translation units are compiled with -fmad=false: every arithmetic step keeps the reference's
+// geometry_dev.cuh -- device functions shared by geometry.cu, rollout_persist.cu and train.cu: obstacle primitives
+// (Rectangle / Sphere inside + ray cast), the stable 32-key warp sort of the LiDAR returns, u_ref, the Euler step,
+// the policy tail and reward / cost terms of an env step, and the per-warp pieces of the graph build (2-D LiDAR,
+// active hits, neighbour scan, edge-row fill).  The 5-launch rollout step and the persistent rollout kernel run these
+// same functions, which is what keeps the two paths bit-identical.
+// Every including unit is compiled with -fmad=false: every arithmetic step keeps the reference's
 // one-rounding-per-op semantics (bit-exact index sets / hit ordering / masks against the CPU oracle).
 //
 // Replaces (reference paths): gcbfplus/env/obstacle.py:53-96 (Rectangle), :234-270 (Sphere), env/utils.py:82-131,
@@ -231,6 +234,247 @@ __device__ __forceinline__ void euler_dev(const gcbf_env_desc& d, const float* x
                              (KIND == GCBF_ENV_LINEAR_DRONE && c >= 3);
         if (limited) v = isnan(v) ? v : fminf(fmaxf(v, -d.v_lim), d.v_lim);
         xn[c] = v;
+    }
+}
+
+// u = clip_action(act), x' = agent_step_euler(x, u); returns ||u - u_ref||^2, the control term of the reward
+// (double_integrator.py:145-198)
+template <int KIND>
+__device__ __forceinline__ float step_agent(const gcbf_env_desc& d, const float* x, const float* gl, const float* act,
+                                            const float* ur, const bool stop_mask, float* xn) {
+    constexpr int NU = EnvTraits<KIND>::NU;
+    float u[NU], sq = 0.f;
+#pragma unroll
+    for (int c = 0; c < NU; ++c) {
+        u[c] = isnan(act[c]) ? act[c] : fminf(fmaxf(act[c], -d.u_lim), d.u_lim);
+        const float df = u[c] - ur[c];
+        sq = (c == 0) ? df * df : sq + df * df;
+    }
+    euler_dev<KIND>(d, x, gl, u, xn, stop_mask);
+    return sq;
+}
+
+// policy tail of a rollout step: pi = tanh(z + bHO) (policy.py:72), a = 2 pi + u_ref (gcbf_plus.py:182-186)
+template <int KIND>
+__device__ __forceinline__ void policy_action(const gcbf_env_desc& d, const float* x, const float* gl, const float* z,
+                                              const float* bHO, float* ur, float* act) {
+    u_ref_dev<KIND>(d, x, gl, ur);
+#pragma unroll
+    for (int c = 0; c < EnvTraits<KIND>::NU; ++c) act[c] = 2.f * tanhf(z[c] + bHO[c]) + ur[c];
+}
+
+// get_cost's agent term (double_integrator.py:183-198): any neighbour j of the previous graph with 2r > ||x - x_j||.
+// edge_src holds the agent's edge row [rs, rs + rd): self / goal edge first, then agent senders, then hit codes (< 0).
+template <int PD, int SD>
+__device__ __forceinline__ bool collides_prev(const float* x, int rs, int rd, const int32_t* edge_src,
+                                              const float* agent_prev, float two_r) {
+    bool col = false;
+    for (int e = rs + 1; e < rs + rd; ++e) {
+        const int s = edge_src[e];
+        if (s < 0) break;
+        float dd = 0.f;
+#pragma unroll
+        for (int c = 0; c < PD; ++c) {
+            const float dlt = x[c] - agent_prev[(size_t)s * SD + c];
+            dd = (c == 0) ? dlt * dlt : dd + dlt * dlt;
+        }
+        col = col || (two_r > sqrtf(dd));
+    }
+    return col;
+}
+
+// Reward and cost of one graph from per-thread sums acc = [sum ||u - u_ref||^2, #colliding, #inside an obstacle]:
+// warp sums, then thread 0 adds the NW warp sums in warp order.  Warps without agents add +0, so CTAs of different
+// widths give the same bits.  Every thread of the CTA calls it.
+template <int NW>
+__device__ __forceinline__ void reduce_reward_cost(const float* acc, float* s_red, int N, float* reward, float* cost) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+    for (int q = 0; q < 3; ++q) {
+        const float v = warp_sum(acc[q]);
+        if (lane == 0) s_red[q * NW + warp] = v;
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        float t[3] = {0.f, 0.f, 0.f};
+        for (int w = 0; w < NW; ++w) {
+            t[0] += s_red[0 * NW + w];
+            t[1] += s_red[1 * NW + w];
+            t[2] += s_red[2 * NW + w];
+        }
+        *reward = -(t[0] / (float)N);
+        *cost = t[1] / (float)N + t[2] / (float)N;
+    }
+}
+
+// ------------------------------------------------------------------------------------
+// graph build of one agent per warp (graph_build_kernel and the persistent rollout kernel)
+// ------------------------------------------------------------------------------------
+// 2-D obstacle rows in shared memory are 24 floats: the packed rectangle, then the derived fields of the far-obstacle
+// skip at [14] reach^2, [15..18] edge dx, [19..22] edge dy.
+constexpr int OBS2D = 24;
+__device__ __forceinline__ void derive_far_fields(float* sobs, int O, float comm_radius, int tid, int nthreads) {
+    for (int o = tid; o < O; o += nthreads) {
+        float* ob = sobs + OBS2D * o;
+        const float reach = comm_radius + sqrtf(ob[2] * ob[2] + ob[3] * ob[3]) + 2e-3f;
+        ob[14] = reach * reach;
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            const int kp = (k + 3) & 3;
+            ob[15 + k] = ob[6 + 2 * kp] - ob[6 + 2 * k];   // x4 - x3
+            ob[19 + k] = ob[7 + 2 * kp] - ob[7 + 2 * k];   // y4 - y3
+        }
+    }
+}
+
+// 2-D LiDAR (env/utils.py:49-131) of the agent at p, one ray per lane: the R closest returns in stable argsort order
+// -> my_hits[R][2].  sobs: O obstacle rows of OBS2D floats (derive_far_fields), stab: [n_rays][2] ray offsets.
+__device__ __forceinline__ void lidar2d_warp(const float* p, const float* stab, const float* sobs, int O, int n_rays,
+                                             int R, int lane, float* my_hits) {
+    const bool ray_ok = lane < n_rays;
+    const int rl = ray_ok ? lane : 0;
+    const float x1 = p[0], y1 = p[1];
+    const float x2 = x1 + stab[rl * 2 + 0], y2 = y1 + stab[rl * 2 + 1];
+    const float rdx = x1 - x2, rdy = y1 - y2;
+    float alpha;
+    if (O == 0) {
+        alpha = 1.f * NO_HIT;
+    } else {
+        // A rectangle whose bounding circle is out of the ray's reach cannot be hit or contain the agent:
+        // every edge test gives valid = 0 and alpha = 0 * alpha + 1e6 = 1e6 exactly -- unless an edge is
+        // exactly parallel to the ray (det == 0 -> alpha = x/0 -> NaN in the reference, obstacle.py:88-94).
+        // The skip is taken only when it is bit-identical to the full evaluation (agent-uniform branch).
+        alpha = NO_HIT;
+        bool is_in = false;
+        for (int o = 0; o < O; ++o) {
+            const float* ob = sobs + OBS2D * o;
+            const float cx = x1 - ob[0], cy = y1 - ob[1];
+            const bool far = (cx * cx + cy * cy) > ob[14];
+            bool degenerate = false;
+            if (far) {
+#pragma unroll
+                for (int k = 0; k < 4; ++k) {
+                    const float det = rdx * ob[19 + k] - rdy * ob[15 + k];
+                    degenerate = degenerate || !(det != 0.f);   // det == 0 or NaN
+                }
+            }
+            if (!far) is_in = is_in || rect_inside(ob, x1, y1, 0.f);
+            if (!far || __any_sync(0xffffffffu, degenerate))
+                alpha = nanmin(alpha, rect_raytrace(ob, x1, y1, x2, y2));
+        }
+        alpha = alpha * (1.f - (is_in ? 1.f : 0.f));
+    }
+    const float hx = x1 + (x2 - x1) * alpha;
+    const float hy = y1 + (y2 - y1) * alpha;
+    SortKey k;
+    k.flag = ray_ok ? (isnan(alpha) ? 1 : 0) : 2;
+    k.alpha = alpha;
+    k.idx = lane;
+    // argsort is stable: when no ray of this agent hit anything (every alpha == 1e6) the order is the
+    // identity and the 15-stage warp sort can be skipped (warp-uniform, the common case in open space)
+    const bool all_miss = __all_sync(0xffffffffu, !ray_ok || alpha == NO_HIT);
+    if (!all_miss) k = warp_sort32(k, lane);
+    const float shx = __shfl_sync(0xffffffffu, hx, k.idx);
+    const float shy = __shfl_sync(0xffffffffu, hy, k.idx);
+    if (lane < R) {
+        my_hits[lane * 2 + 0] = shx;
+        my_hits[lane * 2 + 1] = shy;
+    }
+}
+
+// active hit nodes: ||p - hit|| < comm_radius - 0.1 (double_integrator.py:254-257); bit r = hit r (ballot, lane r)
+template <int PD>
+__device__ __forceinline__ unsigned active_hit_bits(const gcbf_env_desc& d, const float* p, const float* my_hits, int lane,
+                                                    bool valid) {
+    bool act = false;
+    if (valid && lane < d.n_hits) {
+        float acc = 0.f;
+#pragma unroll
+        for (int c = 0; c < PD; ++c) {
+            const float dlt = p[c] - my_hits[lane * PD + c];
+            acc = (c == 0) ? dlt * dlt : acc + dlt * dlt;
+        }
+        act = acc < d.lidar_sq_thr;   // == (sqrtf(acc) < lidar_radius), threshold precomputed exactly on the host
+    }
+    return __ballot_sync(0xffffffffu, act);
+}
+
+// neighbours of agent i: ||p_i - p_j|| < comm_radius, j != i (double_integrator.py:227-232), j's position at
+// pos + j * STRIDE.  sqrtf(acc) < Rc  <=>  acc < d.comm_sq_thr (smallest fp32 whose correctly rounded sqrt is >= Rc;
+// host-computed), so the scan needs no sqrt.  Writes one ballot word per 32 candidates to my_bits (lane 0) and
+// returns the neighbour count.  Full words run without the per-lane range / self tests (the self bit is cleared after
+// the ballot), unrolled x4: this scan was 40 % of graph_build_kernel's instructions.
+template <int PD, int STRIDE>
+__device__ __forceinline__ int neighbour_bits(const gcbf_env_desc& d, const float* p, int i, const float* pos, int lane,
+                                              unsigned* my_bits) {
+    const int N = d.n_agents;
+    int cnt = 0;
+    const int n_full = N >> 5;
+#pragma unroll 4
+    for (int w = 0; w < n_full; ++w) {
+        const int j = (w << 5) + lane;
+        float acc;
+        if (PD == 2) {
+            const float2 q = *reinterpret_cast<const float2*>(pos + j * STRIDE);
+            const float dx = p[0] - q.x, dy = p[1] - q.y;
+            acc = dx * dx;
+            acc = acc + dy * dy;
+        } else {
+            acc = 0.f;
+#pragma unroll
+            for (int c = 0; c < PD; ++c) {
+                const float dlt = p[c] - pos[j * STRIDE + c];
+                acc = (c == 0) ? dlt * dlt : acc + dlt * dlt;
+            }
+        }
+        unsigned bits = __ballot_sync(0xffffffffu, acc < d.comm_sq_thr);
+        if (w == (i >> 5)) bits &= ~(1u << (i & 31));
+        if (lane == 0) my_bits[w] = bits;
+        cnt += __popc(bits);
+    }
+    if (N & 31) {
+        const int j = (n_full << 5) + lane;
+        bool ok = false;
+        if (j < N && j != i) {
+            float acc = 0.f;
+#pragma unroll
+            for (int c = 0; c < PD; ++c) {
+                const float dlt = p[c] - pos[j * STRIDE + c];
+                acc = (c == 0) ? dlt * dlt : acc + dlt * dlt;
+            }
+            ok = acc < d.comm_sq_thr;
+        }
+        const unsigned bits = __ballot_sync(0xffffffffu, ok);
+        if (lane == 0) my_bits[n_full] = bits;
+        cnt += __popc(bits);
+    }
+    return cnt;
+}
+
+// Edge row of receiver a_id at rbase: [goal | agents ascending | active hits ascending] (edge codes: gcbf_b200.h).
+// Agent j of the graph is sender sender0 + j.
+__device__ __forceinline__ void fill_row(int32_t* er, int32_t* es, int rbase, int a_id, int sender0,
+                                         const unsigned* my_bits, int n_words, unsigned hit_bits, int lane) {
+    if (lane == 0) {
+        er[rbase] = a_id;
+        es[rbase] = -1;
+    }
+    int pos = rbase + 1;
+    const unsigned lt = (1u << lane) - 1u;
+    for (int w = 0; w < n_words; ++w) {
+        const unsigned bits = my_bits[w];
+        if (bits == 0u) continue;            // warp-uniform: most words of a sparse neighbourhood are empty
+        if ((bits >> lane) & 1u) {
+            const int e = pos + __popc(bits & lt);
+            er[e] = a_id;
+            es[e] = sender0 + (w << 5) + lane;
+        }
+        pos += __popc(bits);
+    }
+    if ((hit_bits >> lane) & 1u) {
+        const int e = pos + __popc(hit_bits & lt);
+        er[e] = a_id;
+        es[e] = -2 - lane;
     }
 }
 

@@ -177,6 +177,57 @@ edge_l1_kernel(const gcbf_env_desc d, const float* __restrict__ W1, const float*
     }
 }
 
+// ---- segment softmax of given gate logits + weighted aggregation (gnn.py:64-72) for one receiver, one warp: the
+// receiver's edge rows are [rs, rs + rd) of ATT (logits) and MSG ([.][128] messages); returns this lane's 4 columns
+// of AG.  Shared by attn_aggregate_kernel (inference) and the persistent rollout kernel.
+__device__ __forceinline__ float4 aggregate_logits(int rs, int rd, const float* ATT, const float* MSG, int lane) {
+    float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (rd <= 4) {
+        // fast path (typical degree: goal + 0..3 neighbours / hits): every logit and message row is requested before
+        // anything is consumed, so the warp waits for ONE round trip to L2 instead of three
+        float lg[4];
+        float4 mv[4];
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+            const int e = rs + min(q, max(rd - 1, 0));
+            lg[q] = (q < rd) ? ATT[e] : -INFINITY;
+            mv[q] = (q < rd) ? *reinterpret_cast<const float4*>(MSG + (size_t)e * 128 + lane * 4)
+                             : make_float4(0.f, 0.f, 0.f, 0.f);
+        }
+        float mx = -INFINITY;
+#pragma unroll
+        for (int q = 0; q < 4; ++q) mx = fmaxf(mx, lg[q]);      // same left-to-right order as the general path
+        float den = 0.f;
+#pragma unroll
+        for (int q = 0; q < 4; ++q)
+            if (q < rd) den += expf(lg[q] - mx);
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+            if (q < rd) {
+                const float att = expf(lg[q] - mx) / den;
+                acc.x = fmaf(att, mv[q].x, acc.x);
+                acc.y = fmaf(att, mv[q].y, acc.y);
+                acc.z = fmaf(att, mv[q].z, acc.z);
+                acc.w = fmaf(att, mv[q].w, acc.w);
+            }
+        }
+        return acc;
+    }
+    float mx = -INFINITY;
+    for (int e = rs; e < rs + rd; ++e) mx = fmaxf(mx, ATT[e]);
+    float den = 0.f;
+    for (int e = rs; e < rs + rd; ++e) den += expf(ATT[e] - mx);
+    for (int e = rs; e < rs + rd; ++e) {
+        const float att = expf(ATT[e] - mx) / den;
+        const float4 m = *reinterpret_cast<const float4*>(MSG + (size_t)e * 128 + lane * 4);
+        acc.x = fmaf(att, m.x, acc.x);
+        acc.y = fmaf(att, m.y, acc.y);
+        acc.z = fmaf(att, m.z, acc.z);
+        acc.w = fmaf(att, m.w, acc.w);
+    }
+    return acc;
+}
+
 // ---- gate logit + segment softmax + weighted aggregation (gnn.py:64-72); warp per receiver.
 // gate = G2 @ a3 + ba3 ; att = softmax over the receiver's edges ; AG[a] = sum att * MSG.
 static __global__ void __launch_bounds__(256)
@@ -184,7 +235,9 @@ attn_aggregate_kernel(const int A, const int edge_cap, const float* __restrict__
                       const float* __restrict__ a3, const float* __restrict__ ba3,
                       const int32_t* __restrict__ row_start, const int32_t* __restrict__ row_deg,
                       float* __restrict__ ATT, float* __restrict__ AG, int32_t* __restrict__ zero_counter = nullptr) {
-    // G2 == nullptr: ATT already holds the gate logits (written by the EPI_RELU_DOT GEMM epilogue)
+    // G2 == nullptr (inference): ATT already holds the gate logits (written by the EPI_RELU_DOT GEMM epilogue) and is
+    // left as it is.  Otherwise (training) the gate logits are computed here and ATT receives the attention weights
+    // that the backward pass reads.
     // zero_counter (rollout step): edge counter of the NEXT graph, cleared here so that no memset node sits in the
     // per-step kernel chain (the graph build two kernels later accumulates into it)
     if (zero_counter && blockIdx.x == 0 && threadIdx.x == 0) zero_counter[0] = 0;
@@ -196,40 +249,11 @@ attn_aggregate_kernel(const int A, const int edge_cap, const float* __restrict__
         const int rs = row_start[a];
         int rd = row_deg[a];
         if (rs < 0 || rs + rd > edge_cap) rd = 0;
-        if (!G2 && rd <= 4) {
-            // inference fast path (typical degree: goal + 0..3 neighbours / hits): every logit and message row is
-            // requested before anything is consumed, so the warp waits for ONE round trip to L2 instead of three
-            float lg[4];
-            float4 mv[4];
-#pragma unroll
-            for (int q = 0; q < 4; ++q) {
-                const int e = rs + min(q, max(rd - 1, 0));
-                lg[q] = (q < rd) ? ATT[e] : -INFINITY;
-                mv[q] = (q < rd) ? *reinterpret_cast<const float4*>(MSG + (size_t)e * 128 + lane * 4)
-                                 : make_float4(0.f, 0.f, 0.f, 0.f);
-            }
-            float mx = -INFINITY;
-#pragma unroll
-            for (int q = 0; q < 4; ++q) mx = fmaxf(mx, lg[q]);      // same left-to-right order as the general path
-            float den = 0.f;
-#pragma unroll
-            for (int q = 0; q < 4; ++q)
-                if (q < rd) den += expf(lg[q] - mx);
-            float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-            for (int q = 0; q < 4; ++q) {
-                if (q < rd) {
-                    const float att = expf(lg[q] - mx) / den;
-                    acc.x = fmaf(att, mv[q].x, acc.x);
-                    acc.y = fmaf(att, mv[q].y, acc.y);
-                    acc.z = fmaf(att, mv[q].z, acc.z);
-                    acc.w = fmaf(att, mv[q].w, acc.w);
-                }
-            }
-            *reinterpret_cast<float4*>(AG + (size_t)a * 128 + lane * 4) = acc;
+        if (!G2) {
+            *reinterpret_cast<float4*>(AG + (size_t)a * 128 + lane * 4) = aggregate_logits(rs, rd, ATT, MSG, lane);
             continue;
         }
-        if (G2 && rd <= 4) {
+        if (rd <= 4) {
             // training fast path: the gate rows and the message rows of all (<= 4) edges are requested up front and the
             // 4 dot products are reduced together; same arithmetic order as the general path below
             float sg[4];
@@ -274,18 +298,14 @@ attn_aggregate_kernel(const int A, const int edge_cap, const float* __restrict__
             continue;
         }
         float mx = -INFINITY;
-        if (G2) {
-            for (int e = rs; e < rs + rd; ++e) {
-                const float4 g = *reinterpret_cast<const float4*>(G2 + (size_t)e * 128 + lane * 4);
-                float s = g.x * w.x + g.y * w.y + g.z * w.z + g.w * w.w;
-                s = warp_sum(s) + bias;
-                if (lane == 0) ATT[e] = s;
-                mx = fmaxf(mx, s);
-            }
-            __syncwarp();
-        } else {
-            for (int e = rs; e < rs + rd; ++e) mx = fmaxf(mx, ATT[e]);
+        for (int e = rs; e < rs + rd; ++e) {
+            const float4 g = *reinterpret_cast<const float4*>(G2 + (size_t)e * 128 + lane * 4);
+            float s = g.x * w.x + g.y * w.y + g.z * w.z + g.w * w.w;
+            s = warp_sum(s) + bias;
+            if (lane == 0) ATT[e] = s;
+            mx = fmaxf(mx, s);
         }
+        __syncwarp();
         float den = 0.f;
         for (int e = rs; e < rs + rd; ++e) den += expf(ATT[e] - mx);
         float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);

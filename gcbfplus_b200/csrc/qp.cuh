@@ -1,5 +1,5 @@
 // qp.cuh -- CBF-QP action labels u_qp (gcbfplus/algo/gcbf_plus.py:299-352 get_qp_action, :193-211 get_b_u_qp).
-// Included by train.cu (uses its u_ref_train and the data-only mode of gnn_backward_impl).
+// Included by train.cu (uses u_ref_dev of geometry_dev.cuh and the data-only mode of gnn_backward_impl).
 //
 // Per graph with N agents, x = [u | r]:
 //     min 1/2 |u|^2 - u_ref.u + 5 |r|^2 + 1000 sum r   s.t.  -Lg_h u - r <= Lf_h + 0.1 alpha h,  |u| <= u_lim,  r >= 0
@@ -89,7 +89,7 @@ qp_assemble_kernel(const gcbf_env_desc d, const float alpha, const float* __rest
     float lf, lg[NU], ur[NU];
     qp_lie_terms<KIND>(d, xi, ci, &lf, lg);
     lf_sum += lf;
-    u_ref_train<KIND>(d, xi, gl, ur);
+    u_ref_dev<KIND>(d, xi, gl, ur);
 #pragma unroll
     for (int c = 0; c < NU; ++c) {
         QS[(size_t)i * 4 + c] = lg[c];

@@ -10,14 +10,16 @@
 // Per env-step (cluster of C CTAs, 512 threads each; per-env receiver-ordered edge lists):
 //   E   edge tiles of 128 edges -> CTA (tile % C): edge features + message layer 1 produced in-CTA -> folded message
 //       GEMM 256->128 (wgmma 3xTF32, register accumulator) -> chained gate GEMM 128->128 -> logits         [gemm_tc_prod.cuh]
-//   A   warp per receiver: segment softmax + weighted aggregate                                             [gnn.cuh attn_aggregate_kernel]
+//   A   warp per receiver: segment softmax + weighted aggregate                                             [gnn.cuh aggregate_logits]
 //   U1  (agent tile, column half) items: update layer 128->256, bias + one-hot row, ReLU                   [gemm_tc.cuh EPI_BIAS_RELU]
 //   U2  same items: folded update/head layer 256->256, ReLU, output-layer partial sums                      [gemm_tc.cuh EPI_RELU_DOTN]
 //   G   policy tail (tanh, a = 2 pi + u_ref, clip, Euler; record action / next state / reward / cost) + LiDAR +
 //       stable top-k + radius neighbour lists of the next state, rows laid out in agent order through a
-//       CTA-local prefix sum and a cluster-wide exchange of the CTA totals over distributed shared memory    [geometry.cu graph_build_kernel]
-// Every arithmetic step is the one the 5-launch path performs (same operand split, same MMA order, same epilogues,
-// same reduction orders), so the two paths give the same bits (tests/test_gpu_rollout.py).  This translation unit is
+//       CTA-local prefix sum and a cluster-wide exchange of the CTA totals over distributed shared memory    [geometry_dev.cuh]
+// The phases call the device functions the 5-launch kernels call (GEMM main loops and epilogues; aggregate; policy
+// tail, LiDAR, neighbour scan and row fill), so the two paths give the same bits (tests/test_gpu_rollout.py).  What
+// differs stays here: the edge-row limit of a local group, the row base from the prefix over the cluster, and that
+// only the environment's first CTA records.  This translation unit is
 // compiled with -fmad=false like geometry.cu (the LiDAR / dynamics code must keep one rounding per operation); the
 // GEMM-side code uses explicit fmaf wherever the other translation units rely on contraction.
 //
@@ -82,7 +84,6 @@ struct PArgs {
     // (arrival counter in global memory) once per step.
     int soft;                                            // 0 / 1 = mode
     unsigned* gbar;                                      // [E] arrival counters of the environment barrier (zeroed by the launcher)
-    int* gtot;                                           // [E][8] (unused since the pair mode; kept for the layout)
 };
 
 __device__ __forceinline__ unsigned long long gtime() {
@@ -124,7 +125,7 @@ rollout_persist_kernel(const __grid_constant__ PArgs P, const __grid_constant__ 
     using TR = EnvTraits<KIND>;
     constexpr int SD = TR::SD, ED = TR::ED, NU = TR::NU, PD = TR::PD;
     static_assert(PD == 2 && NU == PNU, "persistent rollout kernel: 2-D environments");
-    constexpr int OBW = 16, OBS2 = 24;
+    constexpr int OBW = 16, OBS2 = OBS2D;
     constexpr int A_BYTES = 16384, B_BYTES = 16384;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = smem_align1024(smem_raw);
@@ -143,9 +144,6 @@ rollout_persist_kernel(const __grid_constant__ PArgs P, const __grid_constant__ 
     const gcbf_env_desc& d = P.d;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int C = P.C;
-    uint32_t rank_u;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(rank_u));
-    (void)rank_u;
     const bool soft = P.soft != 0;
     const int rank = (int)(blockIdx.x % C);          // CTA inside the environment
     const int env = blockIdx.x / C;
@@ -214,17 +212,7 @@ rollout_persist_kernel(const __grid_constant__ PArgs P, const __grid_constant__ 
     }
     for (int i = tid; i < d.n_rays * PD; i += PT) stab[i] = P.ray_table[i];
     __syncthreads();
-    for (int o = tid; o < O; o += PT) {
-        float* ob = sobs + OBS2 * o;
-        const float reach = d.comm_radius + sqrtf(ob[2] * ob[2] + ob[3] * ob[3]) + 2e-3f;
-        ob[14] = reach * reach;
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-            const int kp = (k + 3) & 3;
-            ob[15 + k] = ob[6 + 2 * kp] - ob[6 + 2 * k];
-            ob[19 + k] = ob[7 + 2 * kp] - ob[7 + 2 * k];
-        }
-    }
+    derive_far_fields(sobs, O, d.comm_radius, tid, PT);
     uint32_t it = 0;      // k-blocks pushed through the 3-stage ring so far (all roles advance it identically)
     uint32_t ne = 0;      // edge tiles this CTA has processed (chain barriers)
     int M_cur = 0;        // edge rows of my local group's segment in the current graph
@@ -340,51 +328,8 @@ rollout_persist_kernel(const __grid_constant__ PArgs P, const __grid_constant__ 
                 const int rs = rs_t[a];
                 int rd = rd_t[a];
                 if (rs < 0 || rs + rd > cap) rd = 0;
-                const float* ATT = P.logit + env_e0;
-                const float* MSG = P.msg + env_e0 * 128;
-                float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
-                if (rd <= 4) {
-                    float lg[4];
-                    float4 mv[4];
-#pragma unroll
-                    for (int q = 0; q < 4; ++q) {
-                        const int e = rs + min(q, max(rd - 1, 0));
-                        lg[q] = (q < rd) ? ATT[e] : -INFINITY;
-                        mv[q] = (q < rd) ? *reinterpret_cast<const float4*>(MSG + (size_t)e * 128 + lane * 4)
-                                         : make_float4(0.f, 0.f, 0.f, 0.f);
-                    }
-                    float mx = -INFINITY;
-#pragma unroll
-                    for (int q = 0; q < 4; ++q) mx = fmaxf(mx, lg[q]);
-                    float den = 0.f;
-#pragma unroll
-                    for (int q = 0; q < 4; ++q)
-                        if (q < rd) den += expf(lg[q] - mx);
-#pragma unroll
-                    for (int q = 0; q < 4; ++q) {
-                        if (q < rd) {
-                            const float att = expf(lg[q] - mx) / den;
-                            acc.x = fmaf(att, mv[q].x, acc.x);
-                            acc.y = fmaf(att, mv[q].y, acc.y);
-                            acc.z = fmaf(att, mv[q].z, acc.z);
-                            acc.w = fmaf(att, mv[q].w, acc.w);
-                        }
-                    }
-                } else {
-                    float mx = -INFINITY;
-                    for (int e = rs; e < rs + rd; ++e) mx = fmaxf(mx, ATT[e]);
-                    float den = 0.f;
-                    for (int e = rs; e < rs + rd; ++e) den += expf(ATT[e] - mx);
-                    for (int e = rs; e < rs + rd; ++e) {
-                        const float att = expf(ATT[e] - mx) / den;
-                        const float4 m = *reinterpret_cast<const float4*>(MSG + (size_t)e * 128 + lane * 4);
-                        acc.x = fmaf(att, m.x, acc.x);
-                        acc.y = fmaf(att, m.y, acc.y);
-                        acc.z = fmaf(att, m.z, acc.z);
-                        acc.w = fmaf(att, m.w, acc.w);
-                    }
-                }
-                *reinterpret_cast<float4*>(P.ag + (size_t)a * 128 + lane * 4) = acc;
+                *reinterpret_cast<float4*>(P.ag + (size_t)a * 128 + lane * 4) =
+                    aggregate_logits(rs, rd, P.logit + env_e0, P.msg + env_e0 * 128, lane);
             }
             fence_async_global();          // generic-proxy writes of AG -> TMA (async proxy) reads in phase U1
             SYNC_LOCAL();
@@ -492,42 +437,24 @@ rollout_persist_kernel(const __grid_constant__ PArgs P, const __grid_constant__ 
                         const float4 v = *reinterpret_cast<const float4*>(z_t + ((size_t)p * A_tot + a) * 4);
                         zz[0] += v.x; zz[1] += v.y; zz[2] += v.z; zz[3] += v.w;
                     }
-                    float x[SD], gl[SD], ur[NU], u[NU], xn[SD];
+                    float x[SD], gl[SD], ur[NU], act[NU], xn[SD];
 #pragma unroll
                     for (int c = 0; c < SD; ++c) {
                         x[c] = sst[i * SD + c];              // state t (== agent_t[a], this CTA's copy)
                         gl[c] = P.goal[a * SD + c];
                     }
-                    u_ref_dev<KIND>(d, x, gl, ur);
-                    float sq = 0.f;
+                    policy_action<KIND>(d, x, gl, zz, sk + K_BHO, ur, act);
+                    if (rec)
 #pragma unroll
-                    for (int c = 0; c < NU; ++c) {
-                        const float act = 2.f * tanhf(zz[c] + sk[K_BHO + c]) + ur[c];
-                        if (rec) act_t[a * NU + c] = act;
-                        u[c] = isnan(act) ? act : fminf(fmaxf(act, -d.u_lim), d.u_lim);
-                        const float df = u[c] - ur[c];
-                        sq = (c == 0) ? df * df : sq + df * df;
-                    }
-                    euler_dev<KIND>(d, x, gl, u, xn);
+                        for (int c = 0; c < NU; ++c) act_t[a * NU + c] = act[c];
+                    const float sq = step_agent<KIND>(d, x, gl, act, ur, true, xn);
 #pragma unroll
                     for (int c = 0; c < SD; ++c) sst[i * SD + c] = xn[c];
                     if (rec) {
 #pragma unroll
                         for (int c = 0; c < SD; ++c) agent_n[a * SD + c] = xn[c];
                         const float nr = sqrtf(sq);
-                        bool col = false;
-                        const int rs = rs_t[a], rd = rd_t[a];
-                        for (int e = rs + 1; e < rs + rd; ++e) {
-                            const int sidx = es_t[env_e0 + e];
-                            if (sidx < 0) break;
-                            float dd = 0.f;
-#pragma unroll
-                            for (int c = 0; c < PD; ++c) {
-                                const float dlt = x[c] - agent_t[(size_t)sidx * SD + c];
-                                dd = (c == 0) ? dlt * dlt : dd + dlt * dlt;
-                            }
-                            col = col || (d.two_r > sqrtf(dd));
-                        }
+                        const bool col = collides_prev<PD, SD>(x, rs_t[a], rd_t[a], es_t + env_e0, agent_t, d.two_r);
                         bool in_obs = false;
                         if (O > 0) {
                             const float* ob = P.obstacles + (d.obs_per_graph ? (size_t)env * O * OBW : 0);
@@ -538,24 +465,7 @@ rollout_persist_kernel(const __grid_constant__ PArgs P, const __grid_constant__ 
                         acc[2] += in_obs ? 1.f : 0.f;
                     }
                 }
-                if (rec) {
-#pragma unroll
-                    for (int q = 0; q < 3; ++q) {
-                        const float v = warp_sum(acc[q]);
-                        if (lane == 0) s_red[q * PW + warp] = v;
-                    }
-                    __syncthreads();
-                    if (tid == 0) {
-                        float s3[3] = {0.f, 0.f, 0.f};
-                        for (int w = 0; w < PW; ++w) {
-                            s3[0] += s_red[0 * PW + w];
-                            s3[1] += s_red[1 * PW + w];
-                            s3[2] += s_red[2 * PW + w];
-                        }
-                        P.rewards[(size_t)t * E + env] = -(s3[0] / (float)N);
-                        P.costs[(size_t)t * E + env] = s3[1] / (float)N + s3[2] / (float)N;
-                    }
-                }
+                if (rec) reduce_reward_cost<PW>(acc, s_red, N, P.rewards + (size_t)t * E + env, P.costs + (size_t)t * E + env);
             }
             __syncthreads();
             if (stamp) pr[5] = gtime();
@@ -572,99 +482,11 @@ rollout_persist_kernel(const __grid_constant__ PArgs P, const __grid_constant__ 
                 for (int c = 0; c < PD; ++c) p[c] = sst[ii * SD + c];
                 const size_t a_glob = (size_t)env_a0 + ii;
                 float* my_hits = hits_n + a_glob * R * PD;
-                if (valid) {
-                    const bool ray_ok = lane < d.n_rays;
-                    const int rl = ray_ok ? lane : 0;
-                    const float x1 = p[0], y1 = p[1];
-                    const float x2 = x1 + stab[rl * 2 + 0], y2 = y1 + stab[rl * 2 + 1];
-                    const float rdx = x1 - x2, rdy = y1 - y2;
-                    float alpha;
-                    if (O == 0) {
-                        alpha = 1.f * NO_HIT;
-                    } else {
-                        alpha = NO_HIT;
-                        bool is_in = false;
-                        for (int o = 0; o < O; ++o) {
-                            const float* ob = sobs + OBS2 * o;
-                            const float cx = x1 - ob[0], cy = y1 - ob[1];
-                            const bool far = (cx * cx + cy * cy) > ob[14];
-                            bool degenerate = false;
-                            if (far) {
-#pragma unroll
-                                for (int k = 0; k < 4; ++k) {
-                                    const float det = rdx * ob[19 + k] - rdy * ob[15 + k];
-                                    degenerate = degenerate || !(det != 0.f);
-                                }
-                            }
-                            if (!far) is_in = is_in || rect_inside(ob, x1, y1, 0.f);
-                            if (!far || __any_sync(0xffffffffu, degenerate))
-                                alpha = nanmin(alpha, rect_raytrace(ob, x1, y1, x2, y2));
-                        }
-                        alpha = alpha * (1.f - (is_in ? 1.f : 0.f));
-                    }
-                    const float hx = x1 + (x2 - x1) * alpha;
-                    const float hy = y1 + (y2 - y1) * alpha;
-                    SortKey k;
-                    k.flag = ray_ok ? (isnan(alpha) ? 1 : 0) : 2;
-                    k.alpha = alpha;
-                    k.idx = lane;
-                    const bool all_miss = __all_sync(0xffffffffu, !ray_ok || alpha == NO_HIT);
-                    if (!all_miss) k = warp_sort32(k, lane);
-                    const float shx = __shfl_sync(0xffffffffu, hx, k.idx);
-                    const float shy = __shfl_sync(0xffffffffu, hy, k.idx);
-                    if (lane < R) {
-                        my_hits[lane * 2 + 0] = shx;
-                        my_hits[lane * 2 + 1] = shy;
-                    }
-                }
+                if (valid) lidar2d_warp(p, stab, sobs, O, d.n_rays, R, lane, my_hits);
                 __syncwarp();
-                unsigned hit_bits = 0u;
-                {
-                    bool act = false;
-                    if (valid && lane < R) {
-                        float acc = 0.f;
-#pragma unroll
-                        for (int c = 0; c < PD; ++c) {
-                            const float dlt = p[c] - my_hits[lane * PD + c];
-                            acc = (c == 0) ? dlt * dlt : acc + dlt * dlt;
-                        }
-                        act = acc < d.lidar_sq_thr;
-                    }
-                    hit_bits = __ballot_sync(0xffffffffu, act);
-                }
+                const unsigned hit_bits = active_hit_bits<PD>(d, p, my_hits, lane, valid);
                 int cnt = 0;
-                if (valid) {
-                    unsigned* my_bits = sbits + slot * n_words;
-                    const int n_full = N >> 5;
-#pragma unroll 4
-                    for (int w = 0; w < n_full; ++w) {
-                        const int j = (w << 5) + lane;
-                        const float2 q = *reinterpret_cast<const float2*>(sst + j * SD);
-                        const float dx = p[0] - q.x, dy = p[1] - q.y;
-                        float acc = dx * dx;
-                        acc = acc + dy * dy;
-                        unsigned bits = __ballot_sync(0xffffffffu, acc < d.comm_sq_thr);
-                        if (w == (i >> 5)) bits &= ~(1u << (i & 31));
-                        if (lane == 0) my_bits[w] = bits;
-                        cnt += __popc(bits);
-                    }
-                    if (N & 31) {
-                        const int j = (n_full << 5) + lane;
-                        bool ok = false;
-                        if (j < N && j != i) {
-                            float acc = 0.f;
-#pragma unroll
-                            for (int c = 0; c < PD; ++c) {
-                                const float dlt = p[c] - sst[j * SD + c];
-                                acc = (c == 0) ? dlt * dlt : acc + dlt * dlt;
-                            }
-                            ok = acc < d.comm_sq_thr;
-                        }
-                        const unsigned bits = __ballot_sync(0xffffffffu, ok);
-                        if (lane == 0) my_bits[n_full] = bits;
-                        cnt += __popc(bits);
-                    }
-                }
+                if (valid) cnt = neighbour_bits<PD, SD>(d, p, i, sst, lane, sbits + slot * n_words);
                 if (lane == 0 && slot < APC) {
                     s_off[slot + 1] = valid ? (1 + cnt + __popc(hit_bits)) : 0;
                     s_hb[slot] = hit_bits;
@@ -717,33 +539,11 @@ rollout_persist_kernel(const __grid_constant__ PArgs P, const __grid_constant__ 
                     }
                     continue;
                 }
-                int32_t* er = er_n + env_e0;
-                int32_t* es = es_n + env_e0;
                 if (lane == 0) {
                     rs_n[a_id] = rbase;
                     rd_n[a_id] = deg;
-                    er[rbase] = a_id;
-                    es[rbase] = -1;
                 }
-                int pos = rbase + 1;
-                const unsigned lt = (1u << lane) - 1u;
-                const unsigned* my_bits = sbits + slot * n_words;
-                for (int w = 0; w < n_words; ++w) {
-                    const unsigned bits = my_bits[w];
-                    if (bits == 0u) continue;
-                    if ((bits >> lane) & 1u) {
-                        const int e = pos + __popc(bits & lt);
-                        er[e] = a_id;
-                        es[e] = env_a0 + (w << 5) + lane;
-                    }
-                    pos += __popc(bits);
-                }
-                const unsigned hb = s_hb[slot];
-                if ((hb >> lane) & 1u) {
-                    const int e = pos + __popc(hb & lt);
-                    er[e] = a_id;
-                    es[e] = -2 - lane;
-                }
+                fill_row(er_n + env_e0, es_n + env_e0, rbase, a_id, env_a0, sbits + slot * n_words, n_words, s_hb[slot], lane);
             }
             if (lrank == 0 && tid == 0) atomicAdd(&P.counters[(size_t)tn * 4 + 0], min(env_total, seg_cap));
             M_cur = min(env_total, seg_cap);
@@ -757,7 +557,7 @@ rollout_persist_kernel(const __grid_constant__ PArgs P, const __grid_constant__ 
 }
 
 struct WsLayout {
-    int64_t msg, logit, ag, v1, z, row_start, row_deg, edge_recv, edge_src, gbar, gtot, total;
+    int64_t msg, logit, ag, v1, z, row_start, row_deg, edge_recv, edge_src, gbar, total;
 };
 static WsLayout make_ws_layout(int E, int N, int cap_env) {   // (+ 16 (T + 1) floats of phase stamps appended by the caller)
     WsLayout W;
@@ -774,7 +574,6 @@ static WsLayout make_ws_layout(int E, int N, int cap_env) {   // (+ 16 (T + 1) f
     W.edge_recv = take(2 * EC);
     W.edge_src = take(2 * EC);
     W.gbar = take(E);
-    W.gtot = take(8 * (int64_t)E);
     W.total = o;
     return W;
 }
@@ -889,7 +688,6 @@ extern "C" __attribute__((visibility("default"))) int32_t gcbf_rollout_persisten
     GCBF_REQUIRE(!P.soft || (P.C >= 2 && E * P.C <= sm_count()), "pair mode needs n_graphs * %d <= %d CTAs", P.C, sm_count());
     GCBF_REQUIRE(P.soft || E <= max_cl || force_soft == 0, "more environments (%d) than resident clusters (%d)", E, max_cl);
     P.gbar = reinterpret_cast<unsigned*>(workspace + W.gbar);
-    P.gtot = reinterpret_cast<int*>(workspace + W.gtot);
     P.W1 = actor_params + L.w[L_MSG0];
     P.b1 = actor_params + L.b[L_MSG0];
     P.b23 = infer_blob + I.b23;

@@ -12,6 +12,7 @@
 
 #include "gemm.cuh"
 #include "gemm_tc.cuh"
+#include "geometry_dev.cuh"
 #include "gnn.cuh"
 #include "translayout.cuh"
 #include "smalljobs.cuh"
@@ -26,57 +27,6 @@ int32_t gnn_forward_impl(const gcbf_env_desc* d, int out_dim, const float* P, co
 
 // ------------------------------------------------------------------------------------ act + dynamics (forward)
 // a = 2 pi + u_ref ; u = clip_action(a) ; x' = agent_step_euler(x, u)   (gcbf_plus.py:386-391)
-// u_ref / Euler are restated here (default FMA contraction; the geometry TU keeps the strict copies).
-template <int KIND>
-__device__ __forceinline__ void u_ref_train(const gcbf_env_desc& d, const float* x, const float* gl, float* u) {
-    using T = EnvTraits<KIND>;
-    constexpr int SD = T::SD, NU = T::NU;
-    if (KIND == GCBF_ENV_DUBINS_CAR) {
-        const float PI_F = 3.14159265358979323846f, TWO_PI = 6.283185307179586f;
-        const float pdx = x[0] - gl[0], pdy = x[1] - gl[1];
-        const float dist = sqrtf(pdx * pdx + pdy * pdy);
-        float theta_t = atan2f(-pdy, -pdx);
-        theta_t = theta_t - floorf(theta_t / TWO_PI) * TWO_PI;
-        const float theta = x[2] - floorf(x[2] / TWO_PI) * TWO_PI;
-        const float theta_diff = theta_t - theta;
-        const float dot = (-pdx) * cosf(theta) + (-pdy) * sinf(theta);
-        const float tb = acosf(fminf(fmaxf(dot / (dist + 0.0001f), -1.f), 1.f));
-        float omega = 0.f;
-        const bool c1 = (theta_diff < PI_F) && (theta_diff >= 0.f);
-        if (c1 && theta <= PI_F) omega = tb;
-        if (!c1 && theta <= PI_F) omega = -tb;
-        const bool c2 = (theta_diff > -PI_F) && (theta_diff <= 0.f);
-        if (c2 && theta > PI_F) omega = -tb;
-        if (!c2 && theta > PI_F) omega = tb;
-        omega = fminf(fmaxf(omega, -5.f), 5.f);
-        const float nrm = sqrtf(1e-6f + (pdx * pdx + pdy * pdy));
-        const float coef = (nrm > d.comm_radius) ? d.comm_radius / fmaxf(nrm, d.comm_radius) : 1.f;
-        const float qx = coef * pdx, qy = coef * pdy;
-        u[0] = omega;
-        u[1] = -2.5f * x[3] + 2.3f * sqrtf(qx * qx + qy * qy);
-        return;
-    }
-    float err[SD], acc = 0.f;
-#pragma unroll
-    for (int c = 0; c < SD; ++c) {
-        err[c] = gl[c] - x[c];
-        acc += err[c] * err[c];
-    }
-    const float nrm = sqrtf(acc);
-#pragma unroll
-    for (int c = 0; c < SD; ++c) {
-        const float emax = fabsf(err[c] / nrm * d.comm_radius);
-        err[c] = (isnan(err[c]) || isnan(emax)) ? NAN : fminf(fmaxf(err[c], -emax), emax);
-    }
-#pragma unroll
-    for (int a = 0; a < NU; ++a) {
-        float s = 0.f;
-#pragma unroll
-        for (int c = 0; c < SD; ++c) s += err[c] * d.K[a * SD + c];
-        u[a] = isnan(s) ? NAN : fminf(fmaxf(s, -d.u_lim), d.u_lim);
-    }
-}
-
 template <int KIND>
 __global__ void act_dyn_kernel(const gcbf_env_desc d, const float* __restrict__ agent, const float* __restrict__ goal,
                                const float* __restrict__ pi, float* __restrict__ action, float* __restrict__ xnext) {
@@ -84,53 +34,21 @@ __global__ void act_dyn_kernel(const gcbf_env_desc d, const float* __restrict__ 
     constexpr int SD = T::SD, NU = T::NU;
     const int a = blockIdx.x * blockDim.x + threadIdx.x;
     if (a >= d.n_graphs * d.n_agents) return;
-    float x[SD], gl[SD], ur[NU], u[NU], xd[SD];
+    float x[SD], gl[SD], ur[NU], act[NU], xn[SD];
 #pragma unroll
     for (int c = 0; c < SD; ++c) {
         x[c] = agent[(size_t)a * SD + c];
         gl[c] = goal[(size_t)a * SD + c];
     }
-    u_ref_train<KIND>(d, x, gl, ur);
+    u_ref_dev<KIND>(d, x, gl, ur);
 #pragma unroll
     for (int c = 0; c < NU; ++c) {
-        const float act = 2.f * pi[(size_t)a * NU + c] + ur[c];
-        action[(size_t)a * NU + c] = act;
-        u[c] = isnan(act) ? act : fminf(fmaxf(act, -d.u_lim), d.u_lim);
+        act[c] = 2.f * pi[(size_t)a * NU + c] + ur[c];
+        action[(size_t)a * NU + c] = act[c];
     }
-    if (KIND == GCBF_ENV_SINGLE_INTEGRATOR) {
-        xd[0] = u[0];
-        xd[1] = u[1];
-    } else if (KIND == GCBF_ENV_DOUBLE_INTEGRATOR) {
-        xd[0] = x[2];
-        xd[1] = x[3];
-        xd[2] = u[0] / d.mass;
-        xd[3] = u[1] / d.mass;
-    } else if (KIND == GCBF_ENV_DUBINS_CAR) {
-        const float ddx = x[0] - gl[0], ddy = x[1] - gl[1];
-        const float keep = (sqrtf(ddx * ddx + ddy * ddy) < d.half_r) ? 0.f : 1.f;
-        xd[0] = cosf(x[2]) * x[3] * keep;
-        xd[1] = sinf(x[2]) * x[3] * keep;
-        xd[2] = u[0] * 20.f * keep;
-        xd[3] = u[1] * keep;
-    } else {
+    step_agent<KIND>(d, x, gl, act, ur, true, xn);
 #pragma unroll
-        for (int r = 0; r < SD; ++r) {
-            float s = 0.f;
-#pragma unroll
-            for (int c = 0; c < SD; ++c) s += x[c] * d.A[r * SD + c];
-#pragma unroll
-            for (int c = 0; c < NU; ++c) s += u[c] * d.B[r * NU + c];
-            xd[r] = s;
-        }
-    }
-#pragma unroll
-    for (int c = 0; c < SD; ++c) {
-        float v = xd[c] * d.dt + x[c];
-        const bool limited = (KIND == GCBF_ENV_DOUBLE_INTEGRATOR && c >= 2) || (KIND == GCBF_ENV_DUBINS_CAR && c == 3) ||
-                             (KIND == GCBF_ENV_LINEAR_DRONE && c >= 3);
-        if (limited) v = isnan(v) ? v : fminf(fmaxf(v, -d.v_lim), d.v_lim);
-        xnext[(size_t)a * SD + c] = v;
-    }
+    for (int c = 0; c < SD; ++c) xnext[(size_t)a * SD + c] = xn[c];
 }
 
 // ------------------------------------------------------------------------------------ losses (gcbf_plus.py:362-431)
