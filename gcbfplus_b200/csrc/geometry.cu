@@ -38,7 +38,7 @@ graph_build_kernel(const gcbf_env_desc d, const float* __restrict__ agent, const
     float* salpha = stab + d.n_rays * PD;       // 3-D only: [GB_WARPS, n_rays]
     const int n_words = (N + 31) / 32;
     unsigned* sbits = reinterpret_cast<unsigned*>(salpha + (PD == 3 ? GB_WARPS * d.n_rays : 0));  // [GB_WARPS, n_words]
-    int* stk = reinterpret_cast<int*>(sbits + GB_WARPS * n_words);                                 // 3-D only: [GB_WARPS, 80] top-k scratch
+    int* stk = reinterpret_cast<int*>(sbits + GB_WARPS * n_words);                                 // 3-D only: [GB_WARPS, 96] top-k scratch
     __shared__ int s_off[GB_WARPS + 1];
     __shared__ int s_base;
 
@@ -163,7 +163,9 @@ graph_build_kernel(const gcbf_env_desc d, const float* __restrict__ agent, const
                 for (int o = 16; o > 0; o >>= 1) nA += __shfl_xor_sync(0xffffffffu, nA, o);
                 fast = !__any_sync(0xffffffffu, odd) && nA <= 32 && (d.n_rays - nA) >= R;
                 if (fast) {
-                    int* tk = stk + warp * 80;              // [0,32) ray of a return, [32,64) its alpha bits, [64,80) first misses
+                    // [0,32) ray of a return, [32,64) its alpha bits, [64,96) first misses: up to R <= 32 of them are
+                    // needed (no returns at all)
+                    int* tk = stk + warp * 96;
                     const unsigned lt = (1u << lane) - 1u;
                     int nret = 0, nmiss = 0;
                     for (int r0 = 0; r0 < d.n_rays; r0 += 32) {
@@ -179,7 +181,7 @@ graph_build_kernel(const gcbf_env_desc d, const float* __restrict__ agent, const
                         }
                         if (is_miss) {
                             const int pos = nmiss + __popc(mb & lt);
-                            if (pos < 16) tk[64 + pos] = r;
+                            if (pos < 32) tk[64 + pos] = r;
                         }
                         nret += __popc(rb);
                         nmiss += __popc(mb);
@@ -191,7 +193,7 @@ graph_build_kernel(const gcbf_env_desc d, const float* __restrict__ agent, const
                     k.idx = (lane < nret) ? tk[lane] : (0x40000000 + lane);
                     if (nret > 1) k = warp_sort32(k, lane);
                     if (lane < R) {
-                        const int r = (lane < nret) ? k.idx : tk[64 + min(lane - nret, 15)];
+                        const int r = (lane < nret) ? k.idx : tk[64 + lane - nret];   // lane - nret < R - nret <= 32
                         const float a = (lane < nret) ? k.alpha : NO_HIT;
                         const float x2 = x1 + stab[r * PD + 0], y2 = y1 + stab[r * PD + 1], z2 = z1 + stab[r * PD + PD - 1];
                         my_hits[lane * PD + 0] = x1 + (x2 - x1) * a;
@@ -532,7 +534,7 @@ int32_t gcbf::graph_build_impl(const gcbf_env_desc* desc, const float* agent, co
     const int obw = pd == 2 ? 16 : 4;
     const size_t smem = sizeof(float) * ((size_t)desc->n_agents * pd + (size_t)desc->n_obs * (pd == 2 ? 24 : 4) +
                                          (size_t)desc->n_rays * pd + (pd == 3 ? (size_t)GB_WARPS * desc->n_rays : 0) +
-                                         (size_t)GB_WARPS * ((desc->n_agents + 31) / 32) + (pd == 3 ? (size_t)GB_WARPS * 80 : 0));
+                                         (size_t)GB_WARPS * ((desc->n_agents + 31) / 32) + (pd == 3 ? (size_t)GB_WARPS * 96 : 0));
     GCBF_REQUIRE(smem <= 200 * 1024, "graph_build needs %zu B shared memory (> 200 KB): too many agents/obstacles", smem);
     if (!(flags & 4)) {   // bit 2: the caller's previous kernel already cleared counters[0]
         cudaError_t e = cudaMemsetAsync(counters, 0, sizeof(int32_t), st);
