@@ -19,7 +19,7 @@ enum GemmEpi {
     EPI_BIAS_RELU = 1,  // C = relu(acc + bias (+ bias2))
     EPI_NONE = 2,       // C = acc
     EPI_RELU_MASK = 3,  // C = aux > 0 ? acc : 0      (backward through ReLU, aux = saved activation)
-    EPI_RELU_DOT = 4,   // C[m] = sum_n relu(acc + bias)[n] * aux[n] + bias2[0]   (tensor-core path only; N == BN)
+                        // 4 is unassigned: the C ABI passes these values, so they keep their numbers
     EPI_RELU_DOTN = 5,  // C[(part*m_cap + m)*4 + q] = sum_{n in column tile `part`} relu(acc + bias)[n] * aux[n*ndot + q]
                         // (tensor-core path only: the output layer folded into the last hidden layer's epilogue)
 };

@@ -296,15 +296,6 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                             make_float4(q[h][0], q[h][1], q[h][2], q[h][3]);
             continue;
         }
-        if (EPI == EPI_RELU_DOT) {    // gate logit: relu(acc + bias) . aux  (the row never leaves the SM)
-            float q[2][1];
-            frag_relu_dot<1>(d, bias, aux, 1, 1, wt, q);
-            if ((lane & 3) == 0)
-#pragma unroll
-                for (int h = 0; h < 2; ++h)
-                    if (r0 + 8 * h < M) C[r0 + 8 * h] = q[h][0] + bias2[0];
-            continue;
-        }
 #pragma unroll
         for (int i = 0; i < 64; i += 2) {
             const int m = r0 + 8 * ((i >> 1) & 1);
@@ -397,7 +388,7 @@ inline void launch_nn_inst(int grid, cudaStream_t st, const CUtensorMap& tmA, co
 inline int32_t launch_gemm_tc(int epi, bool accum, const float* A, const float* Bt_hi, const float* Bt_lo,
                               const float* bias, const float* bias2, float* C, const float* aux, RowCount rc, int K,
                               int N, cudaStream_t st, int ndot = 0, int* parts_out = nullptr) {
-    if (K % BK != 0 || (N != 128 && N != 256) || (epi == EPI_RELU_DOT && N != BN) || ndot > 4) {
+    if (K % BK != 0 || (N != 128 && N != 256) || ndot > 4) {
         set_error("gemm_tc: K=%d N=%d epi=%d unsupported", K, N, epi);
         return -1;
     }
@@ -417,7 +408,6 @@ inline int32_t launch_gemm_tc(int epi, bool accum, const float* A, const float* 
             case EPI_BIAS_RELU: GCBF_TC_CASE(EPI_BIAS_RELU, false); break;
             case EPI_NONE: GCBF_TC_CASE(EPI_NONE, false); break;
             case EPI_RELU_MASK: GCBF_TC_CASE(EPI_RELU_MASK, false); break;
-            case EPI_RELU_DOT: GCBF_TC_CASE(EPI_RELU_DOT, false); break;
             case EPI_RELU_DOTN: GCBF_TC_CASE(EPI_RELU_DOTN, false); break;
             default: set_error("bad epilogue"); return -1;
         }

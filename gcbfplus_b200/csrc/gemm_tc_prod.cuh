@@ -145,70 +145,6 @@ __device__ __forceinline__ void edge_tile_mainloop(float (&d)[64], uint8_t* smem
     mbar_arrive(&empty[(it - 1) % STAGES]);
 }
 
-// MSG[e, :128] = relu-layer-1(edge e) @ W23 + b23 (no chained gate layer)
-template <int KIND>
-__global__ void __launch_bounds__(THREADS_NN, 1)
-gemm_tc_prod_kernel(const __grid_constant__ CUtensorMap tmBh, const __grid_constant__ CUtensorMap tmBl,
-                    const __grid_constant__ ProdArgs pa, const float* __restrict__ bias, float* __restrict__ C,
-                    const int32_t* __restrict__ m_ptr, const int m_fixed, const int m_cap) {
-    constexpr int ED = EnvTraits<KIND>::ED;
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = smem_align1024(smem_raw);
-    uint64_t* full = reinterpret_cast<uint64_t*>(smem + STAGES * STG);
-    uint64_t* empty = full + STAGES;
-    float* sW = reinterpret_cast<float*>(smem + STAGES * STG + 256);
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < STAGES; ++s) {
-            mbar_init(&full[s], 1);
-            mbar_init(&empty[s], CONSUMERS);
-        }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    load_l1_table<ED>(sW, pa.W1, pa.b1, threadIdx.x, blockDim.x);
-    __syncthreads();
-    int M = m_ptr ? *m_ptr : m_fixed;
-    M = min(M, m_cap);
-    const int n_tiles = (M + BM - 1) / BM;
-
-    if (warp == 8) {
-        if (lane == 0) {
-            uint32_t it = 0;
-            for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x)
-                for (int kb = 0; kb < 8; ++kb, ++it) {
-                    const int s = it % STAGES;
-                    mbar_wait(&empty[s], ((it / STAGES) & 1) ^ 1);
-                    uint8_t* st = smem + s * STG;
-                    mbar_expect_tx(&full[s], 2 * PLANE);
-                    tma_load_2d(st + 2 * PLANE, &tmBh, &full[s], kb * BK, 0);
-                    tma_load_2d(st + 3 * PLANE, &tmBl, &full[s], kb * BK, 0);
-                }
-        }
-        return;
-    }
-    const int g = warp >> 2, wt = threadIdx.x & 127;
-    const int r = 64 * g + (wt & 63), half = wt >> 6;   // producer: tile row, 16-column half of a k-block
-    uint32_t it = 0;
-    for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-        const int m = tile * BM + r;
-        float f[ED];
-        int stype;
-        edge_row_setup<KIND>(pa, m, m < M, f, stype);
-        float d[64];
-        edge_tile_mainloop<ED>(d, smem, full, empty, it, g, r, half, m < M, sW, f, stype);
-        const int r0 = tile * BM + 64 * g + frag_row0(wt);
-#pragma unroll
-        for (int i = 0; i < 64; i += 2) {
-            const int mm = r0 + 8 * ((i >> 1) & 1);
-            if (mm >= M) continue;
-            const int n = frag_col(wt, i);
-            const float2 bb = *reinterpret_cast<const float2*>(bias + n);
-            *reinterpret_cast<float2*>(C + (size_t)mm * 128 + n) = make_float2(d[i] + bb.x, d[i + 1] + bb.y);
-        }
-    }
-}
-
 // edge message GEMM + chained gate GEMM (see ChainArgs).  Barriers: full / empty = the 3-stage ring of W23 planes;
 // main_done = both warpgroups' main-loop MMAs retired (stage 2 free for the gate weights); b2_full / b2_empty = the two
 // gate-weight slots; t2f = the chained GEMM retired (the stages may be refilled for the next tile).
@@ -316,57 +252,40 @@ edge_chain_kernel(const __grid_constant__ CUtensorMap tmBh, const __grid_constan
 
 constexpr int PROD_SMEM = STAGES * STG + 256 + L1_FLOATS * 4 + 1024;
 
-// MSG[e, :128] = relu-layer-1(edge e) @ W23 + b23: edge_l1 producer + folded message GEMM (K = 256, N = 128).
-// chain != nullptr: the gate layer (K = N = 128, weights gate_Bt_*) and its folded gate vector run inside the same
-// kernel and the logits are written to chain->logits.
+// MSG[e, :128] = relu-layer-1(edge e) @ W23 + b23: edge_l1 producer + folded message GEMM (K = 256, N = 128), with the
+// gate layer (K = N = 128, weights gate_Bt_*) and its folded gate vector chained in the same kernel: the logits are
+// written to chain.logits.
 inline int32_t launch_edge_msg(const gcbf_env_desc* d, const float* W1, const float* b1, const float* agent,
                                const float* goal, const float* hits, const int32_t* edge_recv,
                                const int32_t* edge_src, const int32_t* counters, int clip_all, const float* Bt_hi,
                                const float* Bt_lo, const float* bias, float* msg, cudaStream_t st,
-                               const float* gate_Bt_hi = nullptr, const float* gate_Bt_lo = nullptr,
-                               const ChainArgs* chain = nullptr) {
+                               const float* gate_Bt_hi, const float* gate_Bt_lo, const ChainArgs& chain) {
+    if (!counters) {
+        set_error("launch_edge_msg: the chained gate GEMM needs the device edge counter");
+        return -1;
+    }
     ProdArgs pa;
     memset(&pa, 0, sizeof(pa));
     pa.d = *d;
     pa.W1 = W1; pa.b1 = b1; pa.agent = agent; pa.goal = goal; pa.hits = hits;
     pa.edge_recv = edge_recv; pa.edge_src = edge_src; pa.clip_all = clip_all;
     const int K = 256, N = 128;
-    CUtensorMap tmB, tmBl;
+    CUtensorMap tmB, tmBl, tmG, tmGl;
     if (int32_t r = make_map(&tmB, Bt_hi, N, K, N)) return r;
     if (int32_t r = make_map(&tmBl, Bt_lo, N, K, N)) return r;
-    const RowCount rc{counters, 0, d->edge_cap};
+    if (int32_t r = make_map(&tmG, gate_Bt_hi, 128, 128, 128)) return r;
+    if (int32_t r = make_map(&tmGl, gate_Bt_lo, 128, 128, 128)) return r;
     const int grid = min((d->edge_cap + BM - 1) / BM, sm_count());
-    if (chain) {
-        if (!counters) {
-            set_error("launch_edge_msg: the chained gate GEMM needs the device edge counter");
-            return -1;
-        }
-        CUtensorMap tmG, tmGl;
-        if (int32_t r = make_map(&tmG, gate_Bt_hi, 128, 128, 128)) return r;
-        if (int32_t r = make_map(&tmGl, gate_Bt_lo, 128, 128, 128)) return r;
-        GCBF_DISPATCH_ENV(d->env_kind, {
-            auto kern = edge_chain_kernel<KIND>;
-            static bool attr_done = false;
-            if (!attr_done) {
-                cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, PROD_SMEM);
-                attr_done = true;
-            }
-            kern<<<grid, THREADS_NN, PROD_SMEM, st>>>(tmB, tmBl, tmG, tmGl, pa, bias, msg, rc.ptr, rc.cap, *chain);
-            count_launch();
-            return check_launch("edge_chain_kernel");
-        });
-        return -1;
-    }
     GCBF_DISPATCH_ENV(d->env_kind, {
-        auto kern = gemm_tc_prod_kernel<KIND>;
+        auto kern = edge_chain_kernel<KIND>;
         static bool attr_done = false;
         if (!attr_done) {
             cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, PROD_SMEM);
             attr_done = true;
         }
-        kern<<<grid, THREADS_NN, PROD_SMEM, st>>>(tmB, tmBl, pa, bias, msg, rc.ptr, rc.fixed, rc.cap);
+        kern<<<grid, THREADS_NN, PROD_SMEM, st>>>(tmB, tmBl, tmG, tmGl, pa, bias, msg, counters, d->edge_cap, chain);
         count_launch();
-        return check_launch("gemm_tc_prod_kernel");
+        return check_launch("edge_chain_kernel");
     });
     return -1;
 }

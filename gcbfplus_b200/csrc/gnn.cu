@@ -1,6 +1,4 @@
 // gnn.cu -- GNN forward for one network (CBF h(x) or policy pi(x)) over a swarm batch.
-#include <stdlib.h>
-
 #include "gemm.cuh"
 #include "gemm_tc.cuh"
 #include "gnn.cuh"
@@ -151,8 +149,7 @@ extern "C" __attribute__((visibility("default"))) int32_t gcbf_gemm_tc(int32_t e
                                                                        int32_t m_cap, int32_t K, int32_t N,
                                                                        int32_t ndot, void* stream) {
     GCBF_REQUIRE(A && Bt_hi && Bt_lo && C, "gcbf_gemm_tc: NULL pointer");
-    GCBF_REQUIRE((epi != EPI_RELU_DOT && epi != EPI_RELU_DOTN) || (bias && aux), "gcbf_gemm_tc: bias and aux required");
-    GCBF_REQUIRE(epi != EPI_RELU_DOT || bias2, "gcbf_gemm_tc: bias2 required");
+    GCBF_REQUIRE(epi != EPI_RELU_DOTN || (bias && aux), "gcbf_gemm_tc: bias and aux required");
     GCBF_REQUIRE(epi != EPI_RELU_DOTN || (ndot >= 1 && ndot <= 4), "gcbf_gemm_tc: ndot must be in [1, 4]");
     GCBF_REQUIRE((epi != EPI_BIAS && epi != EPI_BIAS_RELU) || bias, "gcbf_gemm_tc: bias required");
     GCBF_REQUIRE(epi != EPI_RELU_MASK || aux, "gcbf_gemm_tc: aux required");
@@ -361,13 +358,10 @@ int32_t gnn_infer_impl(const gcbf_env_desc* d, int out_dim, const float* P, cons
         return launch_gemm_nn(epi, false, X, Wf, bias, bias2, Y, nullptr, rows, K, N, st);
     };
     if (use_tc && !keep_activations) {
-        // tensor-core path, 4 launches: {edge features + layer 1 produced in-kernel -> folded message GEMM},
-        // {gate layer + folded gate vector -> logits}, {softmax-aggregate produced in-kernel -> update layer 1},
+        // tensor-core path, 4 launches: {edge features + layer 1 produced in-kernel -> folded message GEMM -> chained
+        // gate layer + folded gate vector -> logits}, {softmax + aggregate}, {update layer 1},
         // {update/head folded layer (+ output layer) below}
-        // GCBF_CHAIN=0: gate layer as its own GEMM launch (A/B measurements)
-        static const bool chain_on = [] { const char* e = getenv("GCBF_CHAIN"); return !(e && e[0] == '0'); }();
-        if (!(select & 1)) {
-        } else if (chain_on) {
+        if (select & 1) {
             tc::ChainArgs ch;
             ch.bias_g = P + L.b[L_ATT0];
             ch.avec = blob + I.a23;
@@ -375,13 +369,7 @@ int32_t gnn_infer_impl(const gcbf_env_desc* d, int out_dim, const float* P, cons
             ch.logits = ws + W.att;
             if ((rc = tc::launch_edge_msg(d, P + L.w[L_MSG0], P + L.b[L_MSG0], agent, goal, hits, edge_recv, edge_src,
                                           counters, clip_all, blob + I.t_w23, blob + I.t_w23 + 256 * 128, blob + I.b23,
-                                          ws + W.msg, st, blob + I.t_a1, blob + I.t_a1 + 128 * 128, &ch))) return rc;
-        } else {
-            if ((rc = tc::launch_edge_msg(d, P + L.w[L_MSG0], P + L.b[L_MSG0], agent, goal, hits, edge_recv, edge_src,
-                                          counters, clip_all, blob + I.t_w23, blob + I.t_w23 + 256 * 128, blob + I.b23,
-                                          ws + W.msg, st))) return rc;
-            if ((rc = tc::launch_gemm_tc(EPI_RELU_DOT, false, ws + W.msg, blob + I.t_a1, blob + I.t_a1 + 128 * 128,
-                                         P + L.b[L_ATT0], blob + I.c23, ws + W.att, blob + I.a23, re, 128, 128, st))) return rc;
+                                          ws + W.msg, st, blob + I.t_a1, blob + I.t_a1 + 128 * 128, ch))) return rc;
         }
         // (measured: producing the aggregate inside the update GEMM (tc::launch_attn_upd) is slower than the
         //  separate warp-per-receiver kernel + TMA-fed GEMM: 36.6 us vs 13.2 + 11.7 us -- its N-split repeats

@@ -235,7 +235,7 @@ attn_aggregate_kernel(const int A, const int edge_cap, const float* __restrict__
                       const float* __restrict__ a3, const float* __restrict__ ba3,
                       const int32_t* __restrict__ row_start, const int32_t* __restrict__ row_deg,
                       float* __restrict__ ATT, float* __restrict__ AG, int32_t* __restrict__ zero_counter = nullptr) {
-    // G2 == nullptr (inference): ATT already holds the gate logits (written by the EPI_RELU_DOT GEMM epilogue) and is
+    // G2 == nullptr (inference): ATT already holds the gate logits (written by tc::edge_chain_kernel) and is
     // left as it is.  Otherwise (training) the gate logits are computed here and ATT receives the attention weights
     // that the backward pass reads.
     // zero_counter (rollout step): edge counter of the NEXT graph, cleared here so that no memset node sits in the

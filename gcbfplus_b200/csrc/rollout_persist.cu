@@ -739,22 +739,16 @@ extern "C" __attribute__((visibility("default"))) int32_t gcbf_rollout_persisten
     cfg.blockDim = dim3(rp::PT, 1, 1);
     cfg.dynamicSmemBytes = smem;
     cfg.stream = (cudaStream_t)stream;
-    cudaLaunchAttribute attr[2];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = (unsigned)(P.soft ? 2 : P.C);
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
+    cudaLaunchAttribute attr;
+    attr.id = cudaLaunchAttributeClusterDimension;
+    attr.val.clusterDim.x = (unsigned)(P.soft ? 2 : P.C);
+    attr.val.clusterDim.y = 1;
+    attr.val.clusterDim.z = 1;
+    cfg.attrs = &attr;
     cfg.numAttrs = 1;
     // pair mode spins on a counter the other CTAs of the environment must reach: every CTA has to be resident.  The grid
-    // was checked against the SM count (1 CTA / SM) and the cluster-of-2 occupancy above; GCBF_PERSIST_COOP=1 additionally
-    // asks the driver to guarantee it (cooperative launch attribute).  A protocol failure ends in a trap, not a hang.
-    static const bool coop = [] { const char* e = getenv("GCBF_PERSIST_COOP"); return e && e[0] == '1'; }();
-    if (P.soft && coop) {
-        attr[1].id = cudaLaunchAttributeCooperative;
-        attr[1].val.cooperative = 1;
-        cfg.numAttrs = 2;
-    }
+    // was checked against the SM count (1 CTA / SM) and the cluster-of-2 occupancy above.  A protocol failure ends in a
+    // trap, not a hang.
     cudaError_t e = cudaSuccess;
     if (P.soft && (e = cudaMemsetAsync(P.gbar, 0, sizeof(unsigned) * E, (cudaStream_t)stream)) != cudaSuccess) {
         set_error("cudaMemsetAsync: %s", cudaGetErrorString(e));

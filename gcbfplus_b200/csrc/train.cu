@@ -3,13 +3,11 @@
 // step and the action clip back into the actor), global-norm clip + AdamW + apply_if_finite,
 // and the target-network polyak update.  On the tensor-core path the step runs on the folded
 // network (gnn_backward_folded / unfold_jobs below: 4 GEMMs per pass and direction instead of
-// 9-10, same gradient); the layer-by-layer step remains for the SIMT path and GCBF_TRAIN_FOLD=0.
+// 9-10, same gradient); the strict-fp32 SIMT path runs the layer-by-layer step.
 //
 // Replaces gcbfplus/algo/gcbf_plus.py:354-447 (update_inner / get_loss / value_and_grad),
 // trainer/utils.py:62-75 (compute_norm_and_clip), optax.adamw + optax.apply_if_finite
 // (gcbf_plus.py:109-110,127-128) and gcbf_plus.py:188-191 (update_tgt).
-#include <stdlib.h>
-
 #include "gemm.cuh"
 #include "gemm_tc.cuh"
 #include "geometry_dev.cuh"
@@ -559,12 +557,11 @@ struct BwdArgs {
     int use_tc;            // 1: backward-data GEMMs on the wgmma path
 };
 
-// dW += X^T (w dY) and db (+ db2) += sum_m w dY: tensor-core kernel (MN-major 3xTF32, column sums fused into its
-// operand-split pass) or the SIMT split-M kernel followed by column-sum launches.
+// dW += X^T (w dY) and db (+ db2) += sum_m w dY: the SIMT split-M kernel followed by column-sum launches.  Only
+// the SIMT train step computes weight gradients layer by layer; the folded step has its own (gnn_backward_folded).
 static int32_t dense_bwd_weight(const BwdArgs& b, const float* X, int ldx, const float* dY, float* C, float* db,
                                 float* db2, const int32_t* row2agent, RowCount rc, int K1, int N, int A,
                                 cudaStream_t st) {
-    if (b.use_tc) return tc::launch_gemm_tn_tc(X, ldx, dY, C, b.roww, row2agent, rc, K1, N, A, st, db, db2);
     if (int32_t r = launch_gemm_tn(X, ldx, dY, C, b.roww, row2agent, rc, K1, N, A, st)) return r;
     if (int32_t r = launch_colsum(dY, db, b.roww, row2agent, rc, N, A, st)) return r;
     if (db2) return launch_colsum(dY, db2, b.roww, row2agent, rc, N, A, st);
@@ -757,7 +754,9 @@ static int32_t gnn_backward_folded(const BwdArgs& b, const float* blob, float* G
     return 0;
 }
 
-// Chain rule of the folded products: G (flax layout) += d(folded) / d(parameters) applied to Gf.  `scratch`: 256 * 128 + 128 floats.
+constexpr int64_t UNFOLD_SCRATCH = 256 * 128 + 128;   // floats of unfold_jobs' `scratch`: T [256, 128] and t [128]
+
+// Chain rule of the folded products: G (flax layout) += d(folded) / d(parameters) applied to Gf.
 //   W23 = W2 W3, b23 = b2 W3 + b3          -> dW2 = dW23 W3^T, dW3 = W2^T dW23 + b2 (x) db23, db2 = db23 W3^T, db3 = db23
 //   a23 = A2 a3, c23 = ba2 . a3 + ba3      -> dA2 = da23 (x) a3, da3 = A2^T da23 + ba2 dc23, dba2 = a3 dc23, dba3 = dc23
 //   UH = U2 U3 H1, buh = (bu2 U3 + bu3) H1 + bh1
@@ -916,23 +915,41 @@ __global__ void fill_kernel(float* __restrict__ p, const int n, const float v) {
 }
 
 // ------------------------------------------------------------------------------------ train workspace layout
+// One parameter region per network, holding what the step of its GEMM path needs: the SIMT step the transposed
+// weights (TransLayout, at `pt`), the folded tensor-core step [folded blob (InferLayout) at `pt` | gradient of the
+// folded weights at `gf` | un-fold scratch at `scr`].
+struct TrainNetWs {
+    int64_t pt, gf, scr;
+};
 struct TrainWs {
-    int64_t ws0, ws1, ws2, gws, pt_cbf, pt_act, h, hn, pi, act, xn, d_es, dh, dhn, da, dpi, lab, total;
+    int64_t ws0, ws1, ws2, gws;
+    TrainNetWs net_cbf, net_act;
+    int64_t h, hn, pi, act, xn, d_es, dh, dhn, da, dpi, lab, total;
 };
 static TrainWs make_train_ws(const gcbf_env_desc* d) {
     const int ed = env_ed(d->env_kind), nu = env_nu(d->env_kind), sd = env_sd(d->env_kind);
     const int64_t A = (int64_t)d->n_graphs * d->n_agents;
     const GnnWs W = make_ws(d->edge_cap, A);
-    const TransLayout Tc = make_trans_layout(make_layout(ed, 1)), Ta = make_trans_layout(make_layout(ed, nu));
     TrainWs t;
     int64_t o = 0;
-    auto take = [&](int64_t n) { int64_t r = o; o += (n + 7) & ~(int64_t)7; return r; };   // 32-byte slots: 256-bit epilogue stores
+    auto up8 = [](int64_t n) { return (n + 7) & ~(int64_t)7; };   // 32-byte slots: 256-bit epilogue stores
+    auto take = [&](int64_t n) { int64_t r = o; o += up8(n); return r; };
+    auto take_net = [&](int out_dim) {
+        const InferLayout I = make_infer_layout(out_dim);
+        const int64_t simt = make_trans_layout(make_layout(ed, out_dim)).total;
+        const int64_t folded = up8(I.total) + up8(I.t_w23) + UNFOLD_SCRATCH;
+        TrainNetWs n;
+        n.pt = take(simt > folded ? simt : folded);
+        n.gf = n.pt + up8(I.total);
+        n.scr = n.gf + up8(I.t_w23);
+        return n;
+    };
     t.ws0 = take(W.total);
     t.ws1 = take(W.total);
     t.ws2 = take(W.total);
     t.gws = take(W.total);
-    t.pt_cbf = take(make_prepared_layout(make_layout(ed, 1), Tc).total);
-    t.pt_act = take(make_prepared_layout(make_layout(ed, nu), Ta).total);
+    t.net_cbf = take_net(1);
+    t.net_act = take_net(nu);
     t.h = take(A);
     t.hn = take(A);
     t.pi = take(A * nu);
@@ -1014,56 +1031,40 @@ extern "C" __attribute__((visibility("default"))) int32_t gcbf_train_step(
         set_error("cudaMemsetAsync: %s", cudaGetErrorString(e));
         return (int32_t)e;
     }
+    // tensor-core path: the folded step; SIMT path: the layer-by-layer step (see TrainWs for the parameter regions)
     const int use_tc = hp_host[6] != 0.f;
-    // folded train step (tensor-core path; GCBF_TRAIN_FOLD=0 keeps the layer-by-layer step): the prepared-parameter
-    // regions of the workspace hold [folded blob | gradient of the folded weights | un-fold scratch] instead
-    static const bool fold_on = [] { const char* e = getenv("GCBF_TRAIN_FOLD"); return !(e && e[0] == '0'); }();
-    const bool fold = use_tc && fold_on;
-    const InferLayout Ic = make_infer_layout(1), Ia = make_infer_layout(nu);
-    auto up8 = [](int64_t n) { return (n + 7) & ~(int64_t)7; };
-    float* blob_c = ws + TW.pt_cbf;
-    float* gf_c = blob_c + up8(Ic.total);
-    float* scr_c = gf_c + up8(Ic.t_w23);
-    float* blob_a = ws + TW.pt_act;
-    float* gf_a = blob_a + up8(Ia.total);
-    float* scr_a = gf_a + up8(Ia.t_w23);
-    if (fold) {
-        const int64_t scr = 256 * 128 + 128;
-        GCBF_REQUIRE(up8(Ic.total) + up8(Ic.t_w23) + scr <= TW.pt_act - TW.pt_cbf &&
-                         up8(Ia.total) + up8(Ia.t_w23) + scr <= TW.h - TW.pt_act,
-                     "gcbf_train_step: folded blobs do not fit the prepared-parameter regions");
+    float* blob_c = ws + TW.net_cbf.pt;
+    float* blob_a = ws + TW.net_act.pt;
+    float* gf_c = ws + TW.net_cbf.gf;
+    float* gf_a = ws + TW.net_act.gf;
+    if (use_tc) {
         RC(prepare_infer_pair(ed, 1, cbf_params, blob_c, nu, actor_params, blob_a, st));
-        if ((e = cudaMemsetAsync(gf_c, 0, sizeof(float) * Ic.t_w23, st)) != cudaSuccess ||
-            (e = cudaMemsetAsync(gf_a, 0, sizeof(float) * Ia.t_w23, st)) != cudaSuccess) {
+        if ((e = cudaMemsetAsync(gf_c, 0, sizeof(float) * make_infer_layout(1).t_w23, st)) != cudaSuccess ||
+            (e = cudaMemsetAsync(gf_a, 0, sizeof(float) * make_infer_layout(nu).t_w23, st)) != cudaSuccess) {
             set_error("cudaMemsetAsync: %s", cudaGetErrorString(e));
             return (int32_t)e;
         }
-    } else if (use_tc) {
-        RC(build_prepared(Lc, cbf_params, ws + TW.pt_cbf, st));
-        RC(build_prepared(La, actor_params, ws + TW.pt_act, st));
     } else {
-        RC(build_transposes(Lc, make_trans_layout(Lc), cbf_params, ws + TW.pt_cbf, st));
-        RC(build_transposes(La, make_trans_layout(La), actor_params, ws + TW.pt_act, st));
+        RC(build_transposes(Lc, make_trans_layout(Lc), cbf_params, ws + TW.net_cbf.pt, st));
+        RC(build_transposes(La, make_trans_layout(La), actor_params, ws + TW.net_act.pt, st));
     }
     // ---- forward: h = cbf(g), pi = actor(g), x' = f(x, clip(2 pi + u_ref)), h' = cbf(g')
-    const float* ptc = use_tc ? ws + TW.pt_cbf : nullptr;
-    const float* pta = use_tc ? ws + TW.pt_act : nullptr;
-    auto forward = [&](int out_dim, const float* params, const float* pt, const float* blob, const float* x, int clip_all,
-                       float* out, float* fws) -> int32_t {
-        if (fold)
+    auto forward = [&](int out_dim, const float* params, const float* blob, const float* x, int clip_all, float* out,
+                       float* fws) -> int32_t {
+        if (use_tc)
             return gnn_infer_impl(d, out_dim, params, blob, 1, x, goal, hits, row_start, row_deg, edge_recv, edge_src,
                                   counters, clip_all, out, fws, st, nullptr, nullptr, nullptr, 0xF, 1);
-        return gnn_forward_impl(d, out_dim, params, pt, x, goal, hits, row_start, row_deg, edge_recv, edge_src, counters,
-                                clip_all, out, fws, st);
+        return gnn_forward_impl(d, out_dim, params, nullptr, x, goal, hits, row_start, row_deg, edge_recv, edge_src,
+                                counters, clip_all, out, fws, st);
     };
-    RC(forward(1, cbf_params, ptc, blob_c, agent, 0, ws + TW.h, ws + TW.ws0));
-    RC(forward(nu, actor_params, pta, blob_a, agent, 0, ws + TW.pi, ws + TW.ws1));
+    RC(forward(1, cbf_params, blob_c, agent, 0, ws + TW.h, ws + TW.ws0));
+    RC(forward(nu, actor_params, blob_a, agent, 0, ws + TW.pi, ws + TW.ws1));
     GCBF_DISPATCH_ENV(d->env_kind, {
         act_dyn_kernel<KIND><<<(A + 127) / 128, 128, 0, st>>>(*d, agent, goal, ws + TW.pi, ws + TW.act, ws + TW.xn);
     });
     count_launch();
     RC(check_launch("act_dyn_kernel"));
-    RC(forward(1, cbf_params, ptc, blob_c, ws + TW.xn, 1, ws + TW.hn, ws + TW.ws2));
+    RC(forward(1, cbf_params, blob_c, ws + TW.xn, 1, ws + TW.hn, ws + TW.ws2));
     // ---- losses and their derivatives wrt h, h', a
     {
         const int grid = min((A + 255) / 256, 2 * sm_count());
@@ -1090,7 +1091,7 @@ extern "C" __attribute__((visibility("default"))) int32_t gcbf_train_step(
     b.gw = ws + TW.gws;
     b.out_dim = 1;
     b.P = cbf_params;
-    b.PT = ws + TW.pt_cbf;
+    b.PT = ws + TW.net_cbf.pt;
     b.fw = ws + TW.ws2;
     b.out = ws + TW.hn;
     b.d_out = ws + TW.dhn;
@@ -1101,7 +1102,7 @@ extern "C" __attribute__((visibility("default"))) int32_t gcbf_train_step(
     b.je = nullptr;
     b.use_tc = use_tc;
     auto backward = [&](const float* blob, float* gf) -> int32_t {
-        return fold ? gnn_backward_folded(b, blob, gf, st) : gnn_backward_impl(b, st);
+        return use_tc ? gnn_backward_folded(b, blob, gf, st) : gnn_backward_impl(b, st);
     };
     RC(backward(blob_c, gf_c));
     // ---- through the Euler step / clips into the policy output
@@ -1115,7 +1116,7 @@ extern "C" __attribute__((visibility("default"))) int32_t gcbf_train_step(
     b.agent = agent;
     b.out_dim = nu;
     b.P = actor_params;
-    b.PT = ws + TW.pt_act;
+    b.PT = ws + TW.net_act.pt;
     b.fw = ws + TW.ws1;
     b.out = ws + TW.pi;
     b.d_out = ws + TW.dpi;
@@ -1127,16 +1128,16 @@ extern "C" __attribute__((visibility("default"))) int32_t gcbf_train_step(
     // ---- backward 3: cbf on g
     b.out_dim = 1;
     b.P = cbf_params;
-    b.PT = ws + TW.pt_cbf;
+    b.PT = ws + TW.net_cbf.pt;
     b.fw = ws + TW.ws0;
     b.out = ws + TW.h;
     b.d_out = ws + TW.dh;
     b.G = grad_cbf;
     RC(backward(blob_c, gf_c));
-    if (fold) {
+    if (use_tc) {
         SmallJobList JT, JU;      // both networks share the two un-fold launches
-        unfold_jobs(ed, 1, cbf_params, blob_c, gf_c, grad_cbf, scr_c, JT, JU);
-        unfold_jobs(ed, nu, actor_params, blob_a, gf_a, grad_actor, scr_a, JT, JU);
+        unfold_jobs(ed, 1, cbf_params, blob_c, gf_c, grad_cbf, ws + TW.net_cbf.scr, JT, JU);
+        unfold_jobs(ed, nu, actor_params, blob_a, gf_a, grad_actor, ws + TW.net_act.scr, JT, JU);
         RC(JT.launch(st));
         RC(JU.launch(st));
     }

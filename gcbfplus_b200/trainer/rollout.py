@@ -26,13 +26,13 @@ from .data import Rollout
 
 
 class _Chain:
-    """Per-chain scratch: a contiguous slice [e0, e1) of the environments with its own topology arrays,
-    policy output and activation workspace, so that chains are independent branches of the CUDA graph."""
+    """Scratch of the step-by-step path: topology arrays, policy output and activation workspace of all the
+    environments (e0 = 0: the first of them)."""
 
-    def __init__(self, eng: "RolloutEngine", e0: int, e1: int):
+    def __init__(self, eng: "RolloutEngine"):
         env, dev = eng.env, eng.env.device
-        self.e0, self.e1 = e0, e1
-        E, N, nu = e1 - e0, env.num_agents, env.action_dim
+        self.e0 = 0
+        E, N, nu = eng.E, env.num_agents, env.action_dim
         f32, i32 = torch.float32, torch.int32
         self.desc = env.desc(E, eng.O)
         cap = self.desc.edge_cap
@@ -46,7 +46,6 @@ class _Chain:
         self.counters = torch.zeros(eng.T + 1, 4, dtype=i32, device=dev)
         n_ws = env.lib.gcbf_rollout_workspace_floats(C.byref(self.desc))
         self.ws = torch.empty(int(n_ws), dtype=f32, device=dev)
-        self.stream = None
         if eng.controller is not None:
             # CBF-QP baseline: pairwise-CBF workspace, relaxations (scratch) and the per-step iteration record
             n_qp = env.lib.gcbf_cbfqp_workspace_floats(C.byref(self.desc))
@@ -57,13 +56,9 @@ class _Chain:
 
 class RolloutEngine:
     def __init__(self, env, n_envs: int, T: Optional[int] = None, n_obs: Optional[int] = None,
-                 use_cuda_graph: bool = True, policy: str = "actor", n_chains: Optional[int] = None,
-                 persistent: Optional[bool] = None):
+                 use_cuda_graph: bool = True, policy: str = "actor", persistent: Optional[bool] = None):
         """policy: 'actor' (a = 2 pi + u_ref, algo.step), 'u_ref' (test.py --u-ref), or a CBF-QP baseline: a
-        DecShareCBF / CentralizedCBF object, or its name ('dec_share_cbf' / 'centralized_cbf': built with alpha = 1).
-        n_chains: the environments are split into independent chains that run as parallel branches of
-        the CUDA graph (each per-step kernel is latency-bound and fills a fraction of the 132 SMs, so
-        concurrent chains overlap their launch / tail latencies).  Results do not depend on it."""
+        DecShareCBF / CentralizedCBF object, or its name ('dec_share_cbf' / 'centralized_cbf': built with alpha = 1)."""
         self.env = env
         self.E = n_envs
         self.T = T or env.max_episode_steps
@@ -93,13 +88,7 @@ class RolloutEngine:
         self.actions = torch.zeros(T, E, N, nu, dtype=f32, device=dev)
         self.rewards = torch.zeros(T, E, dtype=f32, device=dev)
         self.costs = torch.zeros(T, E, dtype=f32, device=dev)
-        if n_chains is None:
-            n_chains = 1   # measured: no gain at fixed E (each chain's step latency does not shrink with its batch)
-        if not use_cuda_graph:
-            n_chains = 1
-        assert E % n_chains == 0
-        per = E // n_chains
-        self.chains = [_Chain(self, c * per, (c + 1) * per) for c in range(n_chains)]
+        self.chains = [_Chain(self)]   # a one-element list: bench.py reads eng.chains[0]
         self.desc = self.chains[0].desc
         self.params_buf = torch.zeros(_lib.param_count(env.edge_dim, nu), dtype=f32, device=dev)
         # folded inference weights (gcbf_prepare_infer), rebuilt by set_params()
@@ -112,7 +101,7 @@ class RolloutEngine:
         per_agent = min(1 + (N - 1) + R, max(2 * env.edge_cap_per_agent, 48))
         self._pdesc = env.desc(E, self.O, edge_cap=E * N * per_agent)
         level = int(env.lib.gcbf_rollout_persistent_supported(C.byref(self._pdesc))) \
-            if (policy == "actor" and self.use_tc and len(self.chains) == 1) else 0
+            if (policy == "actor" and self.use_tc) else 0
         ok = level > 0
         if persistent is None:
             # default only where every environment's cluster is resident at once (level 2): otherwise the environments
@@ -125,7 +114,7 @@ class RolloutEngine:
             persistent = (level == 2 and env.ENV_ID != "DubinsCar" and os.environ.get("GCBF_PERSISTENT", "1") != "0")
         if persistent and not ok:
             raise ValueError("persistent rollout unsupported for this configuration (2-D env, n <= 512, tensor-core path, "
-                             "actor policy, one chain)")
+                             "actor policy)")
         self.persistent = bool(persistent)
         #: optional [T + 1, 8] int64 device tensor: in-kernel %globaltimer stamps of the persistent rollout (set before
         #: the first run(); see gcbf_rollout_persistent in include/gcbf_b200.h)
@@ -140,9 +129,8 @@ class RolloutEngine:
 
     @property
     def counters(self) -> torch.Tensor:
-        """[T+1, 4]: per step total edge count (col 0) and overflow flag (col 1) over all chains."""
-        c = torch.stack([ch.counters for ch in self.chains])
-        return torch.stack([c[:, :, 0].sum(0), c[:, :, 1].amax(0), c[:, :, 2].sum(0), c[:, :, 3].sum(0)], dim=1)
+        """[T+1, 4] int32 record: per step total edge count (col 0) and overflow flag (col 1)."""
+        return self.chains[0].counters
 
     # ------------------------------------------------------------------ one env step (enqueue only)
     def _build(self, ch: _Chain, t: int, stream: int) -> None:
@@ -188,11 +176,6 @@ class RolloutEngine:
         _lib.check(rc, "gcbf_env_step")
         self._build(ch, t + 1, stream)
 
-    def _enqueue_chain(self, ch: _Chain, stream: int) -> None:
-        self._build(ch, 0, stream)
-        for t in range(self.T):
-            self._step(ch, t, stream)
-
     def _enqueue_persistent(self, n_steps: int, stream: int) -> None:
         env, ch = self.env, self.chains[0]
         rc = env.lib.gcbf_rollout_persistent(
@@ -204,22 +187,14 @@ class RolloutEngine:
         _lib.check(rc, "gcbf_rollout_persistent")
 
     def _enqueue_all(self) -> None:
-        dev = self.env.device
-        main = torch.cuda.current_stream(dev)
+        stream = torch.cuda.current_stream(self.env.device).cuda_stream
         if self.persistent:
-            self._enqueue_persistent(self.T, main.cuda_stream)
+            self._enqueue_persistent(self.T, stream)
             return
-        if len(self.chains) == 1:
-            self._enqueue_chain(self.chains[0], main.cuda_stream)
-            return
-        for ch in self.chains:                              # fork: parallel branches
-            if ch.stream is None:
-                ch.stream = torch.cuda.Stream(dev)
-            ch.stream.wait_stream(main)
-            with torch.cuda.stream(ch.stream):
-                self._enqueue_chain(ch, ch.stream.cuda_stream)
-        for ch in self.chains:                              # join
-            main.wait_stream(ch.stream)
+        ch = self.chains[0]
+        self._build(ch, 0, stream)
+        for t in range(self.T):
+            self._step(ch, t, stream)
 
     # ------------------------------------------------------------------ public
     def set_initial(self, agent0: torch.Tensor, goal: torch.Tensor, obstacle) -> None:
@@ -240,8 +215,8 @@ class RolloutEngine:
     def run(self, check: bool = True) -> None:
         """Run the T-step rollout from the current initial conditions (async)."""
         dev = self.env.device
-        for ch in self.chains:
-            ch.counters.zero_()
+        ch = self.chains[0]
+        ch.counters.zero_()
         lib = self.env.lib
         if self.use_cuda_graph:
             if self._graph is None:
@@ -249,11 +224,10 @@ class RolloutEngine:
                 st = torch.cuda.current_stream(dev).cuda_stream
                 if self.persistent:
                     self._enqueue_persistent(min(self.T, 1), st)
-                    self.chains[0].counters.zero_()
+                    ch.counters.zero_()
                 else:
-                    for ch in self.chains:
-                        self._build(ch, 0, st)
-                        self._step(ch, 0, st)
+                    self._build(ch, 0, st)
+                    self._step(ch, 0, st)
                 torch.cuda.synchronize(dev)
                 g = torch.cuda.CUDAGraph()
                 n0 = lib.gcbf_launch_count()
@@ -274,7 +248,7 @@ class RolloutEngine:
         device record once; call after run())."""
         if self.controller is None:
             raise RuntimeError("qp_stats() needs a CBF-QP baseline policy")
-        return iter_stats(torch.cat([ch.qp_iters.reshape(-1) for ch in self.chains]))
+        return iter_stats(self.chains[0].qp_iters.reshape(-1))
 
     def check_overflow(self) -> None:
         c = self.counters.cpu()
@@ -282,7 +256,7 @@ class RolloutEngine:
             cap = self._pdesc.edge_cap if self.persistent else self.desc.edge_cap
             raise RuntimeError(f"edge capacity overflow during rollout: up to {int(c[:, 0].max())} edges; edge_cap={cap}"
                                + (" split evenly over the environments / CTA pairs (persistent kernel)" if self.persistent
-                                  else " per chain") + "; raise env.edge_cap_per_agent")
+                                  else "") + "; raise env.edge_cap_per_agent")
 
     def result(self) -> Rollout:
         """trainer/data.py Rollout in the reference's (b, T) order (views/transposes of the record)."""

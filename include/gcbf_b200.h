@@ -383,10 +383,10 @@ int32_t gcbf_gemm_nn(int32_t epi, int32_t accum, const float* A, const float* B,
 /* gemm_tc: the wgmma tensor-core variant (3xTF32 split, fp32 accumulation in registers, TMA-staged
  * operands): C[M,N] = epi(A[M,K] @ Bt[N,K]^T) with Bt = the TRANSPOSED weight (K-major operands);
  * Bt is passed as its tf32 split Bt_hi + Bt_lo (gcbf_split_tf32; weights are split once per update);
- * same epilogues / row-count convention as gemm_nn, plus EPI_RELU_DOT (N == 128: C[m] = relu(acc + bias) . aux
- * + bias2[0]) and EPI_RELU_DOTN (C[(part * m_cap + m) * 4 + q] = relu(acc + bias) . aux[:, q] over the 128 columns of
- * column tile `part`, q < ndot <= 4, the other q written 0).  K % 32 == 0, N in {128, 256};
- * A must be backed by at least m_cap rows. */
+ * same epilogues / row-count convention as gemm_nn, plus EPI_RELU_DOTN = 5
+ * (C[(part * m_cap + m) * 4 + q] = relu(acc + bias) . aux[:, q] over the 128 columns of column tile `part`,
+ * q < ndot <= 4, the other q written 0); epi = 4 is not an epilogue and returns an error.
+ * K % 32 == 0, N in {128, 256}; A must be backed by at least m_cap rows. */
 int32_t gcbf_gemm_tc(int32_t epi, int32_t accum, const float* A, const float* Bt_hi, const float* Bt_lo,
                      const float* bias, const float* bias2, float* C, const float* aux,
                      const int32_t* m_ptr, int32_t m_fixed, int32_t m_cap, int32_t K, int32_t N, int32_t ndot,
