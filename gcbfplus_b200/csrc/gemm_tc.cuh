@@ -10,10 +10,11 @@
 //
 // CTA layout of the kernels here (288 threads): warps 0-7 are two consumer warpgroups, warpgroup g owning rows
 // [64 g, 64 g + 64) of a 128 x 128 output tile (one m64n128k8 accumulator: 64 registers per thread); warp 8 issues
-// the TMA loads.  The consumers split their own rows of A into tf32 hi / lo planes in shared memory (the weight planes
-// arrive pre-split), issue the MMAs -- the split of k-block kb + 1 overlaps the MMAs of k-block kb -- and run the
-// epilogue straight from the accumulator registers.  Persistent tile loop; M may come from a device counter (edge
-// count) so the launch is CUDA-graph friendly.  gemm_tn_tc_kernel (weight gradient) is described at its definition.
+// the TMA loads.  The consumers hold A in registers: each thread splits its own A fragment into tf32 hi / lo (the
+// weight planes arrive pre-split in shared memory) and feeds it to the register-A form of wgmma -- the split of k8
+// step j + 1 overlaps the MMAs of step j -- and runs the epilogue straight from the accumulator registers.
+// Persistent tile loop; M may come from a device counter (edge count) so the launch is CUDA-graph friendly.
+// gemm_tn_tc_kernel (weight gradient) is described at its definition.
 #pragma once
 #include <cuda.h>
 
@@ -32,7 +33,7 @@ constexpr int WK = 8;                     // tf32: 32 bytes of K per MMA
 constexpr int CONSUMERS = 256;            // two warpgroups
 constexpr int THREADS_NN = CONSUMERS + 32;
 constexpr int PLANE = BM * BK * 4;        // 16 KB: one hi or lo plane of a 128-row k-block
-constexpr int STG = 4 * PLANE;            // pipeline stage: A hi | A lo | B hi | B lo
+constexpr int STG = 4 * PLANE;            // pipeline stage: A (fp32) | (unused) | B hi | B lo
 constexpr int STAGES = 3;
 constexpr int WG_ROWS_BYTES = 64 * 128;   // the 64 rows of one warpgroup inside a plane
 
@@ -130,6 +131,27 @@ __device__ __forceinline__ void wgmma_tf32(float (&d)[64], uint64_t da, uint64_t
         : "l"(da), "l"(db), "r"(accumulate)
         : "memory");
 }
+// D[64 x 128] (+)= A[64 x 8] B[8 x 128], A (tf32 bit patterns) from registers, B from shared memory.  A fragment of
+// thread `lane` of warp w of the warpgroup (PTX ISA, wgmma .tf32 register fragment of A): a[0] = (row 16 w + lane / 4,
+// column lane % 4), a[1] = (row + 8, same column), a[2] = (same row, column + 4), a[3] = (row + 8, column + 4).  The
+// registers are read asynchronously: they must stay unchanged until a wgmma.wait_group retires the MMA.
+__device__ __forceinline__ void wgmma_tf32_rs(float (&d)[64], const uint32_t (&a)[4], uint64_t db, uint32_t accumulate) {
+    asm volatile(
+        "{\n"
+        ".reg .pred p;\n"
+        "setp.ne.b32 p, %69, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+        "{%64, %65, %66, %67}, %68, p, 1, 1;\n"
+        "}\n"
+        : GCBF_ACC8(0), GCBF_ACC8(8), GCBF_ACC8(16), GCBF_ACC8(24), GCBF_ACC8(32), GCBF_ACC8(40), GCBF_ACC8(48),
+          GCBF_ACC8(56)
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(accumulate)
+        : "memory");
+}
 #undef GCBF_ACC8
 
 // 12 MMAs of one 32-wide k-block of a 3xTF32 product (small terms first): a_* = the warpgroup's 64 rows, b_* = 128 rows
@@ -144,6 +166,21 @@ __device__ __forceinline__ void mma_kblock(float (&d)[64], uint32_t a_hi, uint32
     }
 }
 
+// The 3 MMAs of one k8 step of a 3xTF32 product, A from registers, in the order of mma_kblock: lo * Bhi, hi * Blo,
+// hi * Bhi.  b_hi / b_lo: shared-memory address of the k8 step's B columns (k-block plane + 32 bytes per k8 step).
+// The lo MMA and the two hi MMAs are committed as two groups, so the wg_wait<1> that follows in the main loops retires
+// the lo group of this step (and everything before it): the next step's fragment is then produced while only the 4 hi
+// registers of this step are in flight, which keeps the persistent rollout kernel within its 128 registers.
+__device__ __forceinline__ void mma_k8_rs(float (&d)[64], const uint32_t (&a_hi)[4], const uint32_t (&a_lo)[4],
+                                          uint32_t b_hi, uint32_t b_lo, bool first) {
+    wg_fence();                                // the fragment registers were just written
+    wgmma_tf32_rs(d, a_lo, make_desc(b_hi), first ? 0u : 1u);
+    wg_commit();
+    wgmma_tf32_rs(d, a_hi, make_desc(b_lo), 1u);
+    wgmma_tf32_rs(d, a_hi, make_desc(b_hi), 1u);
+    wg_commit();
+}
+
 // Accumulator fragment of an m64n128 wgmma: element i of thread t of the warpgroup (warp w = t / 32, lane l) holds
 // row 16 w + l / 4 + 8 ((i / 2) % 2), column 8 (i / 4) + 2 (l % 4) + i % 2.
 __device__ __forceinline__ int frag_row0(int wt) { return 16 * (wt >> 5) + ((wt & 31) >> 2); }
@@ -155,6 +192,15 @@ __device__ __forceinline__ float rn_tf32(float x) { return __uint_as_float((__fl
 __device__ __forceinline__ void split_tf32(const float4& v, float4& h, float4& l) {
     h.x = rn_tf32(v.x); h.y = rn_tf32(v.y); h.z = rn_tf32(v.z); h.w = rn_tf32(v.w);
     l.x = rn_tf32(v.x - h.x); l.y = rn_tf32(v.y - h.y); l.z = rn_tf32(v.z - h.z); l.w = rn_tf32(v.w - h.w);
+}
+// the same split of a register A fragment (wgmma_tf32_rs operands)
+__device__ __forceinline__ void split_frag(const float (&v)[4], uint32_t (&h)[4], uint32_t (&l)[4]) {
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+        const float x = rn_tf32(v[i]);
+        h[i] = __float_as_uint(x);
+        l[i] = __float_as_uint(rn_tf32(v[i] - x));
+    }
 }
 // byte offset of 16-byte chunk c (columns 4c .. 4c + 3 of a k-block) of row r in a K-major SWIZZLE_128B plane
 __device__ __forceinline__ int swz(int r, int c) { return r * 128 + ((c ^ (r & 7)) << 4); }
@@ -196,34 +242,38 @@ static __global__ void split_tf32_kernel(const float* __restrict__ in, float* __
     }
 }
 
-// Main loop of one 128 x 128 tile whose A arrives by TMA (stage layout A hi | A lo | B hi | B lo, A as plain fp32 in
-// the hi plane): warpgroup g splits its 64 rows of A into hi / lo in place, then issues the k-block's MMAs; the split
-// of k-block kb + 1 overlaps the MMAs of k-block kb.  `empty` counts the 256 consumer threads.
+// Main loop of one 128 x 128 tile whose A arrives by TMA (stage layout A | (unused) | B hi | B lo, A as plain fp32):
+// each consumer thread loads its A fragment of a k8 step from the fp32 tile -- for one k8 step the 8 rows of a quad
+// column sit in 8 distinct 16-byte chunks of the swizzled rows, so the loads are free of bank conflicts -- splits it
+// into tf32 hi / lo in registers and issues the step's 3 MMAs (mma_k8_rs): the split of step j + 1 overlaps the hi
+// MMAs of step j, and 12 A registers are live.  `empty` counts the 256 consumer threads.
 __device__ __forceinline__ void tma_a_mainloop(float (&d)[64], uint8_t* smem, uint64_t* full, uint64_t* empty,
                                                uint32_t& it, int nkb, int g, int wt) {
 #pragma unroll
     for (int i = 0; i < 64; ++i) d[i] = 0.f;
+    const int r = frag_row0(wt);               // fragment rows r, r + 8 of the warpgroup's 64; column wt % 4 (+ 4)
+    // byte offset of (row r, column wt % 4) in chunk 0 of the swizzled tile; chunk c is at off ^ (c << 4) (swz)
+    const uint32_t off = g * WG_ROWS_BYTES + swz(r, 0) + (wt & 3) * 4;
     for (int kb = 0; kb < nkb; ++kb, ++it) {
         const int s = it % STAGES;
         mbar_wait(&full[s], (it / STAGES) & 1);
-        uint8_t* st = smem + s * STG;
-        float4* h4 = reinterpret_cast<float4*>(st + g * WG_ROWS_BYTES);
-        float4* l4 = reinterpret_cast<float4*>(st + PLANE + g * WG_ROWS_BYTES);
+        // the chunk XOR is applied to the stage-dependent offset, so the 16 fragment addresses of a k-block are not
+        // loop-invariant registers
+        const uint32_t a = s * STG + off;
+        const uint32_t b_hi = smem_u32(smem + s * STG) + 2 * PLANE;
 #pragma unroll
-        for (int j = 0; j < 4; ++j) {          // the swizzle permutes chunks inside a row: split element-wise
-            float4 h, l;
-            split_tf32(h4[wt + 128 * j], h, l);
-            h4[wt + 128 * j] = h;
-            l4[wt + 128 * j] = l;
+        for (int k = 0; k < BK / WK; ++k) {
+            const uint32_t o0 = a ^ (2 * k << 4), o1 = a ^ ((2 * k + 1) << 4);
+            const float v[4] = {*reinterpret_cast<const float*>(smem + o0),
+                                *reinterpret_cast<const float*>(smem + o0 + 8 * 128),
+                                *reinterpret_cast<const float*>(smem + o1),
+                                *reinterpret_cast<const float*>(smem + o1 + 8 * 128)};
+            uint32_t ah[4], al[4];
+            split_frag(v, ah, al);
+            mma_k8_rs(d, ah, al, b_hi + k * WK * 4, b_hi + PLANE + k * WK * 4, kb == 0 && k == 0);
+            wg_wait<1>();                      // all but this step's hi MMAs retired; at k = 0 that includes the last
+            if (k == 0 && kb > 0) mbar_arrive(&empty[(it - 1) % STAGES]);   // MMAs of k-block kb - 1
         }
-        fence_async_smem();
-        bar_wg(g);
-        wg_fence();
-        const uint32_t a_hi = smem_u32(st) + g * WG_ROWS_BYTES;
-        mma_kblock(d, a_hi, a_hi + PLANE, smem_u32(st) + 2 * PLANE, smem_u32(st) + 3 * PLANE, kb == 0);
-        wg_commit();
-        wg_wait<1>();                          // k-block kb - 1 retired: release its stage
-        if (kb > 0) mbar_arrive(&empty[(it - 1) % STAGES]);
     }
     wg_wait<0>();
     mbar_arrive(&empty[(it - 1) % STAGES]);

@@ -4,9 +4,8 @@
 //   A[e, :] = relu(feat_e @ W1[:ed] + W1[ed + sender_type] + W1[ed+3+2] + b1)   (edge_l1_kernel)
 //   feat_e from agent / goal / hit states through the receiver-grouped edge lists
 //
-// The consumer warpgroups compute their rows' 32 columns per k-block (two threads per row, 16 columns each), split
-// them into the tf32 hi / lo planes and store them straight into the SWIZZLE_128B K-major layout the MMA descriptor
-// expects (16-byte chunk c of row r lives at r*128 + ((c ^ (r & 7)) * 16)); B (weights, pre-split) arrives by TMA.
+// Each consumer thread computes the elements of its own register A fragment (two edge rows, 4 columns per k8 step),
+// splits them into tf32 hi / lo and feeds them to the register-A form of wgmma; B (weights, pre-split) arrives by TMA.
 #pragma once
 #include "gemm_tc.cuh"
 #include "gnn.cuh"
@@ -35,40 +34,42 @@ struct ChainArgs {
 
 constexpr int L1_FLOATS = 9 * 256;   // message layer 1 in shared memory: W1[:ED] and the per-sender-type bias rows
 
-// W1[:ED] and the per-sender-type bias table sW[(ED + t) * 256 + c] = W1[ED + t] + W1[ED + 3 + 2] + b1
+// Position of column c in a row of the layer-1 table: inside each group of 8 columns, c and c + 4 are neighbours
+// (8 a + 4 h + j -> 8 a + 2 j + h), so the two columns of a k8 step's A fragment are one 8-byte load.
+__device__ __forceinline__ int l1_pos(int c) { return (c & ~7) | ((c & 3) << 1) | ((c >> 2) & 1); }
+
+// W1[:ED] and the per-sender-type bias table sW[(ED + t) * 256 + l1_pos(c)] = W1[ED + t] + W1[ED + 3 + 2] + b1
 template <int ED>
 __device__ __forceinline__ void load_l1_table(float* sW, const float* W1, const float* b1, int tid, int nthreads) {
-    for (int i = tid; i < ED * 256; i += nthreads) sW[i] = W1[i];
+    for (int i = tid; i < ED * 256; i += nthreads) sW[(i & ~255) + l1_pos(i & 255)] = W1[i];
     for (int i = tid; i < 3 * 256; i += nthreads) {
         const int t = i / 256, c = i % 256;
-        sW[(ED + t) * 256 + c] = W1[(ED + t) * 256 + c] + W1[(ED + 3 + 2) * 256 + c] + b1[c];
+        sW[(ED + t) * 256 + l1_pos(c)] = W1[(ED + t) * 256 + c] + W1[(ED + 3 + 2) * 256 + c] + b1[c];
     }
 }
 
-// message layer 1 of k-block kb, 16-byte chunks 4 half .. 4 half + 3 of tile row r -> hi / lo planes of stage `st`
+// message layer 1 at columns n0 + j and n0 + j + 4 (n0 = 8 k8-steps, j = lane % 4) of the thread's two fragment rows
+// (features f[h], sender-type table row bias[h], h = 0: row frag_row0, h = 1: row + 8; rows that are not ok give 0)
+// -> the tf32 hi / lo register A fragment of that k8 step
 template <int ED>
-__device__ __forceinline__ void produce_l1_kblock(uint8_t* st, int r, int half, int kb, bool row_ok, const float* sW,
-                                                  const float (&f)[ED], int stype) {
+__device__ __forceinline__ void produce_l1_k8(uint32_t (&ah)[4], uint32_t (&al)[4], int n0, int j, const bool (&ok)[2],
+                                              const float* sW, const float* const (&bias)[2], const float (&f)[2][ED]) {
+    const int p = n0 + 2 * j;                  // l1_pos(n0 + j); l1_pos(n0 + j + 4) = p + 1
+    float2 y[2];
 #pragma unroll
-    for (int cc = 0; cc < 4; ++cc) {
-        const int c = half * 4 + cc;
-        float v[4] = {0.f, 0.f, 0.f, 0.f};
-        if (row_ok) {
-            const int n = kb * BK + c * 4;
+    for (int h = 0; h < 2; ++h) y[h] = *reinterpret_cast<const float2*>(bias[h] + p);
 #pragma unroll
-            for (int j = 0; j < 4; ++j) {
-                float y = sW[(ED + stype) * 256 + n + j];
+    for (int q = 0; q < ED; ++q) {
+        const float2 w = *reinterpret_cast<const float2*>(sW + q * 256 + p);
 #pragma unroll
-                for (int q = 0; q < ED; ++q) y = fmaf(f[q], sW[q * 256 + n + j], y);
-                v[j] = fmaxf(y, 0.f);
-            }
+        for (int h = 0; h < 2; ++h) {
+            y[h].x = fmaf(f[h][q], w.x, y[h].x);
+            y[h].y = fmaf(f[h][q], w.y, y[h].y);
         }
-        float4 h, l;
-        split_tf32(make_float4(v[0], v[1], v[2], v[3]), h, l);
-        const int off = swz(r, c);
-        *reinterpret_cast<float4*>(st + off) = h;
-        *reinterpret_cast<float4*>(st + PLANE + off) = l;
     }
+    const float v[4] = {ok[0] ? fmaxf(y[0].x, 0.f) : 0.f, ok[1] ? fmaxf(y[1].x, 0.f) : 0.f,
+                        ok[0] ? fmaxf(y[0].y, 0.f) : 0.f, ok[1] ? fmaxf(y[1].y, 0.f) : 0.f};
+    split_frag(v, ah, al);
 }
 
 // message tile of warpgroup g -> global rows (bias added; tile row r lands at msg + r * 128, rows >= n_valid skipped)
@@ -119,27 +120,41 @@ __device__ __forceinline__ void edge_row_setup(const ProdArgs& pa, int m, bool r
     }
 }
 
-// main loop of an edge tile: 8 k-blocks of message layer 1 produced in-kernel x W23 (K = 256, N = 128)
+// Row set-up of the two fragment rows of a thread (h = 0: frag_row0, h = 1: + 8): lanes 4 i, 4 i + 1 of a quad set up
+// row h = 0, lanes 4 i + 2, 4 i + 3 row h = 1 (setup_row), and share_rows hands both to the whole quad.
+__device__ __forceinline__ int setup_row(int lane) { return (lane >> 1) & 1; }
+template <int ED>
+__device__ __forceinline__ void share_rows(const float (&fs)[ED], int ss, int lane, float (&f)[2][ED], int (&stype)[2]) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        const int src = (lane & ~3) | (2 * h);
+#pragma unroll
+        for (int q = 0; q < ED; ++q) f[h][q] = __shfl_sync(0xffffffffu, fs[q], src);
+        stype[h] = __shfl_sync(0xffffffffu, ss, src);
+    }
+}
+
+// main loop of an edge tile: 8 k-blocks of message layer 1 produced in-kernel x W23 (K = 256, N = 128), one k8 step
+// at a time as in tma_a_mainloop; the first k8 step of a k-block is produced before the wait for its weights
 template <int ED>
 __device__ __forceinline__ void edge_tile_mainloop(float (&d)[64], uint8_t* smem, uint64_t* full, uint64_t* empty,
-                                                   uint32_t& it, int g, int r, int half, bool row_ok, const float* sW,
-                                                   const float (&f)[ED], int stype) {
+                                                   uint32_t& it, int lane, const bool (&ok)[2], const float* sW,
+                                                   const float (&f)[2][ED], const int (&stype)[2]) {
+    const float* const bias[2] = {sW + (ED + stype[0]) * 256, sW + (ED + stype[1]) * 256};
 #pragma unroll
     for (int i = 0; i < 64; ++i) d[i] = 0.f;
     for (int kb = 0; kb < 8; ++kb, ++it) {
         const int s = it % STAGES;
-        uint8_t* st = smem + s * STG;
-        // this warpgroup's MMAs of the stage's previous use have retired (program order): its A rows are free
-        produce_l1_kblock<ED>(st, r, half, kb, row_ok, sW, f, stype);
-        fence_async_smem();
-        bar_wg(g);
-        mbar_wait(&full[s], (it / STAGES) & 1);
-        wg_fence();
-        const uint32_t a_hi = smem_u32(st) + g * WG_ROWS_BYTES;
-        mma_kblock(d, a_hi, a_hi + PLANE, smem_u32(st) + 2 * PLANE, smem_u32(st) + 3 * PLANE, kb == 0);
-        wg_commit();
-        wg_wait<1>();
-        if (kb > 0) mbar_arrive(&empty[(it - 1) % STAGES]);
+        const uint32_t b_hi = smem_u32(smem + s * STG) + 2 * PLANE;
+#pragma unroll
+        for (int k = 0; k < BK / WK; ++k) {
+            uint32_t ah[4], al[4];
+            produce_l1_k8<ED>(ah, al, kb * BK + k * WK, lane & 3, ok, sW, bias, f);
+            if (k == 0) mbar_wait(&full[s], (it / STAGES) & 1);
+            mma_k8_rs(d, ah, al, b_hi + k * WK * 4, b_hi + PLANE + k * WK * 4, kb == 0 && k == 0);
+            wg_wait<1>();                      // all but this step's hi MMAs retired; at k = 0 that includes the last
+            if (k == 0 && kb > 0) mbar_arrive(&empty[(it - 1) % STAGES]);   // MMAs of k-block kb - 1
+        }
     }
     wg_wait<0>();
     mbar_arrive(&empty[(it - 1) % STAGES]);
@@ -212,15 +227,18 @@ edge_chain_kernel(const __grid_constant__ CUtensorMap tmBh, const __grid_constan
         return;
     }
     const int g = warp >> 2, wt = threadIdx.x & 127;
-    const int r = 64 * g + (wt & 63), half = wt >> 6;
+    const int r = 64 * g + frag_row0(wt);      // the thread's fragment rows r, r + 8 of the tile
+    const int rs = r + 8 * setup_row(lane);    // ... and the one it sets up
     uint32_t it = 0, tc_ = 0;
     for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++tc_) {
         const int m0 = tile * BM;
-        float f[ED];
-        int stype;
-        edge_row_setup<KIND>(pa, m0 + r, m0 + r < M, f, stype);
+        float fs[ED], f[2][ED];
+        int ss, stype[2];
+        edge_row_setup<KIND>(pa, m0 + rs, m0 + rs < M, fs, ss);
+        share_rows<ED>(fs, ss, lane, f, stype);
+        const bool ok[2] = {m0 + r < M, m0 + r + 8 < M};
         float d[64];
-        edge_tile_mainloop<ED>(d, smem, full, empty, it, g, r, half, m0 + r < M, sW, f, stype);
+        edge_tile_mainloop<ED>(d, smem, full, empty, it, lane, ok, sW, f, stype);
         mbar_arrive(main_done);
         bar_consumers();                       // both warpgroups' main loops retired: the hand-over may overwrite stages 0-1
         drain_msg(d, smem, g, wt, bias, C + (size_t)m0 * 128, M - m0);
@@ -246,7 +264,6 @@ edge_chain_kernel(const __grid_constant__ CUtensorMap tmBh, const __grid_constan
             if (rr + 8 < M) ch.logits[rr + 8] = q[1][0] + ch.cst[0];
         }
         mbar_arrive(t2f);
-        bar_consumers();                       // the gate slots (stage 2) are drained before the next tile's A rows land there
     }
 }
 

@@ -149,15 +149,14 @@ rollout_persist_kernel(const __grid_constant__ PArgs P, const __grid_constant__ 
     const int env = blockIdx.x / C;
     const int L = soft ? 2 : C;                      // CTAs per LOCAL group = hardware cluster size
     const int lrank = rank % L, grp = rank / L;      // (cluster rank, group inside the environment)
-    unsigned n_sync = 0;          // environment barriers passed so far (pair mode: arrival target = n_sync * C)
     // SYNC_LOCAL: barrier of the hardware cluster (the CTAs that share edge rows / agent tiles).
-    // SYNC_ENV: all C CTAs of the environment (mode 0: the same cluster barrier; pair mode: software barrier).
+    // SYNC_ENV(n): all C CTAs of the environment (mode 0: the same cluster barrier; pair mode: software barrier), the
+    // n-th environment barrier of the rollout (pair mode: arrival target n * C).  It runs once per env-step.
 #define SYNC_LOCAL() cluster_sync_all()
-#define SYNC_ENV()                                                     \
+#define SYNC_ENV(n)                                                    \
     do {                                                               \
         if (soft) {                                                    \
-            ++n_sync;                                                  \
-            soft_group_sync(P.gbar + env, n_sync * (unsigned)C);       \
+            soft_group_sync(P.gbar + env, (n) * (unsigned)C);          \
         } else {                                                       \
             cluster_sync_all();                                        \
         }                                                              \
@@ -187,12 +186,7 @@ rollout_persist_kernel(const __grid_constant__ PArgs P, const __grid_constant__ 
         mbar_init(&bars[B_T2F], CONSUMERS);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    // message layer 1: W1[:ED] and the per-sender-type bias table (tc::load_l1_table layout)
-    for (int i = tid; i < ED * 256; i += PT) sW[i] = P.W1[i];
-    for (int i = tid; i < 3 * 256; i += PT) {
-        const int t = i / 256, c = i % 256;
-        sW[(ED + t) * 256 + c] = P.W1[(ED + t) * 256 + c] + P.W1[(ED + 3 + 2) * 256 + c] + P.b1[c];
-    }
+    load_l1_table<ED>(sW, P.W1, P.b1, tid, PT);    // message layer 1: W1[:ED] and the per-sender-type bias table
     auto stage = [&](int off, const float* src, int n) {
         for (int i = tid; i < n; i += PT) sk[off + i] = src[i];
     };
@@ -261,20 +255,21 @@ rollout_persist_kernel(const __grid_constant__ PArgs P, const __grid_constant__ 
                     }
                 }
             } else if (warp >= 8) {
-                // consumer warpgroups (warps 8..15): PRODUCE the A operand of the tile (two threads per edge row, 16 of
-                // the 32 columns of a k-block each: features + message layer 1, tf32 hi / lo split, swizzled K-major),
-                // issue the MMAs, drain the message tile (global + shared-memory hand-over), run the chained gate GEMM
-                // and turn it into the gate logits -- the code of tc::edge_chain_kernel, so the two paths give the same bits
+                // consumer warpgroups (warps 8..15): PRODUCE the A operand of the tile in registers (each thread the
+                // fragment of two edge rows: features + message layer 1, tf32 hi / lo split), issue the MMAs, drain the
+                // message tile (global + shared-memory hand-over), run the chained gate GEMM and turn it into the gate
+                // logits -- the code of tc::edge_chain_kernel, so the two paths give the same bits
                 const int g = (warp - 8) >> 2, wt = tid & 127;
-                const int r = 64 * g + (wt & 63), half = wt >> 6;
+                const int r = 64 * g + frag_row0(wt);          // the thread's fragment rows r, r + 8 of the tile
+                const int rs = r + 8 * setup_row(lane);         // ... and the one it sets up (tc::share_rows)
                 uint32_t it_l = it, ne_l = ne;
                 for (int tile = lrank; tile < n_tiles; tile += L, ++ne_l) {
-                    const int ml = tile * BM + r;
+                    const int ml = tile * BM + rs;
                     const bool row_ok = ml < M_cur;
-                    float f[ED];
-                    int stype = 0;
+                    float fs[ED], f[2][ED];
+                    int ss = 0, stype[2];
 #pragma unroll
-                    for (int c = 0; c < ED; ++c) f[c] = 0.f;
+                    for (int c = 0; c < ED; ++c) fs[c] = 0.f;
                     if (row_ok) {
                         const int a = min(max(er_t[seg_e0 + ml], env_a0), env_a0 + N - 1);
                         const int code = min(es_t[seg_e0 + ml], env_a0 + N - 1);
@@ -284,11 +279,13 @@ rollout_persist_kernel(const __grid_constant__ PArgs P, const __grid_constant__ 
                         edge_state_dev<KIND>(sst + (size_t)(a - env_a0) * SD, er);
                         if (code >= 0) edge_state_dev<KIND>(sst + (size_t)(max(code, env_a0) - env_a0) * SD, es);
                         else sender_state_dev<KIND>(code, a, R, agent_t, P.goal, hits_t, es);
-                        edge_feat_dev<KIND>(er, es, code == -1, d.comm_radius, f, &coef, &nrm);
-                        stype = (code >= 0) ? 2 : ((code == -1) ? 1 : 0);
+                        edge_feat_dev<KIND>(er, es, code == -1, d.comm_radius, fs, &coef, &nrm);
+                        ss = (code >= 0) ? 2 : ((code == -1) ? 1 : 0);
                     }
+                    share_rows<ED>(fs, ss, lane, f, stype);
+                    const bool ok[2] = {tile * BM + r < M_cur, tile * BM + r + 8 < M_cur};
                     float dacc[64];
-                    edge_tile_mainloop<ED>(dacc, smem, &bars[B_FULL], &bars[B_EMPTY], it_l, g, r, half, row_ok, sW, f, stype);
+                    edge_tile_mainloop<ED>(dacc, smem, &bars[B_FULL], &bars[B_EMPTY], it_l, lane, ok, sW, f, stype);
                     mbar_arrive(&bars[B_MAIN]);
                     bar_consumers();               // both main loops retired: the hand-over may overwrite stages 0-1
                     drain_msg(dacc, smem, g, wt, sk + K_B23, P.msg + (seg_e0 + (size_t)tile * BM) * 128, M_cur - tile * BM);
@@ -314,7 +311,6 @@ rollout_persist_kernel(const __grid_constant__ PArgs P, const __grid_constant__ 
                         if (rr + 8 < M_cur) P.logit[seg_e0 + rr + 8] = q[1][0] + sk[K_CST];
                     }
                     mbar_arrive(&bars[B_T2F]);
-                    bar_consumers();               // the gate slots (stage 2) are drained before the next tile's A rows land
                 }
             }
             it += 8u * my_tiles;
@@ -402,7 +398,7 @@ rollout_persist_kernel(const __grid_constant__ PArgs P, const __grid_constant__ 
                 it += (uint32_t)nkb * my_items;
                 if (ph2 == 0) fence_async_global();   // V1 rows (generic stores) -> TMA reads of phase U2
                 if (ph2 == 0) SYNC_LOCAL();
-                else SYNC_ENV();                      // the policy tail needs the output sums of EVERY agent
+                else SYNC_ENV((unsigned)t + 1u);      // the policy tail needs the output sums of EVERY agent
                 if (stamp) pr[3 + ph2] = gtime();
             }
         }
