@@ -47,10 +47,19 @@ _SIGNATURES = {
     "gcbf_launch_count": (C.c_int64, []),
     "gcbf_param_count": (C.c_int32, [C.c_int32, C.c_int32]),
     "gcbf_param_offsets": (C.c_int32, [C.c_int32, C.c_int32, C.POINTER(C.c_int32)]),
+    "gcbf_param_count_l": (C.c_int32, [C.c_int32, C.c_int32, C.c_int32]),
+    "gcbf_param_offsets_l": (C.c_int32, [C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_int32)]),
     "gcbf_graph_build": (C.c_int32, [C.POINTER(EnvDesc)] + [_P] * 9 + [C.c_int32, _P]),
     "gcbf_gnn_workspace_floats": (C.c_int64, [C.POINTER(EnvDesc), C.c_int32]),
     "gcbf_gnn_forward": (C.c_int32, [C.POINTER(EnvDesc), C.c_int32, C.c_int32] + [_P] * 10 + [C.c_int32, _P, _P,
                                      C.c_int64, _P]),
+    "gcbf_gnn_workspace_floats_l": (C.c_int64, [C.POINTER(EnvDesc), C.c_int32, C.c_int32]),
+    "gcbf_gnn_forward_l": (C.c_int32, [C.POINTER(EnvDesc), C.c_int32, C.c_int32, C.c_int32] + [_P] * 10 +
+                           [C.c_int32, _P, _P, C.c_int64, _P]),
+    "gcbf_params_t_count_l": (C.c_int32, [C.c_int32, C.c_int32, C.c_int32]),
+    "gcbf_prepare_params_l": (C.c_int32, [C.c_int32, C.c_int32, C.c_int32, _P, _P, _P]),
+    "gcbf_rollout_workspace_floats_l": (C.c_int64, [C.POINTER(EnvDesc), C.c_int32]),
+    "gcbf_rollout_step_l": (C.c_int32, [C.POINTER(EnvDesc), C.c_int32, _P, _P, C.c_int32] + [_P] * 21 + [C.c_int64, _P]),
     "gcbf_infer_count": (C.c_int32, [C.c_int32, C.c_int32]),
     "gcbf_prepare_infer": (C.c_int32, [C.c_int32, C.c_int32, _P, _P, _P]),
     "gcbf_gnn_infer": (C.c_int32, [C.POINTER(EnvDesc), C.c_int32, C.c_int32, _P, _P, C.c_int32] + [_P] * 8 +
@@ -157,9 +166,14 @@ def sqrt_threshold(r: float) -> float:
     return float(a)
 
 
-def param_offsets(edge_dim: int, out_dim: int):
-    arr = (C.c_int32 * 24)()
-    check(load().gcbf_param_offsets(edge_dim, out_dim, arr), "gcbf_param_offsets")
+def param_offsets(edge_dim: int, out_dim: int, n_layers: int = 1):
+    """W, b offsets of the Dense layers in forward order (gcbf_param_offsets_l): 2 * (9 n_layers + 3) entries."""
+    if n_layers == 1:
+        arr = (C.c_int32 * 24)()
+        check(load().gcbf_param_offsets(edge_dim, out_dim, arr), "gcbf_param_offsets")
+        return list(arr)
+    arr = (C.c_int32 * (2 * (9 * n_layers + 3)))()
+    check(load().gcbf_param_offsets_l(edge_dim, out_dim, n_layers, arr), "gcbf_param_offsets_l")
     return list(arr)
 
 
@@ -168,8 +182,8 @@ def param_offsets(edge_dim: int, out_dim: int):
 USE_TC = os.environ.get("GCBF_TENSOR_CORES", "1") != "0"
 
 
-def param_count(edge_dim: int, out_dim: int) -> int:
-    n = load().gcbf_param_count(edge_dim, out_dim)
+def param_count(edge_dim: int, out_dim: int, n_layers: int = 1) -> int:
+    n = load().gcbf_param_count_l(edge_dim, out_dim, n_layers)
     if n <= 0:
-        raise RuntimeError("gcbf_param_count: bad dims")
+        raise RuntimeError(f"gcbf_param_count_l: bad dims (edge_dim {edge_dim}, out_dim {out_dim}, n_layers {n_layers})")
     return int(n)

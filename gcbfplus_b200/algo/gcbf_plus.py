@@ -29,8 +29,8 @@ class GCBFPlus(MultiAgentController):
                  max_grad_norm: float = 2.0, seed: int = 0, **kwargs):
         """Same kwargs as gcbf_plus.py:36-60."""
         super().__init__(env=env, node_dim=node_dim, edge_dim=edge_dim, action_dim=action_dim, n_agents=n_agents)
-        if gnn_layers != 1:
-            raise NotImplementedError("the sm_90a path implements gnn_layers=1 (train.py default, all pretrained models)")
+        if gnn_layers < 1:
+            raise ValueError(f"gnn_layers must be >= 1, got {gnn_layers}")
         self.batch_size = batch_size
         self.buffer_size = buffer_size
         self.lr_actor = lr_actor
@@ -49,9 +49,10 @@ class GCBFPlus(MultiAgentController):
         self.state_dim = state_dim
         dev = env.device
         # gcbf_plus.py:98-133: cbf, target cbf (copy), actor; xavier-uniform init (NumPy PCG64 stream)
-        self.cbf_params = NetParams(edge_dim, 1, "cbf", device=dev).init_xavier(seed * 2 + 1)
+        self.cbf_params = NetParams(edge_dim, 1, "cbf", device=dev, n_layers=gnn_layers).init_xavier(seed * 2 + 1)
         self.cbf_tgt_params = self.cbf_params.clone()
-        self.actor_net_params = NetParams(edge_dim, action_dim, "actor", device=dev).init_xavier(seed * 2 + 2)
+        self.actor_net_params = NetParams(edge_dim, action_dim, "actor", device=dev,
+                                          n_layers=gnn_layers).init_xavier(seed * 2 + 2)
         self.runner = GnnRunner(env)
         self.rng = np.random.default_rng(seed=seed + 1)       # gcbf_plus.py:139
         self._trainer_state = None                            # lazily built by update() (algo/train.py)

@@ -4,6 +4,8 @@ Layout of one network (CBF or actor) = the 12 Dense layers in forward order
 (gcbfplus/nn/gnn.py:44-104, algo/module/cbf.py:12-53, algo/module/policy.py:63-128;
 names per SURVEY A.3), kernel [in, out] row-major then bias, each 16-byte aligned;
 offsets come from libgcbf_b200 (gcbf_param_offsets) so C and Python cannot drift.
+With n_layers GNN layers (gnn.py:78-104) the 9 Dense layers of GNNLayer_0 .. GNNLayer_<n-1> come first, then the
+head (gcbf_param_offsets_l).
 Checkpoints keep the reference format: pickle of {'params': nested dict} with NumPy leaves
 (gcbfplus/algo/gcbf.py:344-357); the reference's own pickles (jax.Array leaves) load
 through a stub unpickler, no JAX needed.
@@ -20,14 +22,21 @@ import torch
 from .. import _lib
 
 
-def layer_specs(edge_dim: int, out_dim: int, kind: str) -> List[Tuple[str, int, int]]:
-    g = "params/GNN_0/GNNLayer_0/"
+def layer_specs(edge_dim: int, out_dim: int, kind: str, n_layers: int = 1) -> List[Tuple[str, int, int]]:
+    """(flax path, in, out) in forward order.  Layer 0 reads the 3-wide one-hot node types; every later layer reads the
+    previous layer's 128-wide output, so its msg/Dense_0 is [ed + 256, 256] and its update/Dense_0 [256, 256]."""
+    specs = []
+    for l in range(n_layers):
+        g = f"params/GNN_0/GNNLayer_{l}/"
+        nd = 3 if l == 0 else 128
+        specs += [
+            (g + "msg/Dense_0", edge_dim + 2 * nd, 256), (g + "msg/Dense_1", 256, 256), (g + "Dense_0", 256, 128),
+            (g + "attn/Dense_0", 128, 128), (g + "attn/Dense_1", 128, 128), (g + "Dense_1", 128, 1),
+            (g + "update/Dense_0", nd + 128, 256), (g + "update/Dense_1", 256, 256), (g + "Dense_2", 256, 128),
+        ]
     head = "CBFHead" if kind == "cbf" else "PolicyHead"
     last = "Dense_0" if kind == "cbf" else "OutputDense"
-    return [
-        (g + "msg/Dense_0", edge_dim + 6, 256), (g + "msg/Dense_1", 256, 256), (g + "Dense_0", 256, 128),
-        (g + "attn/Dense_0", 128, 128), (g + "attn/Dense_1", 128, 128), (g + "Dense_1", 128, 1),
-        (g + "update/Dense_0", 131, 256), (g + "update/Dense_1", 256, 256), (g + "Dense_2", 256, 128),
+    return specs + [
         (f"params/{head}/Dense_0", 128, 256), (f"params/{head}/Dense_1", 256, 256),
         (f"params/{last}", 256, out_dim),
     ]
@@ -77,12 +86,12 @@ def load_pickle(path: str) -> dict:
 class NetParams:
     """One network's parameters as a flat fp32 device buffer."""
 
-    def __init__(self, edge_dim: int, out_dim: int, kind: str, device="cuda"):
+    def __init__(self, edge_dim: int, out_dim: int, kind: str, device="cuda", n_layers: int = 1):
         assert kind in ("cbf", "actor")
-        self.edge_dim, self.out_dim, self.kind = edge_dim, out_dim, kind
-        self.specs = layer_specs(edge_dim, out_dim, kind)
-        self.offsets = _lib.param_offsets(edge_dim, out_dim)
-        self.count = _lib.param_count(edge_dim, out_dim)
+        self.edge_dim, self.out_dim, self.kind, self.n_layers = edge_dim, out_dim, kind, n_layers
+        self.specs = layer_specs(edge_dim, out_dim, kind, n_layers)
+        self.offsets = _lib.param_offsets(edge_dim, out_dim, n_layers)
+        self.count = _lib.param_count(edge_dim, out_dim, n_layers)
         self.flat = torch.zeros(self.count, dtype=torch.float32, device=device)
         self._flat_t = None   # transposed GEMM weights for the tensor-core path (gcbf_prepare_params)
 
@@ -93,12 +102,12 @@ class NetParams:
             return None
         lib = _lib.load()
         if self._flat_t is None:
-            n = lib.gcbf_params_t_count(self.edge_dim, self.out_dim)
+            n = lib.gcbf_params_t_count_l(self.edge_dim, self.out_dim, self.n_layers)
             self._flat_t = torch.empty(int(n), dtype=torch.float32, device=self.flat.device)
         if stream is None:
             stream = torch.cuda.current_stream(self.flat.device).cuda_stream
-        _lib.check(lib.gcbf_prepare_params(self.edge_dim, self.out_dim, _lib.ptr(self.flat), _lib.ptr(self._flat_t),
-                                           stream), "gcbf_prepare_params")
+        _lib.check(lib.gcbf_prepare_params_l(self.edge_dim, self.out_dim, self.n_layers, _lib.ptr(self.flat),
+                                             _lib.ptr(self._flat_t), stream), "gcbf_prepare_params_l")
         return self._flat_t
 
     # ---- init (nn/utils.py:21 xavier_uniform kernels, zero biases) ----
@@ -115,6 +124,10 @@ class NetParams:
     # ---- nested dict <-> flat ----
     def from_tree(self, tree: dict) -> "NetParams":
         flat = flatten_tree(tree)
+        known = {path for path, _, _ in self.specs}
+        extra = sorted({k.rsplit("/", 1)[0] for k in flat if "/GNNLayer_" in k} - known)
+        if extra:   # a deeper network's checkpoint: loading its first layers only would silently drop the rest
+            raise ValueError(f"checkpoint has GNN layers this {self.n_layers}-layer network lacks: {extra[0]} ...")
         host = np.zeros(self.count, dtype=np.float32)
         for i, (path, fi, fo) in enumerate(self.specs):
             w = np.asarray(flat[path + "/kernel"], dtype=np.float32)
@@ -138,7 +151,7 @@ class NetParams:
         return sum(fi * fo + fo for _, fi, fo in self.specs)
 
     def clone(self) -> "NetParams":
-        out = NetParams(self.edge_dim, self.out_dim, self.kind, device=self.flat.device)
+        out = NetParams(self.edge_dim, self.out_dim, self.kind, device=self.flat.device, n_layers=self.n_layers)
         out.flat.copy_(self.flat)
         return out
 

@@ -271,6 +271,7 @@ def update(algo, rollout: Rollout, step: int) -> dict:
     with the replay kept on the device (SURVEY 8f2).  Action labels: the CBF-QP of every graph in the
     batch, solved on the device with the TARGET cbf (get_b_u_qp, :193-213) -- `batch_u_qp`."""
     env = algo._env
+    require_one_layer(algo.cbf_params.n_layers, "update()")
     if algo._trainer_state is None:
         algo._trainer_state = TrainState(algo)
     if not hasattr(algo, "buffer"):
@@ -324,6 +325,14 @@ def update(algo, rollout: Rollout, step: int) -> dict:
     return info
 
 
+def require_one_layer(n_layers: int, what: str) -> None:
+    """The train step's backward and the QP labels' Lie-derivative Jacobian are one-hop (one GNN layer); deeper networks
+    run forward only (rollouts, evaluation, h / pi)."""
+    if n_layers != 1:
+        raise NotImplementedError(f"{what} implements gnn_layers = 1, got {n_layers} GNN layers "
+                                  "(forward, rollout and evaluation support any depth)")
+
+
 def batch_u_ref(algo, batch) -> torch.Tensor:
     env = algo._env
     n = batch["agent"].shape[0]
@@ -346,6 +355,7 @@ def qp_labels(algo, graph: SwarmGraph, params=None, with_aux: bool = False, max_
     A graph whose count equals max_iter stopped at the cap (its label is the capped iterate)."""
     env = algo._env
     lib = env.lib
+    require_one_layer((params or algo.cbf_tgt_params).n_layers, "the CBF-QP labels")
     G, N = graph.n_graphs, env.num_agents
     d = env.desc(G, 0, edge_cap=graph.edge_recv.numel())
     cache = algo.__dict__.setdefault("_qp_ws", {})
@@ -388,6 +398,7 @@ def batch_u_qp(algo, batch, agents_per_chunk: int = 32768, info: Optional[dict] 
     largest per-graph edge count (`graph/max_edges`, sizes the minibatch edge lists exactly) and ORs the
     edge-capacity overflow flags of the chunk graphs; an overflow doubles env.edge_cap_per_agent and relabels."""
     env = algo._env
+    require_one_layer(algo.cbf_tgt_params.n_layers, "the CBF-QP labels")
     if algo._trainer_state is None:
         algo._trainer_state = TrainState(algo)
     ts: TrainState = algo._trainer_state

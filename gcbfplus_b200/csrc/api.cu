@@ -61,3 +61,31 @@ extern "C" __attribute__((visibility("default"))) int32_t gcbf_param_offsets(int
     }
     return 0;
 }
+
+extern "C" __attribute__((visibility("default"))) int32_t gcbf_param_count_l(int32_t edge_dim, int32_t out_dim,
+                                                                             int32_t n_layers) {
+    if (edge_dim < 1 || edge_dim > 6 || out_dim < 1 || out_dim > 4 || n_layers < 1 || n_layers > gcbf::GCBF_MAX_LAYERS)
+        return -1;
+    return gcbf::make_deep_layout(edge_dim, out_dim, n_layers).total;
+}
+
+extern "C" __attribute__((visibility("default"))) int32_t gcbf_param_offsets_l(int32_t edge_dim, int32_t out_dim,
+                                                                               int32_t n_layers, int32_t* off) {
+    if (edge_dim < 1 || edge_dim > 6 || out_dim < 1 || out_dim > 4 || n_layers < 1 ||
+        n_layers > gcbf::GCBF_MAX_LAYERS || !off) {
+        gcbf::set_error("gcbf_param_offsets_l: bad argument");
+        return -1;
+    }
+    const gcbf::DeepLayout D = gcbf::make_deep_layout(edge_dim, out_dim, n_layers);
+    int k = 0;
+    for (int l = 0; l < n_layers; ++l)
+        for (int i = 0; i < gcbf::L_HEAD0; ++i) {
+            off[k++] = D.layer[l].w[i];
+            off[k++] = D.layer[l].b[i];
+        }
+    for (int i = gcbf::L_HEAD0; i <= gcbf::L_OUT; ++i) {
+        off[k++] = D.layer[0].w[i];
+        off[k++] = D.layer[0].b[i];
+    }
+    return 0;
+}

@@ -89,6 +89,49 @@ inline ParamLayout make_layout(int edge_dim, int out_dim) {
     return L;
 }
 
+// ---- flat parameter layout of an n_layers-deep network (gnn.py:78-104 with n_layers > 1) -----------------------
+// Forward order: the 9 Dense layers of GNN layer 0, ..., of layer n - 1, then the 3 of the head.  layer[l] views GNN
+// layer l plus the head as a 12-entry ParamLayout (its `total` is the whole network's).  From layer 1 on, msg/Dense_0
+// reads [edge | y_sender | y_receiver] (ed + 256 rows) and update/Dense_0 reads [y | aggregate] (256 rows); every layer
+// outputs 128.  n_layers = 1 gives make_layout's offsets.
+constexpr int GCBF_MAX_LAYERS = 8;
+struct DeepLayout {
+    int n_layers;
+    ParamLayout layer[GCBF_MAX_LAYERS];
+    int total;
+};
+inline DeepLayout make_deep_layout(int edge_dim, int out_dim, int n_layers) {
+    DeepLayout D;
+    D.n_layers = n_layers;
+    const ParamLayout L0 = make_layout(edge_dim, out_dim);
+    int off = 0;
+    auto place = [&](ParamLayout& P, int i, int in) {
+        P.in[i] = in;
+        P.out[i] = L0.out[i];
+        P.w[i] = off;
+        off += in * L0.out[i];
+        off = (off + 3) & ~3;
+        P.b[i] = off;
+        off += L0.out[i];
+        off = (off + 3) & ~3;
+    };
+    for (int l = 0; l < n_layers; ++l)
+        for (int i = 0; i < L_HEAD0; ++i)
+            place(D.layer[l], i, l == 0 ? L0.in[i] : (i == L_MSG0 ? edge_dim + 256 : (i == L_UPD0 ? 256 : L0.in[i])));
+    for (int i = L_HEAD0; i <= L_OUT; ++i) place(D.layer[0], i, L0.in[i]);
+    for (int l = 0; l < n_layers; ++l) {
+        for (int i = L_HEAD0; i <= L_OUT; ++i) {
+            D.layer[l].in[i] = D.layer[0].in[i];
+            D.layer[l].out[i] = D.layer[0].out[i];
+            D.layer[l].w[i] = D.layer[0].w[i];
+            D.layer[l].b[i] = D.layer[0].b[i];
+        }
+        D.layer[l].total = off;
+    }
+    D.total = off;
+    return D;
+}
+
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

@@ -551,3 +551,357 @@ extern "C" __attribute__((visibility("default"))) int64_t gcbf_rollout_workspace
     const int64_t A = (int64_t)desc->n_graphs * desc->n_agents;
     return make_ws(desc->edge_cap, A).total + 8 * A + 16;
 }
+
+// =====================================================================================================
+// Networks with n_layers > 1 (gnn.py:78-104), tensor-core path, unfolded weights.
+// Edges and their features are the same in every layer; only the node features change.  Receivers are always agents,
+// so goal and hit nodes never receive a message: their layer output is update_l([y_{l-1} | 0]), one constant row per
+// layer for "goal" and one for "hit".  They ride along as node rows A and A + 1 of every node-level GEMM.
+// From layer 1 on, the first message layer W1 = [We; Ws; Wr] is split: pre1_e = feat_e We + S[src_e] + R[recv_e] + b1
+// with the node-level products S = y Ws and R = y Wr, so the edge kernel gathers two 256-wide rows instead of running a
+// K = ed + 256 GEMM per edge.
+// =====================================================================================================
+namespace gcbf {
+
+// Transposed tf32 hi / lo planes of every GEMM weight of a deep network (gcbf_prepare_params_l): slot i < 12 is
+// Dense layer i of ParamLayout layer[l] (L_MSG0 holds Ws, DEEP_WR holds Wr at l >= 1; the head lives in layer 0's
+// slots); -1 where the weight is not a GEMM operand.  hi at t[l][i], lo at t[l][i] + rows * cols.
+constexpr int DEEP_WR = 12;
+struct DeepPlanes {
+    int t[GCBF_MAX_LAYERS][13], src[GCBF_MAX_LAYERS][13], rows[GCBF_MAX_LAYERS][13], cols[GCBF_MAX_LAYERS][13];
+    int total;
+};
+static DeepPlanes make_deep_planes(const DeepLayout& D, int ed) {
+    DeepPlanes Q;
+    int off = 0;
+    for (int l = 0; l < D.n_layers; ++l) {
+        const ParamLayout& L = D.layer[l];
+        for (int i = 0; i < 13; ++i) {
+            int src = -1, rows = 0;
+            if (i == L_MSG0 || i == DEEP_WR) {
+                if (l > 0) { src = L.w[L_MSG0] + (ed + (i == DEEP_WR ? 128 : 0)) * 256; rows = 128; }
+            } else if (i == L_UPD0) {
+                src = L.w[i] + (l == 0 ? 3 * 256 : 0);
+                rows = l == 0 ? 128 : 256;
+            } else if (i == L_HEAD0 || i == L_HEAD1) {
+                if (l == 0) { src = L.w[i]; rows = L.in[i]; }
+            } else if (i != L_GATE && i != L_OUT) {
+                src = L.w[i];
+                rows = L.in[i];
+            }
+            const int cols = (i == DEEP_WR) ? 256 : L.out[i];
+            Q.src[l][i] = src;
+            Q.rows[l][i] = rows;
+            Q.cols[l][i] = cols;
+            Q.t[l][i] = src < 0 ? -1 : off;
+            if (src >= 0) off += 2 * rows * cols;
+        }
+    }
+    Q.total = off;
+    return Q;
+}
+
+static int32_t build_deep_planes(int ed, int out_dim, int n_layers, const float* P, float* PT, cudaStream_t st) {
+    const DeepLayout D = make_deep_layout(ed, out_dim, n_layers);
+    const DeepPlanes Q = make_deep_planes(D, ed);
+    PlaneJobList PJ;
+    for (int l = 0; l < n_layers; ++l) {
+        for (int i = 0; i < 13; ++i) {
+            if (Q.t[l][i] < 0) continue;
+            PJ.add(P + Q.src[l][i], Q.rows[l][i], Q.cols[l][i], true, PT + Q.t[l][i],
+                   PT + Q.t[l][i] + Q.rows[l][i] * Q.cols[l][i]);
+        }
+        if (int32_t rc = PJ.launch(st)) return rc;   // <= 11 jobs per layer
+    }
+    return 0;
+}
+
+// Workspace of the deep forward: the one-layer activations with A + 2 node rows, S | R and the update input [y | ag].
+struct DeepWs {
+    GnnWs g;
+    int64_t s, r, cat, total;
+};
+static DeepWs make_deep_ws(int64_t cap, int64_t A) {
+    DeepWs W;
+    W.g = make_ws(cap, A + 2);
+    int64_t o = W.g.total;
+    W.s = o;
+    o += (A + 2) * 256;
+    W.r = o;
+    o += (A + 2) * 256;
+    W.cat = o;
+    o += (A + 2) * 256;
+    W.total = o;
+    return W;
+}
+
+// X1 = relu(feat We + S[sender row] + R[receiver] + b1); warp per edge, lane owns 8 output columns.  The sender row of
+// a goal / hit node is the constant row A / A + 1.
+template <int ED>
+__global__ void __launch_bounds__(256)
+edge_deep_kernel(const int A, const int edge_cap, const float* __restrict__ We, const float* __restrict__ b1,
+                 const float* __restrict__ feat, const float* __restrict__ S, const float* __restrict__ R,
+                 const int32_t* __restrict__ edge_recv, const int32_t* __restrict__ edge_src,
+                 const int32_t* __restrict__ counters, float* __restrict__ X1) {
+    __shared__ __align__(16) float sW[ED][256];
+    __shared__ __align__(16) float sB[256];
+    for (int i = threadIdx.x; i < ED * 256; i += blockDim.x) sW[i / 256][i % 256] = We[i];
+    for (int i = threadIdx.x; i < 256; i += blockDim.x) sB[i] = b1[i];
+    __syncthreads();
+    const int nE = min(counters[0], edge_cap);
+    const int lane = threadIdx.x & 31;
+    const int warps_total = (gridDim.x * blockDim.x) >> 5;
+    for (int e = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; e < nE; e += warps_total) {
+        const int a = min(max(edge_recv[e], 0), A - 1);
+        const int code = min(edge_src[e], A - 1);
+        const int srow = code >= 0 ? code : (code == -1 ? A : A + 1);
+        const float4* sp = reinterpret_cast<const float4*>(S + (size_t)srow * 256 + lane * 8);
+        const float4* rp = reinterpret_cast<const float4*>(R + (size_t)a * 256 + lane * 8);
+        const float4 s0 = sp[0], s1 = sp[1], r0 = rp[0], r1 = rp[1];
+        const float sv[8] = {s0.x, s0.y, s0.z, s0.w, s1.x, s1.y, s1.z, s1.w};
+        const float rv[8] = {r0.x, r0.y, r0.z, r0.w, r1.x, r1.y, r1.z, r1.w};
+        float f[ED];
+#pragma unroll
+        for (int c = 0; c < ED; ++c) f[c] = feat[(size_t)e * FEAT_LD + c];
+        float y[8];
+#pragma unroll
+        for (int j = 0; j < 8; ++j) y[j] = sB[lane * 8 + j] + sv[j] + rv[j];
+#pragma unroll
+        for (int c = 0; c < ED; ++c) {
+#pragma unroll
+            for (int j = 0; j < 8; ++j) y[j] = fmaf(f[c], sW[c][lane * 8 + j], y[j]);
+        }
+        float4* dst = reinterpret_cast<float4*>(X1 + (size_t)e * 256 + lane * 8);
+        dst[0] = make_float4(fmaxf(y[0], 0.f), fmaxf(y[1], 0.f), fmaxf(y[2], 0.f), fmaxf(y[3], 0.f));
+        dst[1] = make_float4(fmaxf(y[4], 0.f), fmaxf(y[5], 0.f), fmaxf(y[6], 0.f), fmaxf(y[7], 0.f));
+    }
+}
+
+// Rows A (goal, one-hot [0,1,0]) and A + 1 (hit, [1,0,0]) of layer 0's first update layer: relu(U0[type] + bu0), the
+// aggregate being zero.
+static __global__ void const_rows_l0_kernel(const int A, const float* __restrict__ U0, const float* __restrict__ bu0,
+                                            float* __restrict__ V1) {
+    for (int i = threadIdx.x; i < 2 * 256; i += blockDim.x) {
+        const int r = i / 256, c = i % 256;
+        V1[(size_t)(A + r) * 256 + c] = fmaxf(U0[(1 - r) * 256 + c] + bu0[c], 0.f);
+    }
+}
+
+// CAT[r] = [Y[r] | AG[r]] for the A + 2 node rows; the goal / hit rows (r >= A) take a zero aggregate.
+static __global__ void __launch_bounds__(256)
+node_concat_kernel(const int A, const float* __restrict__ Y, const float* __restrict__ AG, float* __restrict__ CAT) {
+    const int n = (A + 2) * 64;
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        const int r = i >> 6, q = i & 63;
+        float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (q < 32) v = *reinterpret_cast<const float4*>(Y + (size_t)r * 128 + q * 4);
+        else if (r < A) v = *reinterpret_cast<const float4*>(AG + (size_t)r * 128 + (q - 32) * 4);
+        *reinterpret_cast<float4*>(CAT + (size_t)r * 256 + q * 4) = v;
+    }
+}
+
+// Forward of an n_layers-deep network.  out != nullptr: tanh(head) [A, out_dim]; else z_out [1][A][4] receives the
+// output layer's pre-activations without bias (the rollout step's policy tail adds the bias and the tanh).
+int32_t gnn_forward_deep(const gcbf_env_desc* d, int out_dim, int n_layers, const float* P, const float* PT,
+                         const float* agent, const float* goal, const float* hits, const int32_t* row_start,
+                         const int32_t* row_deg, const int32_t* edge_recv, const int32_t* edge_src,
+                         const int32_t* counters, int clip_all, float* out, float* z_out, float* ws, cudaStream_t st) {
+    const int ed = env_ed(d->env_kind);
+    const DeepLayout D = make_deep_layout(ed, out_dim, n_layers);
+    const DeepPlanes Q = make_deep_planes(D, ed);
+    const int A = d->n_graphs * d->n_agents, cap = d->edge_cap;
+    const DeepWs DW = make_deep_ws(cap, A);
+    const GnnWs& W = DW.g;
+    const RowCount re{counters, 0, cap};
+    const RowCount ra{nullptr, A, A};
+    const RowCount ra2{nullptr, A + 2, A + 2};
+    const int nsm = sm_count();
+    int32_t rc;
+    auto gemm = [&](int epi, int l, int i, const float* X, const float* bias, const float* bias2, float* Y,
+                    RowCount rows) -> int32_t {
+        const int K = Q.rows[l][i], N = Q.cols[l][i];
+        return tc::launch_gemm_tc(epi, false, X, PT + Q.t[l][i], PT + Q.t[l][i] + K * N, bias, bias2, Y, nullptr, rows,
+                                  K, N, st);
+    };
+    for (int l = 0; l < n_layers; ++l) {
+        const ParamLayout& L = D.layer[l];
+        const int egrid = min((cap + 7) / 8, 4 * nsm);
+        if (l == 0) {
+            GCBF_DISPATCH_ENV(d->env_kind, {
+                edge_l1_kernel<KIND><<<egrid, 256, 0, st>>>(*d, P + L.w[L_MSG0], P + L.b[L_MSG0], agent, goal, hits,
+                                                            edge_recv, edge_src, counters, clip_all, ws + W.feat,
+                                                            ws + W.x1);
+            });
+            count_launch();
+            if ((rc = check_launch("edge_l1_kernel"))) return rc;
+        } else {
+            if ((rc = gemm(EPI_NONE, l, L_MSG0, ws + W.v3, nullptr, nullptr, ws + DW.s, ra2))) return rc;
+            if ((rc = gemm(EPI_NONE, l, DEEP_WR, ws + W.v3, nullptr, nullptr, ws + DW.r, ra))) return rc;
+            GCBF_DISPATCH_ENV(d->env_kind, {
+                edge_deep_kernel<EnvTraits<KIND>::ED><<<egrid, 256, 0, st>>>(
+                    A, cap, P + L.w[L_MSG0], P + L.b[L_MSG0], ws + W.feat, ws + DW.s, ws + DW.r, edge_recv, edge_src,
+                    counters, ws + W.x1);
+            });
+            count_launch();
+            if ((rc = check_launch("edge_deep_kernel"))) return rc;
+        }
+        if ((rc = gemm(EPI_BIAS, l, L_MSG1, ws + W.x1, P + L.b[L_MSG1], nullptr, ws + W.x2, re))) return rc;
+        if ((rc = gemm(EPI_BIAS, l, L_MSGOUT, ws + W.x2, P + L.b[L_MSGOUT], nullptr, ws + W.msg, re))) return rc;
+        if ((rc = gemm(EPI_BIAS_RELU, l, L_ATT0, ws + W.msg, P + L.b[L_ATT0], nullptr, ws + W.g1, re))) return rc;
+        if ((rc = gemm(EPI_BIAS, l, L_ATT1, ws + W.g1, P + L.b[L_ATT1], nullptr, ws + W.g2, re))) return rc;
+        {
+            const int grid = min((A + 7) / 8, 4 * nsm);
+            attn_aggregate_kernel<<<grid, 256, 0, st>>>(A, cap, ws + W.g2, ws + W.msg, P + L.w[L_GATE], P + L.b[L_GATE],
+                                                        row_start, row_deg, ws + W.att, ws + W.ag);
+            count_launch();
+            if ((rc = check_launch("attn_aggregate_kernel"))) return rc;
+        }
+        if (l == 0) {
+            // agent one-hot [0,0,1] folded into the bias: row 2 of update/Dense_0
+            if ((rc = gemm(EPI_BIAS_RELU, l, L_UPD0, ws + W.ag, P + L.b[L_UPD0], P + L.w[L_UPD0] + 2 * 256, ws + W.v1,
+                           ra))) return rc;
+            const_rows_l0_kernel<<<1, 256, 0, st>>>(A, P + L.w[L_UPD0], P + L.b[L_UPD0], ws + W.v1);
+            count_launch();
+            if ((rc = check_launch("const_rows_l0_kernel"))) return rc;
+        } else {
+            node_concat_kernel<<<min((A + 2 + 3) / 4, 4 * nsm), 256, 0, st>>>(A, ws + W.v3, ws + W.ag, ws + DW.cat);
+            count_launch();
+            if ((rc = check_launch("node_concat_kernel"))) return rc;
+            if ((rc = gemm(EPI_BIAS_RELU, l, L_UPD0, ws + DW.cat, P + L.b[L_UPD0], nullptr, ws + W.v1, ra2))) return rc;
+        }
+        if ((rc = gemm(EPI_BIAS, l, L_UPD1, ws + W.v1, P + L.b[L_UPD1], nullptr, ws + W.v2, ra2))) return rc;
+        if ((rc = gemm(EPI_BIAS, l, L_UPDOUT, ws + W.v2, P + L.b[L_UPDOUT], nullptr, ws + W.v3, ra2))) return rc;
+    }
+    const ParamLayout& L = D.layer[0];
+    if ((rc = gemm(EPI_BIAS_RELU, 0, L_HEAD0, ws + W.v3, P + L.b[L_HEAD0], nullptr, ws + W.h1, ra))) return rc;
+    if ((rc = gemm(EPI_BIAS, 0, L_HEAD1, ws + W.h1, P + L.b[L_HEAD1], nullptr, ws + W.h2, ra))) return rc;
+    const int grid = min((A + 7) / 8, 4 * nsm);
+    if (out != nullptr) {
+        head_out_kernel<<<grid, 256, 0, st>>>(A, out_dim, ws + W.h2, P + L.w[L_OUT], P + L.b[L_OUT], out);
+        count_launch();
+        return check_launch("head_out_kernel");
+    }
+    head_z_kernel<<<grid, 256, 0, st>>>(A, out_dim, ws + W.h2, P + L.w[L_OUT], z_out);
+    count_launch();
+    return check_launch("head_z_kernel");
+}
+
+}  // namespace gcbf
+
+static bool deep_dims_ok(int32_t edge_dim, int32_t out_dim, int32_t n_layers) {
+    return edge_dim >= 1 && edge_dim <= 6 && out_dim >= 1 && out_dim <= 4 && n_layers >= 1 &&
+           n_layers <= gcbf::GCBF_MAX_LAYERS;
+}
+
+extern "C" __attribute__((visibility("default"))) int32_t gcbf_params_t_count_l(int32_t edge_dim, int32_t out_dim,
+                                                                                int32_t n_layers) {
+    if (!deep_dims_ok(edge_dim, out_dim, n_layers)) return -1;
+    if (n_layers == 1) return gcbf_params_t_count(edge_dim, out_dim);
+    return make_deep_planes(make_deep_layout(edge_dim, out_dim, n_layers), edge_dim).total;
+}
+
+extern "C" __attribute__((visibility("default"))) int32_t gcbf_prepare_params_l(int32_t edge_dim, int32_t out_dim,
+                                                                                int32_t n_layers, const float* params,
+                                                                                float* params_t, void* stream) {
+    GCBF_REQUIRE(deep_dims_ok(edge_dim, out_dim, n_layers) && params && params_t, "gcbf_prepare_params_l: bad argument");
+    GCBF_REQUIRE((((uintptr_t)params | (uintptr_t)params_t) & 15) == 0, "gcbf_prepare_params_l: 16-byte alignment required");
+    if (n_layers == 1) return gcbf_prepare_params(edge_dim, out_dim, params, params_t, stream);
+    return build_deep_planes(edge_dim, out_dim, n_layers, params, params_t, (cudaStream_t)stream);
+}
+
+extern "C" __attribute__((visibility("default"))) int64_t gcbf_gnn_workspace_floats_l(const gcbf_env_desc* desc,
+                                                                                     int32_t out_dim, int32_t n_layers) {
+    if (n_layers == 1) return gcbf_gnn_workspace_floats(desc, out_dim);
+    if (!desc || desc->edge_cap <= 0 || desc->n_graphs <= 0 || desc->n_agents <= 0 || n_layers < 1 ||
+        n_layers > gcbf::GCBF_MAX_LAYERS) return -1;
+    return make_deep_ws(desc->edge_cap, (int64_t)desc->n_graphs * desc->n_agents).total;
+}
+
+extern "C" __attribute__((visibility("default"))) int32_t gcbf_gnn_forward_l(
+    const gcbf_env_desc* desc, int32_t net_kind, int32_t out_dim, int32_t n_layers, const float* params,
+    const float* params_t, const float* agent, const float* goal, const float* hits, const int32_t* row_start,
+    const int32_t* row_deg, const int32_t* edge_recv, const int32_t* edge_src, const int32_t* counters, int32_t clip_all,
+    float* out, float* workspace, int64_t workspace_floats, void* stream) {
+    GCBF_REQUIRE(n_layers >= 1 && n_layers <= GCBF_MAX_LAYERS, "gcbf_gnn_forward_l: n_layers %d outside [1, %d]",
+                 n_layers, GCBF_MAX_LAYERS);
+    if (n_layers == 1)
+        return gcbf_gnn_forward(desc, net_kind, out_dim, params, params_t, agent, goal, hits, row_start, row_deg,
+                                edge_recv, edge_src, counters, clip_all, out, workspace, workspace_floats, stream);
+    GCBF_REQUIRE(desc && params && agent && goal && hits && row_start && row_deg && edge_recv && edge_src && counters &&
+                     out && workspace, "gcbf_gnn_forward_l: NULL pointer argument");
+    GCBF_REQUIRE(params_t, "gcbf_gnn_forward_l: n_layers > 1 runs on the tensor-core path only (params_t from "
+                           "gcbf_prepare_params_l); the strict-fp32 SIMT path implements n_layers = 1");
+    GCBF_REQUIRE(desc->env_kind >= 0 && desc->env_kind <= 3, "bad env_kind");
+    GCBF_REQUIRE(net_kind == GCBF_NET_CBF || net_kind == GCBF_NET_ACTOR, "bad net_kind %d", net_kind);
+    GCBF_REQUIRE(out_dim >= 1 && out_dim <= 4 && (net_kind != GCBF_NET_CBF || out_dim == 1), "bad out_dim %d", out_dim);
+    GCBF_REQUIRE(desc->edge_cap > 0, "edge_cap must be positive");
+    const int64_t need = make_deep_ws(desc->edge_cap, (int64_t)desc->n_graphs * desc->n_agents).total;
+    GCBF_REQUIRE(workspace_floats >= need, "workspace too small: %lld < %lld floats", (long long)workspace_floats,
+                 (long long)need);
+    GCBF_REQUIRE((((uintptr_t)params | (uintptr_t)params_t | (uintptr_t)workspace) & 15) == 0,
+                 "params/params_t/workspace must be 16-byte aligned");
+    return gnn_forward_deep(desc, out_dim, n_layers, params, params_t, agent, goal, hits, row_start, row_deg, edge_recv,
+                            edge_src, counters, clip_all, out, nullptr, workspace, (cudaStream_t)stream);
+}
+
+extern "C" __attribute__((visibility("default"))) int64_t gcbf_rollout_workspace_floats_l(const gcbf_env_desc* desc,
+                                                                                         int32_t n_layers) {
+    if (n_layers == 1) return gcbf_rollout_workspace_floats(desc);
+    if (!desc || desc->edge_cap <= 0 || desc->n_graphs <= 0 || desc->n_agents <= 0 || n_layers < 1 ||
+        n_layers > gcbf::GCBF_MAX_LAYERS) return -1;
+    const int64_t A = (int64_t)desc->n_graphs * desc->n_agents;
+    return make_deep_ws(desc->edge_cap, A).total + 8 * A + 16;
+}
+
+extern "C" __attribute__((visibility("default"))) int32_t gcbf_rollout_step_l(
+    const gcbf_env_desc* desc, int32_t n_layers, const float* actor_params, const float* infer_blob,
+    int32_t use_tensor_cores, const float* agent, const float* goal, const float* obstacles, const float* ray_table,
+    const float* hits, const int32_t* row_start, const int32_t* row_deg, const int32_t* edge_recv,
+    const int32_t* edge_src, const int32_t* counters, float* action, float* next_agent, float* next_hits,
+    int32_t* next_row_start, int32_t* next_row_deg, int32_t* next_edge_recv, int32_t* next_edge_src,
+    int32_t* next_counters, float* reward, float* cost, float* workspace, int64_t workspace_floats, void* stream) {
+    GCBF_REQUIRE(n_layers >= 1 && n_layers <= GCBF_MAX_LAYERS, "gcbf_rollout_step_l: n_layers %d outside [1, %d]",
+                 n_layers, GCBF_MAX_LAYERS);
+    if (n_layers == 1)
+        return gcbf_rollout_step(desc, actor_params, infer_blob, use_tensor_cores, agent, goal, obstacles, ray_table,
+                                 hits, row_start, row_deg, edge_recv, edge_src, counters, action, next_agent, next_hits,
+                                 next_row_start, next_row_deg, next_edge_recv, next_edge_src, next_counters, reward,
+                                 cost, workspace, workspace_floats, stream);
+    GCBF_REQUIRE(desc && actor_params && infer_blob && agent && goal && ray_table && hits && row_start && row_deg &&
+                     edge_recv && edge_src && counters && action && next_agent && next_hits && next_row_start &&
+                     next_row_deg && next_edge_recv && next_edge_src && next_counters && reward && cost && workspace,
+                 "gcbf_rollout_step_l: NULL pointer argument");
+    GCBF_REQUIRE(use_tensor_cores, "gcbf_rollout_step_l: n_layers > 1 runs on the tensor-core path only");
+    GCBF_REQUIRE(next_row_start != row_start && next_row_deg != row_deg && next_edge_recv != edge_recv &&
+                     next_edge_src != edge_src && next_counters != counters,
+                 "gcbf_rollout_step_l: the next graph must not alias the current one (double-buffer the edge lists)");
+    GCBF_REQUIRE(desc->env_kind >= 0 && desc->env_kind <= 3 && desc->edge_cap > 0, "gcbf_rollout_step_l: bad descriptor");
+    GCBF_REQUIRE(desc->n_obs == 0 || obstacles, "obstacles is NULL but n_obs > 0");
+    const int nu = env_nu(desc->env_kind);
+    const int64_t A = (int64_t)desc->n_graphs * desc->n_agents;
+    const DeepWs W = make_deep_ws(desc->edge_cap, A);
+    GCBF_REQUIRE(workspace_floats >= W.total + 8 * A + 8, "workspace too small: %lld < %lld floats",
+                 (long long)workspace_floats, (long long)(W.total + 8 * A + 8));
+    GCBF_REQUIRE((((uintptr_t)workspace | (uintptr_t)actor_params | (uintptr_t)infer_blob) & 15) == 0,
+                 "actor_params/infer_blob/workspace must be 16-byte aligned");
+    cudaStream_t st = (cudaStream_t)stream;
+    const DeepLayout D = make_deep_layout(env_ed(desc->env_kind), nu, n_layers);
+    float* z = workspace + ((W.total + 3) & ~(int64_t)3);    // [1][A][4] output-layer pre-activations
+    if (int32_t rc = gnn_forward_deep(desc, nu, n_layers, actor_params, infer_blob, agent, goal, hits, row_start,
+                                      row_deg, edge_recv, edge_src, counters, 0, nullptr, z, workspace, st)) return rc;
+    TailArgs tl;
+    tl.z = z;
+    tl.parts = 1;
+    tl.z_cap = (int)A;
+    tl.bHO = actor_params + D.layer[0].b[L_OUT];
+    tl.agent_prev = agent;
+    tl.goal = goal;
+    tl.row_start_prev = row_start;
+    tl.row_deg_prev = row_deg;
+    tl.edge_src_prev = edge_src;
+    tl.action = action;
+    tl.next_agent = next_agent;
+    // flags 1: cast rays; the build clears the next edge counter itself
+    return graph_build_impl(desc, nullptr, obstacles, ray_table, next_hits, next_row_start, next_row_deg, next_edge_recv,
+                            next_edge_src, next_counters, 1, tl, reward, cost, stream);
+}

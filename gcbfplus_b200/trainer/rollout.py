@@ -5,7 +5,8 @@ Two device paths with the same arithmetic (bit-identical results, tests/test_gpu
 * persistent (default where supported: 2-D environments, n <= 512): ONE kernel launch for the whole T-step rollout, one
   thread-block cluster per environment looping over the steps (csrc/rollout_persist.cu);
 * 5-launch env-step (gcbf_rollout_step), the whole T-step loop captured in one CUDA graph: LinearDrone, n > 512,
-  GCBF_PERSISTENT=0, the u_ref policy.
+  GCBF_PERSISTENT=0, the u_ref policy, and actors with more than one GNN layer (gcbf_rollout_step_l; the engine takes
+  the depth from the network set_params() receives).
 No host sync inside the loop on either path.
 The CBF-QP baselines (algo/cbf_qp.py) run on the CUDA-graph path: per step the pairwise CBFs + QP solve (2 launches),
 env.step with the QP action as input, and the graph build of the next state.
@@ -103,6 +104,7 @@ class RolloutEngine:
         level = int(env.lib.gcbf_rollout_persistent_supported(C.byref(self._pdesc))) \
             if (policy == "actor" and self.use_tc) else 0
         ok = level > 0
+        self._persistent_requested = persistent is True   # an explicit request, not the default choice below
         if persistent is None:
             # default only where every environment's cluster is resident at once (level 2): otherwise the environments
             # beyond the resident clusters run in a second round
@@ -116,6 +118,8 @@ class RolloutEngine:
             raise ValueError("persistent rollout unsupported for this configuration (2-D env, n <= 512, tensor-core path, "
                              "actor policy)")
         self.persistent = bool(persistent)
+        self._persistent_one_layer = self.persistent   # the path a one-layer actor takes (restored by _set_depth)
+        self.n_layers = 1           # GNN depth of the actor, taken from the network set_params() receives
         #: optional [T + 1, 8] int64 device tensor: in-kernel %globaltimer stamps of the persistent rollout (set before
         #: the first run(); see gcbf_rollout_persistent in include/gcbf_b200.h)
         self.phase_stamps: Optional[torch.Tensor] = None
@@ -147,6 +151,19 @@ class RolloutEngine:
         env, d = self.env, ch.desc
         obs = self.obstacles[ch.e0].data_ptr() if self.O > 0 else None
         b = t % 2
+        if self.policy == "actor" and self.n_layers > 1:
+            rc = env.lib.gcbf_rollout_step_l(
+                C.byref(d), self.n_layers, self.params_buf.data_ptr(), self.infer_blob.data_ptr(), self.use_tc,
+                self.agent[t, ch.e0].data_ptr(), self.goal[ch.e0].data_ptr(), obs, env.ray_table.data_ptr(),
+                self.hits[t, ch.e0].data_ptr(), ch.row_start[b].data_ptr(), ch.row_deg[b].data_ptr(),
+                ch.edge_recv[b].data_ptr(), ch.edge_src[b].data_ptr(), ch.counters[t].data_ptr(),
+                self.actions[t, ch.e0].data_ptr(), self.agent[t + 1, ch.e0].data_ptr(),
+                self.hits[t + 1, ch.e0].data_ptr(), ch.row_start[1 - b].data_ptr(), ch.row_deg[1 - b].data_ptr(),
+                ch.edge_recv[1 - b].data_ptr(), ch.edge_src[1 - b].data_ptr(), ch.counters[t + 1].data_ptr(),
+                self.rewards[t, ch.e0:].data_ptr(), self.costs[t, ch.e0:].data_ptr(), ch.ws.data_ptr(), ch.ws.numel(),
+                stream)
+            _lib.check(rc, "gcbf_rollout_step_l")
+            return
         if self.policy == "actor":      # algo.step + env.step + get_graph(next) in one call (6 launches)
             rc = env.lib.gcbf_rollout_step(
                 C.byref(d), self.params_buf.data_ptr(), self.infer_blob.data_ptr(), self.use_tc,
@@ -206,9 +223,42 @@ class RolloutEngine:
             self.obstacles.copy_(packed.reshape(self.obstacles.shape), non_blocking=True)
         self._obstacle_obj = obstacle
 
+    def _set_depth(self, n_layers: int) -> None:
+        """Re-size the parameter / weight / workspace buffers for an actor with n_layers GNN layers.  The persistent
+        kernel implements one layer, so a deeper actor runs on the step-by-step path; a one-layer actor gets the path
+        the constructor chose for it, whatever actors the engine ran before."""
+        env, dev, nu = self.env, self.env.device, self.env.action_dim
+        if n_layers > 1 and self._persistent_requested:
+            raise ValueError("the persistent rollout implements one GNN layer; this actor has %d" % n_layers)
+        if n_layers > 1 and not self.use_tc:
+            raise ValueError("actors with more than one GNN layer run on the tensor-core path only "
+                             "(GCBF_TENSOR_CORES=0 selects the strict-fp32 path, which implements one layer)")
+        self.n_layers = n_layers
+        self.persistent = self._persistent_one_layer and n_layers == 1
+        if not self.persistent:
+            self._pws = None
+        elif self._pws is None:
+            n = env.lib.gcbf_rollout_persistent_workspace_floats(C.byref(self._pdesc))
+            self._pws = torch.empty(int(n), dtype=torch.float32, device=dev)
+        self._graph = None
+        self.params_buf = torch.zeros(_lib.param_count(env.edge_dim, nu, n_layers), dtype=torch.float32, device=dev)
+        n_blob = env.lib.gcbf_infer_count(env.edge_dim, nu) if n_layers == 1 else \
+            env.lib.gcbf_params_t_count_l(env.edge_dim, nu, n_layers)
+        self.infer_blob = torch.zeros(int(n_blob), dtype=torch.float32, device=dev)
+        ch = self.chains[0]
+        ch.ws = torch.empty(int(env.lib.gcbf_rollout_workspace_floats_l(C.byref(ch.desc), n_layers)),
+                            dtype=torch.float32, device=dev)
+
     def set_params(self, params: NetParams) -> None:
+        if params.n_layers != self.n_layers:
+            self._set_depth(params.n_layers)
         self.params_buf.copy_(params.flat, non_blocking=True)
         env = self.env
+        if self.n_layers > 1:   # transposed tf32 planes of every layer's weights (gcbf_rollout_step_l's infer_blob)
+            _lib.check(env.lib.gcbf_prepare_params_l(env.edge_dim, env.action_dim, self.n_layers,
+                                                     _lib.ptr(self.params_buf), _lib.ptr(self.infer_blob),
+                                                     env._stream()), "gcbf_prepare_params_l")
+            return
         _lib.check(env.lib.gcbf_prepare_infer(env.edge_dim, env.action_dim, _lib.ptr(self.params_buf),
                                               _lib.ptr(self.infer_blob), env._stream()), "gcbf_prepare_infer")
 

@@ -8,6 +8,7 @@ from time import time
 import numpy as np
 
 from .. import dist as gdist
+from ..algo.train import require_one_layer
 from ..utils import jrandom as jr
 from .rollout import RolloutEngine
 from .utils import eval_metrics, rollout
@@ -17,6 +18,8 @@ class Trainer:
 
     def __init__(self, env, env_test, algo, n_env_train: int, n_env_test: int, log_dir: str, seed: int, params: dict,
                  save_log: bool = True):
+        # reject a network the train step cannot train before any directory, checkpoint or rollout is made
+        require_one_layer(algo.cbf_params.n_layers, "Trainer")
         self.env = env
         self.env_test = env_test
         self.algo = algo

@@ -99,6 +99,11 @@ int64_t gcbf_launch_count(void);
  * (24 entries: W,b of the 12 Dense layers in forward order, see DESIGN.md). */
 int32_t gcbf_param_count(int32_t edge_dim, int32_t out_dim);
 int32_t gcbf_param_offsets(int32_t edge_dim, int32_t out_dim, int32_t* offsets24_host);
+/* The same for a network with n_layers GNN layers (gnn.py:78-104; 1 <= n_layers <= 8): W,b of the 9 Dense layers
+ * of GNN layer 0, ..., of layer n_layers - 1, then of the 3 head layers (2 * (9 * n_layers + 3) entries).  From
+ * layer 1 on, msg/Dense_0 is [ed + 256, 256] and update/Dense_0 is [256, 256].  n_layers = 1: the layout above. */
+int32_t gcbf_param_count_l(int32_t edge_dim, int32_t out_dim, int32_t n_layers);
+int32_t gcbf_param_offsets_l(int32_t edge_dim, int32_t out_dim, int32_t n_layers, int32_t* offsets_host);
 
 /* ---------------------------------------------------------------- graph build (a1,a2,a3)
  * Replaces env.get_graph: get_lidar/raytracing/inside_obstacles
@@ -132,6 +137,19 @@ int32_t gcbf_gnn_forward(const gcbf_env_desc* desc, int32_t net_kind, int32_t ou
                          const int32_t* row_start, const int32_t* row_deg, const int32_t* edge_recv,
                          const int32_t* edge_src, const int32_t* counters, int32_t clip_all, float* out,
                          float* workspace, int64_t workspace_floats, void* stream);
+/* The same for n_layers GNN layers (params in the gcbf_param_offsets_l layout).  n_layers = 1 is the call above.
+ * n_layers > 1 runs on the tensor-core path only (params_t from gcbf_prepare_params_l must not be NULL): from layer 1
+ * on, S = y Ws and R = y Wr are node-level GEMMs and each edge gathers S[sender] + R[receiver]; goal and hit nodes,
+ * which never receive a message, are one constant row each per layer. */
+int64_t gcbf_gnn_workspace_floats_l(const gcbf_env_desc* desc, int32_t out_dim, int32_t n_layers);
+int32_t gcbf_params_t_count_l(int32_t edge_dim, int32_t out_dim, int32_t n_layers);
+int32_t gcbf_prepare_params_l(int32_t edge_dim, int32_t out_dim, int32_t n_layers, const float* params,
+                              float* params_t, void* stream);
+int32_t gcbf_gnn_forward_l(const gcbf_env_desc* desc, int32_t net_kind, int32_t out_dim, int32_t n_layers,
+                           const float* params, const float* params_t, const float* agent, const float* goal,
+                           const float* hits, const int32_t* row_start, const int32_t* row_deg,
+                           const int32_t* edge_recv, const int32_t* edge_src, const int32_t* counters,
+                           int32_t clip_all, float* out, float* workspace, int64_t workspace_floats, void* stream);
 
 /* Inference-only forward with FOLDED weights (rollouts; same functions replaced as gcbf_gnn_forward).
  * Each MLP block ends in two activation-free linear layers (nn/mlp.py:23-29, act_final=False), which are
@@ -223,6 +241,20 @@ int32_t gcbf_rollout_step_select(const gcbf_env_desc* desc, const float* actor_p
                                  int32_t* next_row_deg, int32_t* next_edge_recv, int32_t* next_edge_src,
                                  int32_t* next_counters, float* reward, float* cost, float* workspace,
                                  int64_t workspace_floats, int32_t select, void* stream);
+/* The rollout step for an actor with n_layers GNN layers.  n_layers = 1 is gcbf_rollout_step.  n_layers > 1 (tensor-core
+ * path only): infer_blob is the gcbf_prepare_params_l output, the policy forward runs layer by layer unfolded
+ * (gcbf_gnn_forward_l) and the same policy tail + graph build kernel ends the step.
+ * workspace: gcbf_rollout_workspace_floats_l(). */
+int64_t gcbf_rollout_workspace_floats_l(const gcbf_env_desc* desc, int32_t n_layers);
+int32_t gcbf_rollout_step_l(const gcbf_env_desc* desc, int32_t n_layers, const float* actor_params,
+                            const float* infer_blob, int32_t use_tensor_cores, const float* agent,
+                            const float* goal, const float* obstacles, const float* ray_table, const float* hits,
+                            const int32_t* row_start, const int32_t* row_deg, const int32_t* edge_recv,
+                            const int32_t* edge_src, const int32_t* counters, float* action, float* next_agent,
+                            float* next_hits, int32_t* next_row_start, int32_t* next_row_deg,
+                            int32_t* next_edge_recv, int32_t* next_edge_src, int32_t* next_counters,
+                            float* reward, float* cost, float* workspace, int64_t workspace_floats,
+                            void* stream);
 
 /* ---------------------------------------------------------------- persistent rollout (a8 whole scan)
  * The WHOLE rollout() of gcbfplus/trainer/utils.py:25-55 (reset excluded) in ONE kernel launch: one thread-block cluster

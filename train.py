@@ -16,6 +16,9 @@ def train(args):
     print(f"> Running train.py {args}")
     if args.cpu:
         raise SystemExit("--cpu: gcbfplus_b200 is the sm_90a CUDA path only (no CPU fallback by design)")
+    # before any device, directory or run is set up: the train step implements one GNN layer
+    from gcbfplus_b200.algo.train import require_one_layer
+    require_one_layer(args.gnn_layers, "training (train.py --gnn-layers)")
     os.environ.setdefault("WANDB_MODE", "offline")
     # one process per GPU under torchrun (python -m torch.distributed.run --nproc-per-node N train.py ...):
     # environments are sharded over the ranks, gradients all-reduced once per optimizer step (SURVEY 8e)
