@@ -114,7 +114,8 @@ class MinibatchRunner:
     Per minibatch the host then does two tiny device copies (selection indices, global label counts) and one graph
     launch instead of ~170 kernel launches with per-launch tensor-map encoding: the train step stops being bound by
     Python / launch overhead when a rank's share of the minibatch is small (8 GPUs: 32 graphs per rank).
-    GCBF_TRAIN_GRAPH=0 keeps the eager path (same kernels, same order -> same bits)."""
+    GCBF_TRAIN_GRAPH=0 keeps the eager path (same kernels, same order -> same bits: the graph build's canonical edge
+    layout and the train step's fixed-order reductions make every launch deterministic)."""
 
     def __init__(self, algo, batch: dict, mb_size: int, edge_cap: int, u_qp: torch.Tensor):
         env = algo._env

@@ -2,8 +2,11 @@
 // path; SURVEY 8c: fp32 FMA is the parity default).  All operands row-major, contiguous.
 //
 //   gemm_nn : C[M,N] = epi(A[M,K] @ B[K,N])     forward (B = W) and backward-data (B = W^T)
-//   gemm_tn : C[K1,N] += sum_m w[m] * X[m,K1] * dY[m,N]   backward-weight (split over M, red.add)
+//   gemm_tn : C[K1,N] += sum_m w[m] * X[m,K1] * dY[m,N]   backward-weight (split over M, ordered partial sums)
 //   colsum  : db[N] += sum_m w[m] * dY[m,N]
+//
+// No float atomics: a kernel that splits a sum over CTAs writes one partial per CTA to a workspace and
+// partial_sum_kernel adds the partials in CTA order, so every result is bit-identical from run to run.
 //
 // Tiling: CTA tile 128x128, BK = 16, 256 threads, 8x8 register tile per thread split as
 // 2x2 blocks of 4x4 (conflict-free LDS.128), register-prefetch double buffering, persistent
@@ -26,6 +29,78 @@ enum GemmEpi {
 
 constexpr int GEMM_BM = 128, GEMM_BN = 128, GEMM_BK = 16, GEMM_THREADS = 256;
 constexpr int GEMM_LDA = GEMM_BM + 4;  // padded: transposed A tile
+
+// ------------------------------------------------------------------------------------ ordered partial sums
+// Floats of the partials workspace every split reduction of the train step shares (one reduction at a time, in stream
+// order): 160 CTAs of a [128 x 256] weight-gradient tile plus its 256 column sums.  Launchers cap their CTA count so
+// that their partials fit.
+constexpr int64_t PART_FLOATS = 160 * (128 * 256 + 256);
+constexpr int DW_MAX_CTAS_TC = 160;     // tensor-core dW GEMM: [128 x N] partial (+ N column sums) per CTA
+constexpr int DW_MAX_CTAS_SIMT = 320;   // SIMT dW GEMM: [128 x 128] partial per CTA
+
+// destination segments of one reduction: element i of a partial maps to segment k, offset j; dst2 (optional) receives
+// the same sum (a bias gradient shared by two parameters)
+struct PartSeg {
+    float* dst;
+    float* dst2;
+    int n;
+};
+struct PartSegs {
+    PartSeg s[3];
+    int count = 0;
+    PartSegs& add(float* dst, int n, float* dst2 = nullptr) {
+        s[count++] = PartSeg{dst, dst2, n};
+        return *this;
+    }
+    int total() const {
+        int n = 0;
+        for (int k = 0; k < count; ++k) n += s[k].n;
+        return n;
+    }
+};
+
+// dst[i] += sum_{p < P} part[p * stride + i], the p in increasing order: a CTA takes 32 consecutive elements, warp w
+// sums the partials p = w, w + 8, ... and warp 0 adds the 8 warp sums in warp order.  P = nparts, or, with a device row
+// count, the number of parts that had rows: min(nparts, ceil(M / rows_per_part)) (the other parts wrote nothing).
+static __global__ void __launch_bounds__(256)
+partial_sum_kernel(const float* __restrict__ part, const int64_t stride, const int nparts, const PartSegs segs,
+                   const int n_total, const int32_t* __restrict__ m_ptr, const int m_cap, const int rows_per_part) {
+    __shared__ float red[8][32];
+    int P = nparts;
+    if (m_ptr) {
+        const int M = min(*m_ptr, m_cap);
+        P = min(P, (M + rows_per_part - 1) / rows_per_part);
+    }
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    const int i = blockIdx.x * 32 + lane;
+    float s = 0.f;
+    if (i < n_total) {
+#pragma unroll 4
+        for (int p = w; p < P; p += 8) s += part[(size_t)p * stride + i];
+    }
+    red[w][lane] = s;
+    __syncthreads();
+    if (w != 0 || i >= n_total) return;
+    for (int k = 1; k < 8; ++k) s += red[k][lane];
+    int j = i;
+    for (int k = 0; k < segs.count; ++k) {
+        if (j < segs.s[k].n) {
+            segs.s[k].dst[j] += s;
+            if (segs.s[k].dst2) segs.s[k].dst2[j] += s;
+            return;
+        }
+        j -= segs.s[k].n;
+    }
+}
+
+inline int32_t launch_partial_sum(const float* part, int64_t stride, int nparts, const PartSegs& segs, cudaStream_t st,
+                                  const int32_t* m_ptr = nullptr, int m_cap = 0, int rows_per_part = 1) {
+    const int n = segs.total();
+    if (n <= 0 || nparts <= 0) return 0;
+    partial_sum_kernel<<<(n + 31) / 32, 256, 0, st>>>(part, stride, nparts, segs, n, m_ptr, m_cap, rows_per_part);
+    count_launch();
+    return check_launch("partial_sum_kernel");
+}
 
 template <int EPI, bool ACCUM>
 __global__ void __launch_bounds__(GEMM_THREADS, 2)
@@ -138,11 +213,13 @@ gemm_nn_kernel(const float* __restrict__ A, const float* __restrict__ B, const f
 // backward-weight: C[K1,N] += sum_m w(m) X[m, K1] dY[m, N]; K1, N multiples of 128.
 // grid = (K1/128 * N/128) * splits ; each CTA walks m-chunks {split, split+S, ...}.
 // `roww`: optional per-agent weights; `row2agent`: optional row -> agent map (edges -> receiver).
+// `part` (splits > 1): the CTA stores its tile to part[split][K1][N] and partial_sum_kernel adds the splits to C;
+// otherwise (one split) the CTA adds its tile to C itself.
 static __global__ void __launch_bounds__(GEMM_THREADS, 2)
 gemm_tn_kernel(const float* __restrict__ X, const int ldx, const float* __restrict__ dY, float* __restrict__ C,
                const float* __restrict__ roww, const int32_t* __restrict__ row2agent,
                const int32_t* __restrict__ m_ptr, const int m_fixed, const int m_cap, const int K1, const int N,
-               const int splits, const int n_agents_total) {
+               const int splits, const int n_agents_total, float* __restrict__ part) {
     __shared__ __align__(16) float As[2][GEMM_BK][GEMM_BM];
     __shared__ __align__(16) float Bs[2][GEMM_BK][GEMM_BN];
     int M = m_ptr ? *m_ptr : m_fixed;
@@ -210,25 +287,31 @@ gemm_tn_kernel(const float* __restrict__ X, const int ldx, const float* __restri
         if (more) store_smem(buf ^ 1);
         __syncthreads();
     }
+    float* dst = part ? part + (size_t)split * K1 * N : C;
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
         const int kr = k0 + ((i < 4) ? (ty * 4 + i) : (64 + ty * 4 + i - 4));
 #pragma unroll
-        for (int j = 0; j < 8; ++j) {
-            const int n = n0 + ((j < 4) ? (tx * 4 + j) : (64 + tx * 4 + j - 4));
-            atomicAdd(C + (size_t)kr * N + n, acc[i][j]);
+        for (int jh = 0; jh < 2; ++jh) {
+            float4* p = reinterpret_cast<float4*>(dst + (size_t)kr * N + n0 + jh * 64 + tx * 4);
+            float4 v = make_float4(acc[i][jh * 4 + 0], acc[i][jh * 4 + 1], acc[i][jh * 4 + 2], acc[i][jh * 4 + 3]);
+            if (!part) {
+                const float4 o = *p;
+                v.x += o.x; v.y += o.y; v.z += o.z; v.w += o.w;
+            }
+            *p = v;
         }
     }
-    (void)K1;
 }
 
 // db[n] += sum_m w(m) dY[m, n]; N in {128, 256}.  Bandwidth kernel: a CTA of 256 threads reads 8 rows x 128
-// float4-columns (N = 128: 8 rows of 32 float4) per step with 4 loads in flight per thread, block-reduces
-// through shared memory and issues one atomicAdd per column.
+// float4-columns (N = 128: 8 rows of 32 float4) per step with 4 loads in flight per thread and block-reduces
+// through shared memory in row order.  `part`: the CTA stores its column sums to part[blockIdx.x][N] (reduced in
+// CTA order by partial_sum_kernel); otherwise (one CTA) it adds them to db (and db2).
 static __global__ void __launch_bounds__(256)
-colsum_kernel(const float* __restrict__ dY, float* __restrict__ db, const float* __restrict__ roww,
-              const int32_t* __restrict__ row2agent, const int32_t* __restrict__ m_ptr, const int m_fixed,
-              const int m_cap, const int N, const int n_agents_total) {
+colsum_kernel(const float* __restrict__ dY, float* __restrict__ db, float* __restrict__ db2,
+              const float* __restrict__ roww, const int32_t* __restrict__ row2agent, const int32_t* __restrict__ m_ptr,
+              const int m_fixed, const int m_cap, const int N, const int n_agents_total, float* __restrict__ part) {
     __shared__ float4 red[256];
     int M = m_ptr ? *m_ptr : m_fixed;
     M = min(M, m_cap);
@@ -271,10 +354,18 @@ colsum_kernel(const float* __restrict__ dY, float* __restrict__ db, const float*
             const float4 o = red[r * vec_per_row + c4];
             acc.x += o.x; acc.y += o.y; acc.z += o.z; acc.w += o.w;
         }
-        atomicAdd(db + c4 * 4 + 0, acc.x);
-        atomicAdd(db + c4 * 4 + 1, acc.y);
-        atomicAdd(db + c4 * 4 + 2, acc.z);
-        atomicAdd(db + c4 * 4 + 3, acc.w);
+        if (part) {
+            *reinterpret_cast<float4*>(part + (size_t)blockIdx.x * N + c4 * 4) = acc;
+            return;
+        }
+        float* outs[2] = {db, db2};
+        for (int q = 0; q < 2; ++q) {
+            if (!outs[q]) continue;
+            float4* p = reinterpret_cast<float4*>(outs[q] + c4 * 4);
+            float4 o = *p;
+            o.x += acc.x; o.y += acc.y; o.z += acc.z; o.w += acc.w;
+            *p = o;
+        }
     }
 }
 
@@ -317,9 +408,11 @@ inline int32_t launch_gemm_nn(int epi, bool accum, const float* A, const float* 
     return check_launch("gemm_nn_kernel");
 }
 
+// `part` (optional, PART_FLOATS): split-M over up to DW_MAX_CTAS_SIMT CTAs with an ordered reduction of the splits;
+// without it one CTA per output tile walks all rows.
 inline int32_t launch_gemm_tn(const float* X, int ldx, const float* dY, float* C, const float* roww,
                               const int32_t* row2agent, RowCount rc, int K1, int N, int n_agents_total,
-                              cudaStream_t st) {
+                              cudaStream_t st, float* part = nullptr) {
     if (K1 % GEMM_BM != 0 || N % GEMM_BN != 0) {
         set_error("gemm_tn: K1=%d N=%d unsupported", K1, N);
         return -1;
@@ -330,24 +423,32 @@ inline int32_t launch_gemm_tn(const float* X, int ldx, const float* dY, float* C
     if (chunks <= 0) return 0;
     int splits = max(1, (2 * sm_count()) / tiles);
     splits = min(splits, max(1, chunks / 8));  // at least 8 chunks (128 rows) per CTA
+    splits = part ? min(splits, max(1, DW_MAX_CTAS_SIMT / tiles)) : 1;
     gemm_tn_kernel<<<tiles * splits, GEMM_THREADS, 0, st>>>(X, ldx, dY, C, roww, row2agent, rc.ptr, rc.fixed, rc.cap,
-                                                            K1, N, splits, n_agents_total);
+                                                            K1, N, splits, n_agents_total, splits > 1 ? part : nullptr);
     count_launch();
-    return check_launch("gemm_tn_kernel");
+    if (int32_t r = check_launch("gemm_tn_kernel")) return r;
+    if (splits == 1) return 0;
+    return launch_partial_sum(part, (int64_t)K1 * N, splits, PartSegs().add(C, K1 * N), st, rc.ptr, rc.cap, GEMM_BK);
 }
 
+// db (and db2, optional) += sum_m w(m) dY[m, :].  `part` (optional, PART_FLOATS): many CTAs and an ordered reduction;
+// without it one CTA walks all rows.
 inline int32_t launch_colsum(const float* dY, float* db, const float* roww, const int32_t* row2agent, RowCount rc,
-                             int N, int n_agents_total, cudaStream_t st) {
+                             int N, int n_agents_total, cudaStream_t st, float* part = nullptr, float* db2 = nullptr) {
     if (N != 128 && N != 256) {
         set_error("colsum: N=%d unsupported (128 or 256)", N);
         return -1;
     }
     const int rows = rc.ptr ? rc.cap : min(rc.fixed, rc.cap);
     if (rows <= 0) return 0;
-    const int grid = min(max(1, rows / 128), 4 * sm_count());
-    colsum_kernel<<<grid, 256, 0, st>>>(dY, db, roww, row2agent, rc.ptr, rc.fixed, rc.cap, N, n_agents_total);
+    const int grid = part ? min(min(max(1, rows / 128), 4 * sm_count()), (int)(PART_FLOATS / N)) : 1;
+    colsum_kernel<<<grid, 256, 0, st>>>(dY, db, db2, roww, row2agent, rc.ptr, rc.fixed, rc.cap, N, n_agents_total,
+                                        grid > 1 ? part : nullptr);
     count_launch();
-    return check_launch("colsum_kernel");
+    if (int32_t r = check_launch("colsum_kernel")) return r;
+    if (grid == 1) return 0;
+    return launch_partial_sum(part, N, grid, PartSegs().add(db, N, db2), st);
 }
 
 }  // namespace gcbf

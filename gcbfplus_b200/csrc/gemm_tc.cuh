@@ -481,8 +481,9 @@ inline int32_t launch_gemm_tc(int epi, bool accum, const float* A, const float* 
 // 2 stages) and the consumers transpose them while splitting into K-major SWIZZLE_128B hi / lo planes ([128 k1][32 m]
 // and [BN n][32 m]; double-buffered for BN = 128, single for BN = 256).  Rows m >= M are selected to zero (they may
 // hold stale data, possibly NaN), dY is scaled by the row weight, and the column sums sum_m w(m) dY[m, n] are taken
-// from the very values converted.  Split over M: CTA (tile, split) walks 32-row chunks {split, split + S, ...}; the
-// result is red.add'ed to C.
+// from the very values converted.  Split over M: CTA (tile, split) walks 32-row chunks {split, split + S, ...}.  With
+// more than one split each CTA stores its tile (and its column sums) to a workspace and partial_sum_kernel adds the
+// splits to C in split order: no float atomics, the same bits on every run.
 // =====================================================================================================
 constexpr int TN_RAWS = 2;
 
@@ -498,12 +499,15 @@ struct TnCfg {
 // `cs1` / `cs2` (optional): column sums sum_m w(m) dY[m, n] -- the bias gradient of the same layer (and the agent
 // one-hot row of the update layer) -- accumulated by the converting threads, so no separate pass over dY is needed.
 // Only the CTAs of k1-tile 0 contribute.
+// `part` (splits > 1): CTA (tile, split) stores its tile to part[split][K1][N] and its column sums to
+// part[split][K1 * N + n] (stride K1 * N + N); otherwise (one split) it adds them to C / cs1 / cs2 itself.
 template <int BNT>
 __global__ void __launch_bounds__(THREADS_NN, 1)
 gemm_tn_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmY,
                   float* __restrict__ C, const float* __restrict__ roww, const int32_t* __restrict__ row2agent,
                   const int32_t* __restrict__ m_ptr, const int m_fixed, const int m_cap, const int N, const int splits,
-                  const int n_agents_total, float* __restrict__ cs1, float* __restrict__ cs2) {
+                  const int n_agents_total, float* __restrict__ cs1, float* __restrict__ cs2, const int K1,
+                  float* __restrict__ part) {
     using CF = TnCfg<BNT>;
     constexpr int MR = 32 * BNT / 256;                       // m rows of dY converted per thread
     extern __shared__ uint8_t smem_raw[];
@@ -633,25 +637,38 @@ gemm_tn_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant
         if (t < BNT) {
             float v = s_cs[t];
             if (BNT == 128) v += s_cs[t + 128];
-            atomicAdd(cs1 + t, v);
-            if (cs2) atomicAdd(cs2 + t, v);
+            if (part) {
+                part[(size_t)split * ((size_t)K1 * N + N) + (size_t)K1 * N + t] = v;
+            } else {
+                cs1[t] += v;
+                if (cs2) cs2[t] += v;
+            }
         }
     }
+    float* dst = part ? part + (size_t)split * ((size_t)K1 * N + N) : C;
     const int r0 = 64 * g + frag_row0(wt);
 #pragma unroll
     for (int h = 0; h < CF::NH; ++h)
 #pragma unroll
         for (int i = 0; i < 64; i += 2) {
-            float* p = C + (size_t)(k1_0 + r0 + 8 * ((i >> 1) & 1)) * N + h * 128 + frag_col(wt, i);
-            asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(p), "f"(d[h][i]), "f"(d[h][i + 1]) : "memory");
+            float2* p = reinterpret_cast<float2*>(dst + (size_t)(k1_0 + r0 + 8 * ((i >> 1) & 1)) * N + h * 128 + frag_col(wt, i));
+            float2 v = make_float2(d[h][i], d[h][i + 1]);
+            if (!part) {
+                const float2 o = *p;
+                v.x += o.x;
+                v.y += o.y;
+            }
+            *p = v;
         }
 }
 
 // C[K1, N] += sum_m w(m) X[m, :K1] dY[m, :N]; X row stride ldx (>= K1, multiple of 4), K1 % 128 == 0, N in {128, 256}.
 // cs1 / cs2 (optional): += sum_m w(m) dY[m, :N] (bias gradient fused into the same pass over dY).
+// `part` (optional, PART_FLOATS): split-M over up to DW_MAX_CTAS_TC CTAs with an ordered reduction of the splits;
+// without it one CTA per 128-row tile of C walks all rows.
 inline int32_t launch_gemm_tn_tc(const float* X, int ldx, const float* dY, float* C, const float* roww,
                                  const int32_t* row2agent, RowCount rc, int K1, int N, int n_agents_total,
-                                 cudaStream_t st, float* cs1 = nullptr, float* cs2 = nullptr) {
+                                 cudaStream_t st, float* cs1 = nullptr, float* cs2 = nullptr, float* part = nullptr) {
     if (K1 % 128 != 0 || (N != 128 && N != 256) || ldx % 4 != 0) {
         set_error("gemm_tn_tc: K1=%d N=%d ldx=%d unsupported", K1, N, ldx);
         return -1;
@@ -665,6 +682,8 @@ inline int32_t launch_gemm_tn_tc(const float* X, int ldx, const float* dY, float
     const int chunks = (rows + 31) / 32;
     int splits = max(1, sm_count() / tiles);
     splits = min(splits, max(1, chunks * 32 / 128));       // >= 128 rows per CTA
+    splits = part ? min(splits, max(1, DW_MAX_CTAS_TC / tiles)) : 1;
+    float* kpart = splits > 1 ? part : nullptr;
     const int grid = tiles * splits;
 #define GCBF_TN_CASE(BN_)                                                                                             \
     do {                                                                                                              \
@@ -672,13 +691,18 @@ inline int32_t launch_gemm_tn_tc(const float* X, int ldx, const float* dY, float
         static bool done = false;                                                                                     \
         if (!done) { cudaFuncSetAttribute(gemm_tn_tc_kernel<BN_>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem); done = true; } \
         gemm_tn_tc_kernel<BN_><<<grid, THREADS_NN, smem, st>>>(tmX, tmY, C, roww, row2agent, rc.ptr, rc.fixed, rc.cap, N, \
-                                                               splits, n_agents_total, cs1, cs2);                     \
+                                                               splits, n_agents_total, cs1, cs2, K1, kpart);          \
     } while (0)
     if (N == 256) GCBF_TN_CASE(256);
     else GCBF_TN_CASE(128);
 #undef GCBF_TN_CASE
     count_launch();
-    return check_launch("gemm_tn_tc_kernel");
+    if (int32_t r = check_launch("gemm_tn_tc_kernel")) return r;
+    if (splits == 1) return 0;
+    PartSegs segs;
+    segs.add(C, K1 * N);
+    if (cs1) segs.add(cs1, N, cs2);
+    return launch_partial_sum(part, (int64_t)K1 * N + N, splits, segs, st, rc.ptr, rc.cap, 32);
 }
 
 }  // namespace tc

@@ -274,6 +274,69 @@ graph_build_kernel(const gcbf_env_desc d, const float* __restrict__ agent, const
 }
 
 // ------------------------------------------------------------------------------------
+// canonical edge layout.  graph_build_kernel places each CTA's rows at a base taken from an atomic ticket, so the row
+// order in edge_recv / edge_src depends on which CTA ran first.  Two passes move the rows into batch-agent order
+// (row_start[a + 1] = row_start[a] + row_deg[a], row_start[0] = 0) with edge_recv as staging; every sum over the edge
+// arrays (the train step's reductions) then sees the same layout on every run.  No CTA waits on another: each CTA
+// adds up the degrees of all agents before its own chunk itself (A^2 / (2 CANON_T) loads in all, a few microseconds
+// at the graph sizes a minibatch or a rollout chain holds).
+// ------------------------------------------------------------------------------------
+constexpr int CANON_T = 512;
+
+// pass 1: row_start <- exclusive prefix of row_deg; the row at the ticket position in edge_src is copied to its
+// canonical position in edge_recv.  Overflowed rows have row_deg = 0 and move nothing.
+__global__ void __launch_bounds__(CANON_T)
+edge_canon_stage_kernel(const int A, const int cap, int32_t* __restrict__ row_start, const int32_t* __restrict__ row_deg,
+                        const int32_t* __restrict__ edge_src, int32_t* __restrict__ edge_recv) {
+    __shared__ int s_warp[CANON_T / 32];
+    __shared__ int s_scan[CANON_T];
+    __shared__ int s_old[CANON_T];
+    const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
+    const int a0 = blockIdx.x * CANON_T;
+    int pre = 0;
+    for (int a = t; a < a0; a += CANON_T) pre += row_deg[a];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) pre += __shfl_xor_sync(0xffffffffu, pre, o);
+    if (lane == 0) s_warp[warp] = pre;
+    const int a = a0 + t;
+    const int deg = a < A ? row_deg[a] : 0;
+    s_old[t] = a < A ? row_start[a] : 0;
+    s_scan[t] = deg;
+    __syncthreads();
+    int base = 0;
+    for (int w = 0; w < CANON_T / 32; ++w) base += s_warp[w];
+    for (int o = 1; o < CANON_T; o <<= 1) {     // inclusive scan of the chunk's degrees
+        const int v = t >= o ? s_scan[t - o] : 0;
+        __syncthreads();
+        s_scan[t] += v;
+        __syncthreads();
+    }
+    if (a < A) row_start[a] = base + s_scan[t] - deg;
+    for (int q = warp; q < CANON_T && a0 + q < A; q += CANON_T / 32) {
+        const int d = row_deg[a0 + q], from = s_old[q], to = base + s_scan[q] - d;
+        if (from < 0 || from + d > cap || to + d > cap) continue;
+        for (int k = lane; k < d; k += 32) edge_recv[to + k] = edge_src[from + k];
+    }
+}
+
+// pass 2: the staged rows go back to edge_src, and edge_recv gets the receiver ids
+__global__ void __launch_bounds__(CANON_T)
+edge_canon_final_kernel(const int A, const int cap, const int32_t* __restrict__ row_start,
+                        const int32_t* __restrict__ row_deg, int32_t* __restrict__ edge_src,
+                        int32_t* __restrict__ edge_recv) {
+    const int lane = threadIdx.x & 31;
+    const int warps = (gridDim.x * blockDim.x) >> 5;
+    for (int a = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; a < A; a += warps) {
+        const int rs = row_start[a], d = row_deg[a];
+        if (rs < 0 || rs + d > cap) continue;
+        for (int k = lane; k < d; k += 32) {
+            edge_src[rs + k] = edge_recv[rs + k];
+            edge_recv[rs + k] = a;
+        }
+    }
+}
+
+// ------------------------------------------------------------------------------------
 // env step: one CTA per graph (deterministic reward / cost reductions).
 // ------------------------------------------------------------------------------------
 template <int KIND>
@@ -552,7 +615,18 @@ int32_t gcbf::graph_build_impl(const gcbf_env_desc* desc, const float* agent, co
                                                 edge_recv, edge_src, counters, flags & 1, tail, reward, cost, rounds);
     });
     count_launch();
-    return check_launch("graph_build_kernel");
+    if (int32_t rc = check_launch("graph_build_kernel")) return rc;
+    // the fused rollout step and callers that set flags bit 3 (the rollout engine) keep ticket order: rollout outputs do
+    // not depend on the layout (every edge row is computed on its own and each receiver sums its own row in order)
+    if (tail.z || (flags & 8)) return 0;
+    const int A = desc->n_graphs * desc->n_agents, cap = desc->edge_cap;
+    const int chunks = (A + CANON_T - 1) / CANON_T;
+    edge_canon_stage_kernel<<<chunks, CANON_T, 0, st>>>(A, cap, row_start, row_deg, edge_src, edge_recv);
+    count_launch();
+    if (int32_t rc = check_launch("edge_canon_stage_kernel")) return rc;
+    edge_canon_final_kernel<<<chunks, CANON_T, 0, st>>>(A, cap, row_start, row_deg, edge_src, edge_recv);
+    count_launch();
+    return check_launch("edge_canon_final_kernel");
 }
 
 // ------------------------------------------------------------------------------------

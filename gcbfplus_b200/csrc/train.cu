@@ -1,7 +1,9 @@
 // train.cu -- the GCBF+ train step: three GNN forwards with saved activations, the four
 // losses, hand-written backward (dW via split-M GEMMs, dX through the edge features, the Euler
 // step and the action clip back into the actor), global-norm clip + AdamW + apply_if_finite,
-// and the target-network polyak update.  On the tensor-core path the step runs on the folded
+// and the target-network polyak update.  Every sum that spans CTAs is taken in a fixed order (per-CTA partials in the
+// workspace, then partial_sum_kernel; per-edge input gradients gathered per agent), so the step is bit-identical from
+// run to run for the same inputs on the same GPU model.  On the tensor-core path the step runs on the folded
 // network (gnn_backward_folded / unfold_jobs below: 4 GEMMs per pass and direction instead of
 // 9-10, same gradient); the strict-fp32 SIMT path runs the layer-by-layer step.
 //
@@ -63,7 +65,8 @@ loss_kernel(const int A, const TrainHP hp, const float* __restrict__ h, const fl
             const uint8_t* __restrict__ safe_m, const uint8_t* __restrict__ unsafe_m, const float* __restrict__ action,
             const float* __restrict__ u_qp, const float* __restrict__ denoms, float* __restrict__ dh,
             float* __restrict__ dh_next, float* __restrict__ da, float* __restrict__ labelled,
-            float* __restrict__ stats) {
+            float* __restrict__ part) {
+    // part[blockIdx.x][10]: this CTA's stats, reduced in CTA order by partial_sum_kernel
     __shared__ float red[10][8];
     float loc[10];
 #pragma unroll
@@ -121,11 +124,12 @@ loss_kernel(const int A, const TrainHP hp, const float* __restrict__ h, const fl
     if (threadIdx.x < 10) {
         float s = 0.f;
         for (int w = 0; w < 8; ++w) s += red[threadIdx.x][w];
-        atomicAdd(stats + threadIdx.x, s);
+        part[blockIdx.x * 10 + threadIdx.x] = s;
     }
 }
 
-// counts of the label masks (denominators; all-reduced across ranks by the host)
+// counts of the label masks (denominators; all-reduced across ranks by the host).  The atomics add integer-valued
+// floats, which is exact -- hence order-independent -- while the counts stay below 2^24 agents per minibatch.
 __global__ void mask_count_kernel(const int A, const uint8_t* __restrict__ safe_m, const uint8_t* __restrict__ unsafe_m,
                                   float* __restrict__ denoms) {
     float us = 0.f, sf = 0.f;
@@ -147,9 +151,10 @@ __global__ void mask_count_kernel(const int A, const uint8_t* __restrict__ safe_
 __global__ void __launch_bounds__(256)
 head_out_bwd_kernel(const int A, const int nout, const float* __restrict__ H2, const float* __restrict__ W,
                     const float* __restrict__ out, const float* __restrict__ d_out, const float* __restrict__ roww,
-                    float* __restrict__ dH2, float* __restrict__ dW, float* __restrict__ db, const int mask_relu) {
+                    float* __restrict__ dH2, float* __restrict__ part, const int mask_relu) {
     // mask_relu (folded train step): H2 is the ReLU output feeding the folded output layer; dH2 is masked by H2 > 0 here
-    const int lane = threadIdx.x & 31;
+    // part (nullptr: data-only backward): part[blockIdx.x][257 nout] = this CTA's [dW (256 x nout) | db (nout)]
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int warps_total = (gridDim.x * blockDim.x) >> 5;
     float wacc[8][4], bacc[4];
 #pragma unroll
@@ -213,24 +218,30 @@ head_out_bwd_kernel(const int A, const int nout, const float* __restrict__ H2, c
             dst[1] = make_float4(dh[4], dh[5], dh[6], dh[7]);
         }
     }
-    if (!dW) return;   // data-only backward (QP labels): no parameter gradient
-    // block-level reduction first: one atomic per (row, column) and CTA instead of one per warp
-    __shared__ float s_w[256 * 4 + 4];       // [k][j][lane]: the 32 lanes of a warp hit 32 different banks
-    for (int i = threadIdx.x; i < 256 * 4 + 4; i += blockDim.x) s_w[i] = 0.f;
-    __syncthreads();
+    if (!part) return;   // data-only backward (QP labels): no parameter gradient
+    // one slot per warp, summed over the 8 warps in warp order
+    __shared__ float s_w[8][256 * 4 + 4];    // [warp][k][j][lane]: the 32 lanes of a warp hit 32 different banks
 #pragma unroll
     for (int k = 0; k < 8; ++k)
 #pragma unroll
         for (int j = 0; j < 4; ++j)
-            if (j < nout) atomicAdd(&s_w[(k * 4 + j) * 32 + lane], wacc[k][j]);
+            if (j < nout) s_w[warp][(k * 4 + j) * 32 + lane] = wacc[k][j];
     if (lane == 0)      // bacc is warp-uniform (every lane sees the same dz)
-        for (int j = 0; j < nout; ++j) atomicAdd(&s_w[1024 + j], bacc[j]);
+        for (int j = 0; j < nout; ++j) s_w[warp][1024 + j] = bacc[j];
     __syncthreads();
-    for (int i = threadIdx.x; i < 256 * nout; i += blockDim.x) {
-        const int row = i / nout, j = i % nout;          // W row = lane * 8 + k
-        atomicAdd(dW + i, s_w[((row & 7) * 4 + j) * 32 + (row >> 3)]);
+    float* dst = part + (size_t)blockIdx.x * 257 * nout;
+    for (int i = threadIdx.x; i < 257 * nout; i += blockDim.x) {
+        int idx;
+        if (i < 256 * nout) {
+            const int row = i / nout, j = i % nout;      // W row = lane * 8 + k
+            idx = ((row & 7) * 4 + j) * 32 + (row >> 3);
+        } else {
+            idx = 1024 + i - 256 * nout;
+        }
+        float v = 0.f;
+        for (int w = 0; w < 8; ++w) v += s_w[w][idx];
+        dst[i] = v;
     }
-    if (threadIdx.x < nout) atomicAdd(db + threadIdx.x, s_w[1024 + threadIdx.x]);
 }
 
 // ------------------------------------------------------------------------------------ backward: attention + aggregation
@@ -242,10 +253,11 @@ attn_aggregate_bwd_kernel(const int A, const int edge_cap, const float* __restri
                           const float* __restrict__ G2, const float* __restrict__ ATT, const float* __restrict__ a3,
                           const int32_t* __restrict__ row_start, const int32_t* __restrict__ row_deg,
                           const float* __restrict__ roww, float* __restrict__ dMSG, float* __restrict__ dG2,
-                          float* __restrict__ da3, float* __restrict__ dba3, const int mask_relu) {
+                          float* __restrict__ part, const int mask_relu) {
     // mask_relu (folded train step): G2 is the ReLU output of the gate's first layer and a3 the folded gate vector;
     // dG2 is masked by G2 > 0 here
-    const int lane = threadIdx.x & 31;
+    // part (nullptr: data-only backward): part[blockIdx.x][129] = this CTA's [da3 (128) | dba3]
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int warps_total = (gridDim.x * blockDim.x) >> 5;
     const float4 w3 = *reinterpret_cast<const float4*>(a3 + lane * 4);
     float4 acc3 = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -329,30 +341,34 @@ attn_aggregate_bwd_kernel(const int A, const int edge_cap, const float* __restri
             accb += wd;
         }
     }
-    if (!da3) return;  // data-only backward
-    __shared__ float s_a[132];
-    for (int i = threadIdx.x; i < 132; i += blockDim.x) s_a[i] = 0.f;
-    __syncthreads();
-    atomicAdd(&s_a[0 * 32 + lane], acc3.x);       // [component][lane]: conflict-free
-    atomicAdd(&s_a[1 * 32 + lane], acc3.y);
-    atomicAdd(&s_a[2 * 32 + lane], acc3.z);
-    atomicAdd(&s_a[3 * 32 + lane], acc3.w);
+    if (!part) return;  // data-only backward
+    __shared__ float s_a[8][132];                 // [warp][component][lane]: conflict-free; summed in warp order
+    s_a[warp][0 * 32 + lane] = acc3.x;
+    s_a[warp][1 * 32 + lane] = acc3.y;
+    s_a[warp][2 * 32 + lane] = acc3.z;
+    s_a[warp][3 * 32 + lane] = acc3.w;
     accb = warp_sum(accb);
-    if (lane == 0) atomicAdd(&s_a[128], accb);
+    if (lane == 0) s_a[warp][128] = accb;
     __syncthreads();
-    if (threadIdx.x < 128) atomicAdd(da3 + threadIdx.x, s_a[(threadIdx.x & 3) * 32 + (threadIdx.x >> 2)]);
-    if (threadIdx.x == 128) atomicAdd(dba3, s_a[128]);
+    if (threadIdx.x < 129) {
+        const int idx = threadIdx.x < 128 ? (threadIdx.x & 3) * 32 + (threadIdx.x >> 2) : 128;
+        float v = 0.f;
+        for (int w = 0; w < 8; ++w) v += s_a[w][idx];
+        part[(size_t)blockIdx.x * 129 + threadIdx.x] = v;
+    }
 }
 
 // ------------------------------------------------------------------------------------ backward: edge layer 1
 // dY = dX1pre [nE,256] (already masked by X1 > 0).  dW1[:ed] += feat^T (w dY); dW1[ed+t] += sum_{type t} w dY;
 // dW1[ed+5] += sum w dY; db1 += sum w dY.  Thread = output column; CTA = strided chunk of edges.
+// part[blockIdx.x][(ED + 4) x 256]: this CTA's rows 0 .. ED+2 of dW1 and the all-edge sum (dW1[ED+5] and db1).
+__host__ __device__ constexpr int edge_l1_part_floats(int ed) { return (ed + 4) * 256; }
 template <int ED>
 __global__ void __launch_bounds__(256)
 edge_l1_bwd_w_kernel(const int edge_cap, const int n_agents_total, const int32_t* __restrict__ counters,
                      const float* __restrict__ dY, const float* __restrict__ feat,
                      const int32_t* __restrict__ edge_src, const int32_t* __restrict__ edge_recv,
-                     const float* __restrict__ roww, float* __restrict__ dW1, float* __restrict__ db1) {
+                     const float* __restrict__ roww, float* __restrict__ part) {
     // chunks of 64 edges: the per-edge metadata (features, sender type, row weight) is staged in shared memory so that the
     // dY loads of a chunk are independent of it and 8 of them are in flight per thread
     constexpr int CH = 64;
@@ -404,23 +420,23 @@ edge_l1_bwd_w_kernel(const int edge_cap, const int n_agents_total, const int32_t
             }
         }
     }
+    float* dst = part + (size_t)blockIdx.x * edge_l1_part_floats(ED);
 #pragma unroll
-    for (int i = 0; i < ED; ++i) atomicAdd(dW1 + i * 256 + c, accw[i]);
+    for (int i = 0; i < ED; ++i) dst[i * 256 + c] = accw[i];
 #pragma unroll
-    for (int t = 0; t < 3; ++t) atomicAdd(dW1 + (ED + t) * 256 + c, acct[t]);
-    atomicAdd(dW1 + (ED + 3 + 2) * 256 + c, accall);
-    atomicAdd(db1 + c, accall);
+    for (int t = 0; t < 3; ++t) dst[(ED + t) * 256 + c] = acct[t];
+    dst[(ED + 3) * 256 + c] = accall;
 }
 
-// dfeat = dY @ W1[:ed]^T, through the norm-clip, scattered to d_es[recv] (+) and d_es[sender agent] (-).
-// d_es is in edge-state space ([A, ED]); one warp per edge.
+// dfeat = dY @ W1[:ed]^T through the norm-clip, per edge: je[e][:ED] = d out[recv] / d feat_e (edge-state space).
+// The QP labels use it as the Jacobian block; the train step gathers it per agent (edge_grad_gather_kernel).
+// One warp per edge.
 template <int KIND>
 __global__ void __launch_bounds__(256)
 edge_l1_bwd_x_kernel(const gcbf_env_desc d, const float* __restrict__ W1, const float* __restrict__ dY,
                      const float* __restrict__ agent, const float* __restrict__ goal, const float* __restrict__ hits,
                      const int32_t* __restrict__ edge_recv, const int32_t* __restrict__ edge_src,
-                     const int32_t* __restrict__ counters, const int clip_all, float* __restrict__ d_es,
-                     float* __restrict__ je) {
+                     const int32_t* __restrict__ counters, const int clip_all, float* __restrict__ je) {
     using T = EnvTraits<KIND>;
     constexpr int ED = T::ED, SD = T::SD, PD = T::PD;
     __shared__ __align__(16) float sW[ED][256];
@@ -459,18 +475,47 @@ edge_l1_bwd_x_kernel(const gcbf_env_desc d, const float* __restrict__ W1, const 
 #pragma unroll
                 for (int p = 0; p < PD; ++p) df[p] = coef * (df[p] - (er[p] - es[p]) * dotp * inv_n2);
             }
-            if (je) {   // per-edge Jacobian block d out[recv] / d feat_e (QP labels): no reduction
 #pragma unroll
-                for (int c = 0; c < ED; ++c) je[(size_t)e * 8 + c] = df[c];
-                continue;
-            }
+            for (int c = 0; c < ED; ++c) je[(size_t)e * 8 + c] = df[c];
+        }
+    }
+}
+
+// d_es[a] = sum_{e in row a} je[e] - sum_{e : sender(e) = a} je[e]: feat_e = es(recv) - es(sender).  The edges sent by
+// agent a are the mirrors of a's agent edges -- edge a -> j lies in row j, since the radius graph is symmetric -- so
+// every agent reads its own row and its neighbours' rows, in row order, and writes its gradient once.
+template <int ED>
+__global__ void __launch_bounds__(128)
+edge_grad_gather_kernel(const int A, const int edge_cap, const int32_t* __restrict__ row_start,
+                        const int32_t* __restrict__ row_deg, const int32_t* __restrict__ edge_src,
+                        const float* __restrict__ je, float* __restrict__ d_es) {
+    const int a = blockIdx.x * blockDim.x + threadIdx.x;
+    if (a >= A) return;
+    float s[ED];
 #pragma unroll
-            for (int c = 0; c < ED; ++c) {
-                atomicAdd(d_es + (size_t)a * ED + c, df[c]);
-                if (code >= 0) atomicAdd(d_es + (size_t)code * ED + c, -df[c]);
+    for (int c = 0; c < ED; ++c) s[c] = 0.f;
+    const int rs = row_start[a];
+    int rd = row_deg[a];
+    if (rs < 0 || rs + rd > edge_cap) rd = 0;
+    for (int e = rs; e < rs + rd; ++e)
+#pragma unroll
+        for (int c = 0; c < ED; ++c) s[c] += je[(size_t)e * 8 + c];
+    for (int e = rs; e < rs + rd; ++e) {
+        const int j = edge_src[e];
+        if (j < 0 || j >= A) continue;
+        const int rs2 = row_start[j];
+        int rd2 = row_deg[j];
+        if (rs2 < 0 || rs2 + rd2 > edge_cap) rd2 = 0;
+        for (int e2 = rs2; e2 < rs2 + rd2; ++e2) {
+            if (edge_src[e2] == a) {
+#pragma unroll
+                for (int c = 0; c < ED; ++c) s[c] -= je[(size_t)e2 * 8 + c];
+                break;
             }
         }
     }
+#pragma unroll
+    for (int c = 0; c < ED; ++c) d_es[(size_t)a * ED + c] = s[c];
 }
 
 // d_es (edge-state grads of x') -> d pi.   x' = clip_state(x + xdot(x, u) dt), u = clip_action(a),
@@ -552,20 +597,88 @@ struct BwdArgs {
     const float *agent, *goal, *hits;
     const int32_t *row_start, *row_deg, *edge_recv, *edge_src, *counters;
     int clip_all;
-    float* d_es;           // optional [A, ED] (accumulated) : gradient wrt the agents' edge states
-    float* je;             // optional [cap, 8]: per-edge d out[recv] / d feat_e instead of the d_es reduction
+    float* d_es;           // optional [A, ED] (written): gradient wrt the agents' edge states, gathered from `je`
+    float* je;             // [cap, 8] when d_es is wanted or the per-edge blocks are the result: d out[recv] / d feat_e
+    float* part;           // PART_FLOATS: per-CTA partials of the weight-gradient reductions (when G is set)
     int use_tc;            // 1: backward-data GEMMs on the wgmma path
 };
+
+// ---- the parameter-gradient kernels followed by the ordered sum of their per-CTA partials
+static int grid_for_part(int grid, int64_t part_floats) {
+    return min(grid, (int)(PART_FLOATS / part_floats));
+}
+
+// output layer: dW, db (nullptr: data-only) and dH2
+static int32_t head_out_bwd(const BwdArgs& b, int grid, const float* H2, const float* W, float* dH2, float* dW, float* db,
+                            int mask_relu, cudaStream_t st) {
+    const int A = b.d->n_graphs * b.d->n_agents, no = b.out_dim;
+    grid = grid_for_part(grid, 257 * no);
+    head_out_bwd_kernel<<<grid, 256, 0, st>>>(A, no, H2, W, b.out, b.d_out, b.roww, dH2, dW ? b.part : nullptr, mask_relu);
+    count_launch();
+    if (int32_t rc = check_launch("head_out_bwd_kernel")) return rc;
+    if (!dW) return 0;
+    return launch_partial_sum(b.part, 257 * no, grid, PartSegs().add(dW, 256 * no).add(db, no), st);
+}
+
+// attention + aggregation: dMSG, dG2 and (da3 != nullptr) the gate vector's gradient da3, dba3
+static int32_t attn_aggregate_bwd(const BwdArgs& b, int grid, const float* dAG, const float* MSG, const float* G2,
+                                  const float* ATT, const float* a3, float* dMSG, float* dG2, float* da3, float* dba3,
+                                  int mask_relu, cudaStream_t st) {
+    const int A = b.d->n_graphs * b.d->n_agents;
+    grid = grid_for_part(grid, 129);
+    attn_aggregate_bwd_kernel<<<grid, 256, 0, st>>>(A, b.d->edge_cap, dAG, MSG, G2, ATT, a3, b.row_start, b.row_deg,
+                                                    b.roww, dMSG, dG2, da3 ? b.part : nullptr, mask_relu);
+    count_launch();
+    if (int32_t rc = check_launch("attn_aggregate_bwd_kernel")) return rc;
+    if (!da3) return 0;
+    return launch_partial_sum(b.part, 129, grid, PartSegs().add(da3, 128).add(dba3, 1), st);
+}
+
+// edge layer 1: dW1 / db1 (wgrad) from the saved features, and the per-edge input gradient je, gathered into d_es
+static int32_t edge_l1_bwd(const BwdArgs& b, const ParamLayout& L, const float* dY, const float* feat, bool wgrad,
+                           cudaStream_t st) {
+    const gcbf_env_desc* d = b.d;
+    const int ed = env_ed(d->env_kind), cap = d->edge_cap, A = d->n_graphs * d->n_agents, nsm = sm_count();
+    if (wgrad) {
+        float* dW1 = b.G + L.w[L_MSG0];
+        const int grid = grid_for_part(min(max(cap / 64, 1), 4 * nsm), edge_l1_part_floats(ed));   // chunks of 64 edges
+        switch (ed) {
+            case 2: edge_l1_bwd_w_kernel<2><<<grid, 256, 0, st>>>(cap, A, b.counters, dY, feat, b.edge_src, b.edge_recv, b.roww, b.part); break;
+            case 4: edge_l1_bwd_w_kernel<4><<<grid, 256, 0, st>>>(cap, A, b.counters, dY, feat, b.edge_src, b.edge_recv, b.roww, b.part); break;
+            default: edge_l1_bwd_w_kernel<6><<<grid, 256, 0, st>>>(cap, A, b.counters, dY, feat, b.edge_src, b.edge_recv, b.roww, b.part); break;
+        }
+        count_launch();
+        if (int32_t rc = check_launch("edge_l1_bwd_w_kernel")) return rc;
+        if (int32_t rc = launch_partial_sum(b.part, edge_l1_part_floats(ed), grid,
+                                            PartSegs().add(dW1, (ed + 3) * 256).add(dW1 + (ed + 5) * 256, 256, b.G + L.b[L_MSG0]),
+                                            st))
+            return rc;
+    }
+    if (!b.je) return 0;
+    const int grid = min((cap + 7) / 8, 4 * nsm);
+    GCBF_DISPATCH_ENV(d->env_kind, {
+        edge_l1_bwd_x_kernel<KIND><<<grid, 256, 0, st>>>(*d, b.P + L.w[L_MSG0], dY, b.agent, b.goal, b.hits, b.edge_recv,
+                                                         b.edge_src, b.counters, b.clip_all, b.je);
+    });
+    count_launch();
+    if (int32_t rc = check_launch("edge_l1_bwd_x_kernel")) return rc;
+    if (!b.d_es) return 0;
+    switch (ed) {
+        case 2: edge_grad_gather_kernel<2><<<(A + 127) / 128, 128, 0, st>>>(A, cap, b.row_start, b.row_deg, b.edge_src, b.je, b.d_es); break;
+        case 4: edge_grad_gather_kernel<4><<<(A + 127) / 128, 128, 0, st>>>(A, cap, b.row_start, b.row_deg, b.edge_src, b.je, b.d_es); break;
+        default: edge_grad_gather_kernel<6><<<(A + 127) / 128, 128, 0, st>>>(A, cap, b.row_start, b.row_deg, b.edge_src, b.je, b.d_es); break;
+    }
+    count_launch();
+    return check_launch("edge_grad_gather_kernel");
+}
 
 // dW += X^T (w dY) and db (+ db2) += sum_m w dY: the SIMT split-M kernel followed by column-sum launches.  Only
 // the SIMT train step computes weight gradients layer by layer; the folded step has its own (gnn_backward_folded).
 static int32_t dense_bwd_weight(const BwdArgs& b, const float* X, int ldx, const float* dY, float* C, float* db,
                                 float* db2, const int32_t* row2agent, RowCount rc, int K1, int N, int A,
                                 cudaStream_t st) {
-    if (int32_t r = launch_gemm_tn(X, ldx, dY, C, b.roww, row2agent, rc, K1, N, A, st)) return r;
-    if (int32_t r = launch_colsum(dY, db, b.roww, row2agent, rc, N, A, st)) return r;
-    if (db2) return launch_colsum(dY, db2, b.roww, row2agent, rc, N, A, st);
-    return 0;
+    if (int32_t r = launch_gemm_tn(X, ldx, dY, C, b.roww, row2agent, rc, K1, N, A, st, b.part)) return r;
+    return launch_colsum(dY, db, b.roww, row2agent, rc, N, A, st, b.part, db2);
 }
 
 // dX = epi(dY @ W_i^T) (+= if accum).  SIMT: B = W^T from PT; tensor core: Bt = W itself (K-major).
@@ -600,13 +713,8 @@ static int32_t gnn_backward_impl(const BwdArgs& b, cudaStream_t st) {
 #define RC(x) do { if ((rc = (x))) return rc; } while (0)
 #define WG(x) do { if (wgrad) RC(x); } while (0)
     // ---- output layer
-    {
-        const int grid = min((A + 7) / 8, 2 * nsm);
-        head_out_bwd_kernel<<<grid, 256, 0, st>>>(A, b.out_dim, fw + W.h2, b.P + L.w[L_OUT], b.out, b.d_out, b.roww,
-                                                  gw + W.h2, wgrad ? Gz + L.w[L_OUT] : nullptr, wgrad ? Gz + L.b[L_OUT] : nullptr, 0);
-        count_launch();
-        RC(check_launch("head_out_bwd_kernel"));
-    }
+    RC(head_out_bwd(b, min((A + 7) / 8, 2 * nsm), fw + W.h2, b.P + L.w[L_OUT], gw + W.h2,
+                    wgrad ? Gz + L.w[L_OUT] : nullptr, wgrad ? Gz + L.b[L_OUT] : nullptr, 0, st));
     // ---- head MLP
     WG(dense_bwd_weight(b, fw + W.h1, 256, gw + W.h2, b.G + L.w[L_HEAD1], b.G + L.b[L_HEAD1], nullptr, nullptr, ra, 256, 256, A, st));
     RC(dense_bwd_data(b, L, TL, L_HEAD1, EPI_RELU_MASK, false, gw + W.h2, gw + W.h1, fw + W.h1, ra, st));
@@ -620,14 +728,9 @@ static int32_t gnn_backward_impl(const BwdArgs& b, cudaStream_t st) {
     WG(dense_bwd_weight(b, fw + W.ag, 128, gw + W.v1, b.G + L.w[L_UPD0] + 3 * 256, b.G + L.b[L_UPD0], b.G + L.w[L_UPD0] + 2 * 256, nullptr, ra, 128, 256, A, st));
     RC(dense_bwd_data(b, L, TL, L_UPD0, EPI_NONE, false, gw + W.v1, gw + W.ag, nullptr, ra, st));
     // ---- attention + aggregation
-    {
-        const int grid = min((A + 7) / 8, 2 * nsm);
-        attn_aggregate_bwd_kernel<<<grid, 256, 0, st>>>(A, cap, gw + W.ag, fw + W.msg, fw + W.g2, fw + W.att,
-                                                        b.P + L.w[L_GATE], b.row_start, b.row_deg, b.roww, gw + W.msg,
-                                                        gw + W.g2, wgrad ? Gz + L.w[L_GATE] : nullptr, wgrad ? Gz + L.b[L_GATE] : nullptr, 0);
-        count_launch();
-        RC(check_launch("attn_aggregate_bwd_kernel"));
-    }
+    RC(attn_aggregate_bwd(b, min((A + 7) / 8, 2 * nsm), gw + W.ag, fw + W.msg, fw + W.g2, fw + W.att, b.P + L.w[L_GATE],
+                          gw + W.msg, gw + W.g2, wgrad ? Gz + L.w[L_GATE] : nullptr, wgrad ? Gz + L.b[L_GATE] : nullptr, 0,
+                          st));
     // ---- gate MLP (edge rows; dW weighted by the receiver's weight)
     WG(dense_bwd_weight(b, fw + W.g1, 128, gw + W.g2, b.G + L.w[L_ATT1], b.G + L.b[L_ATT1], nullptr, b.edge_recv, re, 128, 128, A, st));
     RC(dense_bwd_data(b, L, TL, L_ATT1, EPI_RELU_MASK, false, gw + W.g2, gw + W.g1, fw + W.g1, re, st));
@@ -639,25 +742,7 @@ static int32_t gnn_backward_impl(const BwdArgs& b, cudaStream_t st) {
     WG(dense_bwd_weight(b, fw + W.x1, 256, gw + W.x2, b.G + L.w[L_MSG1], b.G + L.b[L_MSG1], nullptr, b.edge_recv, re, 256, 256, A, st));
     RC(dense_bwd_data(b, L, TL, L_MSG1, EPI_RELU_MASK, false, gw + W.x2, gw + W.x1, fw + W.x1, re, st));
     // ---- edge layer 1
-    if (wgrad) {
-        const int grid = min(max(cap / 64, 1), 4 * nsm);   // one CTA walks chunks of 64 edges
-        switch (ed) {
-            case 2: edge_l1_bwd_w_kernel<2><<<grid, 256, 0, st>>>(cap, A, b.counters, gw + W.x1, fw + W.feat, b.edge_src, b.edge_recv, b.roww, b.G + L.w[L_MSG0], b.G + L.b[L_MSG0]); break;
-            case 4: edge_l1_bwd_w_kernel<4><<<grid, 256, 0, st>>>(cap, A, b.counters, gw + W.x1, fw + W.feat, b.edge_src, b.edge_recv, b.roww, b.G + L.w[L_MSG0], b.G + L.b[L_MSG0]); break;
-            default: edge_l1_bwd_w_kernel<6><<<grid, 256, 0, st>>>(cap, A, b.counters, gw + W.x1, fw + W.feat, b.edge_src, b.edge_recv, b.roww, b.G + L.w[L_MSG0], b.G + L.b[L_MSG0]); break;
-        }
-        count_launch();
-        RC(check_launch("edge_l1_bwd_w_kernel"));
-    }
-    if (b.d_es || b.je) {
-        const int grid = min((cap + 7) / 8, 4 * nsm);
-        GCBF_DISPATCH_ENV(d->env_kind, {
-            edge_l1_bwd_x_kernel<KIND><<<grid, 256, 0, st>>>(*d, b.P + L.w[L_MSG0], gw + W.x1, b.agent, b.goal, b.hits,
-                                                             b.edge_recv, b.edge_src, b.counters, b.clip_all, b.d_es, b.je);
-        });
-        count_launch();
-        RC(check_launch("edge_l1_bwd_x_kernel"));
-    }
+    RC(edge_l1_bwd(b, L, gw + W.x1, fw + W.feat, wgrad, st));
 #undef WG
 #undef RC
     return 0;
@@ -699,57 +784,29 @@ static int32_t gnn_backward_folded(const BwdArgs& b, const float* blob, float* G
         return tc::launch_gemm_tc(epi, accum, dY, blob + p_off, blob + p_off + K * N, nullptr, nullptr, dX, aux, rows, K, N, st);
     };
     // ---- folded output layer: z = h1 HO + bho, out = tanh(z); dh1 masked by h1 > 0
-    {
-        const int grid = min((A + 7) / 8, 2 * nsm);   // (4 x nsm measured slower: 65.6 vs 54.4 us -- more end-of-kernel atomics)
-        head_out_bwd_kernel<<<grid, 256, 0, st>>>(A, b.out_dim, fw + W.h1, blob + I.ho, b.out, b.d_out, b.roww, gw + W.h1,
-                                                  Gf + I.ho, Gf + I.bho, 1);
-        count_launch();
-        RC(check_launch("head_out_bwd_kernel"));
-    }
+    RC(head_out_bwd(b, min((A + 7) / 8, 2 * nsm), fw + W.h1, blob + I.ho, gw + W.h1, Gf + I.ho, Gf + I.bho, 1, st));
     // ---- h1 = relu(v1 UH + buh)
-    RC(tc::launch_gemm_tn_tc(fw + W.v1, 256, gw + W.h1, Gf + I.uh, b.roww, nullptr, ra, 256, 256, A, st, Gf + I.buh, nullptr));
+    RC(tc::launch_gemm_tn_tc(fw + W.v1, 256, gw + W.h1, Gf + I.uh, b.roww, nullptr, ra, 256, 256, A, st, Gf + I.buh, nullptr,
+                             b.part));
     RC(data(EPI_RELU_MASK, false, gw + W.h1, I.p_uh, 256, 256, gw + W.v1, fw + W.v1, ra));
     // ---- v1 = relu(ag U1[3:] + U1[2] + bu1)
     RC(tc::launch_gemm_tn_tc(fw + W.ag, 128, gw + W.v1, b.G + L.w[L_UPD0] + 3 * 256, b.roww, nullptr, ra, 128, 256, A, st,
-                             b.G + L.b[L_UPD0], b.G + L.w[L_UPD0] + 2 * 256));
+                             b.G + L.b[L_UPD0], b.G + L.w[L_UPD0] + 2 * 256, b.part));
     RC(data(EPI_NONE, false, gw + W.v1, I.p_u1, 256, 128, gw + W.ag, nullptr, ra));
     // ---- attention + aggregation with the folded gate vector (g1 = relu output of the gate's first layer)
-    {
-        const int grid = min((A + 7) / 8, 6 * nsm);   // latency-bound warp-per-receiver loop: as many warps in flight as fit
-        attn_aggregate_bwd_kernel<<<grid, 256, 0, st>>>(A, cap, gw + W.ag, fw + W.msg, fw + W.g1, fw + W.att, blob + I.a23,
-                                                        b.row_start, b.row_deg, b.roww, gw + W.msg, gw + W.g1, Gf + I.a23,
-                                                        Gf + I.c23, 1);
-        count_launch();
-        RC(check_launch("attn_aggregate_bwd_kernel"));
-    }
+    // (latency-bound warp-per-receiver loop: as many warps in flight as fit)
+    RC(attn_aggregate_bwd(b, min((A + 7) / 8, 6 * nsm), gw + W.ag, fw + W.msg, fw + W.g1, fw + W.att, blob + I.a23,
+                          gw + W.msg, gw + W.g1, Gf + I.a23, Gf + I.c23, 1, st));
     // ---- g1 = relu(msg A1 + ba1)
     RC(tc::launch_gemm_tn_tc(fw + W.msg, 128, gw + W.g1, b.G + L.w[L_ATT0], b.roww, b.edge_recv, re, 128, 128, A, st,
-                             b.G + L.b[L_ATT0], nullptr));
+                             b.G + L.b[L_ATT0], nullptr, b.part));
     RC(data(EPI_NONE, true, gw + W.g1, I.p_a1, 128, 128, gw + W.msg, nullptr, re));
     // ---- msg = x1 W23 + b23
     RC(tc::launch_gemm_tn_tc(fw + W.x1, 256, gw + W.msg, Gf + I.w23, b.roww, b.edge_recv, re, 256, 128, A, st, Gf + I.b23,
-                             nullptr));
+                             nullptr, b.part));
     RC(data(EPI_RELU_MASK, false, gw + W.msg, I.p_w23, 128, 256, gw + W.x1, fw + W.x1, re));
     // ---- edge layer 1
-    {
-        const int grid = min(max(cap / 64, 1), 4 * nsm);
-        switch (ed) {
-            case 2: edge_l1_bwd_w_kernel<2><<<grid, 256, 0, st>>>(cap, A, b.counters, gw + W.x1, fw + W.feat, b.edge_src, b.edge_recv, b.roww, b.G + L.w[L_MSG0], b.G + L.b[L_MSG0]); break;
-            case 4: edge_l1_bwd_w_kernel<4><<<grid, 256, 0, st>>>(cap, A, b.counters, gw + W.x1, fw + W.feat, b.edge_src, b.edge_recv, b.roww, b.G + L.w[L_MSG0], b.G + L.b[L_MSG0]); break;
-            default: edge_l1_bwd_w_kernel<6><<<grid, 256, 0, st>>>(cap, A, b.counters, gw + W.x1, fw + W.feat, b.edge_src, b.edge_recv, b.roww, b.G + L.w[L_MSG0], b.G + L.b[L_MSG0]); break;
-        }
-        count_launch();
-        RC(check_launch("edge_l1_bwd_w_kernel"));
-    }
-    if (b.d_es) {
-        const int grid = min((cap + 7) / 8, 4 * nsm);
-        GCBF_DISPATCH_ENV(d->env_kind, {
-            edge_l1_bwd_x_kernel<KIND><<<grid, 256, 0, st>>>(*d, b.P + L.w[L_MSG0], gw + W.x1, b.agent, b.goal, b.hits,
-                                                             b.edge_recv, b.edge_src, b.counters, b.clip_all, b.d_es, nullptr);
-        });
-        count_launch();
-        RC(check_launch("edge_l1_bwd_x_kernel"));
-    }
+    RC(edge_l1_bwd(b, L, gw + W.x1, fw + W.feat, true, st));
 #undef RC
     return 0;
 }
@@ -924,7 +981,7 @@ struct TrainNetWs {
 struct TrainWs {
     int64_t ws0, ws1, ws2, gws;
     TrainNetWs net_cbf, net_act;
-    int64_t h, hn, pi, act, xn, d_es, dh, dhn, da, dpi, lab, total;
+    int64_t h, hn, pi, act, xn, d_es, je, dh, dhn, da, dpi, lab, part, total;
 };
 static TrainWs make_train_ws(const gcbf_env_desc* d) {
     const int ed = env_ed(d->env_kind), nu = env_nu(d->env_kind), sd = env_sd(d->env_kind);
@@ -956,11 +1013,13 @@ static TrainWs make_train_ws(const gcbf_env_desc* d) {
     t.act = take(A * nu);
     t.xn = take(A * sd);
     t.d_es = take(A * ed);
+    t.je = take((int64_t)d->edge_cap * 8);
     t.dh = take(A);
     t.dhn = take(A);
     t.da = take(A * nu);
     t.dpi = take(A * nu);
     t.lab = take(A);
+    t.part = take(PART_FLOATS);
     t.total = o;
     return t;
 }
@@ -1026,8 +1085,7 @@ extern "C" __attribute__((visibility("default"))) int32_t gcbf_train_step(
     cudaError_t e;
     if ((e = cudaMemsetAsync(grad_cbf, 0, sizeof(float) * Lc.total, st)) != cudaSuccess ||
         (e = cudaMemsetAsync(grad_actor, 0, sizeof(float) * La.total, st)) != cudaSuccess ||
-        (e = cudaMemsetAsync(stats, 0, sizeof(float) * 16, st)) != cudaSuccess ||
-        (e = cudaMemsetAsync(ws + TW.d_es, 0, sizeof(float) * (size_t)A * ed, st)) != cudaSuccess) {
+        (e = cudaMemsetAsync(stats, 0, sizeof(float) * 16, st)) != cudaSuccess) {
         set_error("cudaMemsetAsync: %s", cudaGetErrorString(e));
         return (int32_t)e;
     }
@@ -1070,12 +1128,13 @@ extern "C" __attribute__((visibility("default"))) int32_t gcbf_train_step(
         const int grid = min((A + 255) / 256, 2 * sm_count());
         if (nu == 2)
             loss_kernel<2><<<grid, 256, 0, st>>>(A, hp, ws + TW.h, ws + TW.hn, safe_mask, unsafe_mask, ws + TW.act, u_qp,
-                                                 denoms, ws + TW.dh, ws + TW.dhn, ws + TW.da, ws + TW.lab, stats);
+                                                 denoms, ws + TW.dh, ws + TW.dhn, ws + TW.da, ws + TW.lab, ws + TW.part);
         else
             loss_kernel<3><<<grid, 256, 0, st>>>(A, hp, ws + TW.h, ws + TW.hn, safe_mask, unsafe_mask, ws + TW.act, u_qp,
-                                                 denoms, ws + TW.dh, ws + TW.dhn, ws + TW.da, ws + TW.lab, stats);
+                                                 denoms, ws + TW.dh, ws + TW.dhn, ws + TW.da, ws + TW.lab, ws + TW.part);
         count_launch();
         RC(check_launch("loss_kernel"));
+        RC(launch_partial_sum(ws + TW.part, 10, grid, PartSegs().add(stats, 10), st));
     }
     // ---- backward 1: cbf on g' (dW only from labelled receivers; dX from all) -> d_es
     BwdArgs b;
@@ -1099,7 +1158,8 @@ extern "C" __attribute__((visibility("default"))) int32_t gcbf_train_step(
     b.G = grad_cbf;
     b.clip_all = 1;
     b.d_es = ws + TW.d_es;
-    b.je = nullptr;
+    b.je = ws + TW.je;
+    b.part = ws + TW.part;
     b.use_tc = use_tc;
     auto backward = [&](const float* blob, float* gf) -> int32_t {
         return use_tc ? gnn_backward_folded(b, blob, gf, st) : gnn_backward_impl(b, st);
@@ -1124,6 +1184,7 @@ extern "C" __attribute__((visibility("default"))) int32_t gcbf_train_step(
     b.G = grad_actor;
     b.clip_all = 0;
     b.d_es = nullptr;
+    b.je = nullptr;
     RC(backward(blob_a, gf_a));
     // ---- backward 3: cbf on g
     b.out_dim = 1;
@@ -1254,6 +1315,7 @@ extern "C" __attribute__((visibility("default"))) int32_t gcbf_qp_labels(
     b.clip_all = 1;
     b.d_es = nullptr;
     b.je = ws + Q.je;
+    b.part = nullptr;
     b.use_tc = use_tensor_cores;
     RC(gnn_backward_impl(b, st));
     int32_t* rev = reinterpret_cast<int32_t*>(ws + Q.rev);

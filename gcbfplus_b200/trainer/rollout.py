@@ -144,7 +144,7 @@ class RolloutEngine:
                                       env.ray_table.data_ptr(), self.hits[t, ch.e0].data_ptr(),
                                       ch.row_start[t % 2].data_ptr(), ch.row_deg[t % 2].data_ptr(),
                                       ch.edge_recv[t % 2].data_ptr(), ch.edge_src[t % 2].data_ptr(),
-                                      ch.counters[t].data_ptr(), 1, stream)
+                                      ch.counters[t].data_ptr(), 1 | 8, stream)      # bit 3: rows in ticket order
         _lib.check(rc, "gcbf_graph_build")
 
     def _step(self, ch: _Chain, t: int, stream: int) -> None:

@@ -111,7 +111,11 @@ int32_t gcbf_param_offsets_l(int32_t edge_dim, int32_t out_dim, int32_t n_layers
  * GetGraph.to_padded (env/double_integrator.py:223-264,288-320;
  * utils/graph.py:35-44,209-244) for G graphs at once.
  * flags bit0: 1 = cast rays and write `hits`; 0 = `hits` is an input (topology only).
- * counters[0] <- number of edges; counters[1] |= 1 on edge_cap overflow (sticky). */
+ * counters[0] <- number of edges; counters[1] |= 1 on edge_cap overflow (sticky).
+ * Canonical layout: rows in batch-agent order, row_start[0] = 0, row_start[a + 1] = row_start[a] + row_deg[a],
+ * counters[0] = sum of row_deg; every output is bit-identical from run to run (row contents after an overflow are
+ * unspecified).  flags bit3: keep the rows where the build placed them (ticket order, one launch fewer than the
+ * canonical pass) -- for callers whose results do not depend on the layout, such as rollouts. */
 int32_t gcbf_graph_build(const gcbf_env_desc* desc, const float* agent, const float* obstacles,
                          const float* ray_table, float* hits, int32_t* row_start, int32_t* row_deg,
                          int32_t* edge_recv, int32_t* edge_src, int32_t* counters, int32_t flags,
@@ -313,6 +317,9 @@ int32_t gcbf_safe_horizon(const uint8_t* unsafe, uint8_t* safe, int32_t n_rollou
  *     2 sum relu(-h_dot-alpha h+eps), 3 sum ||a-u_qp||^2, 4 #(h<0 & unsafe), 5 #(h>0 & safe),
  *     6 #(h_dot+alpha h>0), 7 n_unsafe, 8 n_safe, 9 n_agents
  *   workspace: gcbf_train_workspace_floats(desc) floats.
+ * Deterministic: no float atomics -- every sum over CTAs is taken in a fixed order (per-CTA partials, then an ordered
+ * sum; per-edge input gradients gathered per agent) -- so grad_cbf, grad_actor and stats are bit-identical from run to
+ * run for the same inputs and edge layout on the same GPU model (the SM count sets the split counts).
  * Sharded training: ranks call this on their shard with the global denoms, then sum
  * [grad_cbf | grad_actor | stats] with ONE all-reduce before gcbf_clip_adamw. */
 int64_t gcbf_train_workspace_floats(const gcbf_env_desc* desc);
