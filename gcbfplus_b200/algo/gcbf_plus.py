@@ -1,5 +1,5 @@
 """GCBFPlus -- host-side mirror of gcbfplus/algo/gcbf_plus.py (and the pieces it inherits from
-gcbfplus/algo/gcbf.py: get_cbf, save, load, actor_params).  All arithmetic is in
+gcbfplus/algo/gcbf.py: get_cbf, online_policy_refinement, save, load, actor_params).  All arithmetic is in
 libgcbf_b200.so; this file is orchestration: parameter buffers, replay, minibatching.
 """
 from __future__ import annotations
@@ -17,6 +17,8 @@ from ..utils.graph import SwarmGraph
 from .base import MultiAgentController
 from .nets import GnnRunner
 from .params import NetParams
+from .refine import (REFINE_LR, REFINE_MAX_ITER, launch_refine, planes_buffer, prepare_planes, refine_workspace,
+                     require_one_layer_refine)
 
 
 class GCBFPlus(MultiAgentController):
@@ -56,6 +58,11 @@ class GCBFPlus(MultiAgentController):
         self.runner = GnnRunner(env)
         self.rng = np.random.default_rng(seed=seed + 1)       # gcbf_plus.py:139
         self._trainer_state = None                            # lazily built by update() (algo/train.py)
+        # online_policy_refinement: the CBF's prepared planes (rebuilt on every call) and the workspace of the last
+        # batch shape (n_graphs, edge_cap)
+        self._refine_planes = planes_buffer(self.cbf_params)
+        self._refine_ws: Optional[torch.Tensor] = None
+        self._refine_ws_key = None
 
     # ------------------------------------------------------------------ reference surface
     @property
@@ -91,6 +98,38 @@ class GCBFPlus(MultiAgentController):
         """gcbf_plus.py:182-186 (deterministic policy: log_pi = 0, policy.py:130-133)."""
         action = self.act(graph, params)
         return action, torch.zeros_like(action)
+
+    def online_policy_refinement(self, graph: SwarmGraph, params: Optional[NetParams] = None, *,
+                                 lr: float = REFINE_LR, max_iter: int = REFINE_MAX_ITER, return_info: bool = False):
+        """gcbf.py:161-201 for every graph of the batch: the action 2 pi + u_ref (or u_ref where u_ref alone keeps the
+        CBF condition) refined by gradient steps on mean_agents relu(-h_dot - alpha h) of the next graph until that
+        value is 0 or max_iter steps were taken; each graph stops on its own.  params: the actor's parameters.
+        Returns actions [G, N, nu]; with return_info also (value [G], iters [G]): the last loop value and the steps
+        taken (bit 30 set where a graph stopped at max_iter with value > 0)."""
+        env = self._env
+        actor = params or self.actor_net_params
+        require_one_layer_refine(actor, "actor")
+        require_one_layer_refine(self.cbf_params, "CBF")
+        pi = self.get_action(graph, actor)
+        G = graph.n_graphs
+        d = env.desc(G, 0, edge_cap=graph.edge_recv.numel())
+        stream = env._stream()
+        if self._refine_ws_key != (G, d.edge_cap):
+            self._refine_ws = None
+            self._refine_ws = refine_workspace(env, d)
+            self._refine_ws_key = (G, d.edge_cap)
+        # the planes of the parameters as they are now (one launch; the optimizer writes them through raw pointers)
+        use_tc = 1 if _lib.USE_TC else 0
+        prepared = prepare_planes(self.cbf_params, self._refine_planes, use_tc, stream)
+        action = torch.empty_like(pi)
+        value = torch.empty(G, dtype=torch.float32, device=pi.device)
+        iters = torch.empty(G, dtype=torch.int32, device=pi.device)
+        launch_refine(env, d, self.alpha, lr, max_iter, use_tc, self.cbf_params, prepared, pi, graph.agent, graph.goal,
+                      graph.hits, graph.row_start, graph.row_deg, graph.edge_recv, graph.edge_src, graph.counters,
+                      action, value, iters, self._refine_ws, stream)
+        if return_info:
+            return action, value, iters
+        return action
 
     def get_cbf(self, graph: SwarmGraph, params: Optional[NetParams] = None) -> torch.Tensor:
         """gcbf.py:209-212 -> [G, N, 1]."""

@@ -27,7 +27,8 @@ static int32_t dense_fwd(int epi, const ParamLayout& L, const TransLayout& TL, i
 int32_t gnn_forward_impl(const gcbf_env_desc* d, int out_dim, const float* P, const float* PT, const float* agent, const float* goal,
                          const float* hits, const int32_t* row_start, const int32_t* row_deg,
                          const int32_t* edge_recv, const int32_t* edge_src, const int32_t* counters, int clip_all,
-                         float* out, float* ws, cudaStream_t st) {
+                         float* out, float* ws, cudaStream_t st, const int32_t* agent_rows) {
+    // agent_rows (optional): device row count of the agent-row GEMMs, like `counters` for the edge rows
     const int ed = env_ed(d->env_kind);
     const ParamLayout L = make_layout(ed, out_dim);
     const TransLayout TL = make_trans_layout(L);
@@ -35,7 +36,7 @@ int32_t gnn_forward_impl(const gcbf_env_desc* d, int out_dim, const float* P, co
     const int cap = d->edge_cap;
     const GnnWs W = make_ws(cap, A);
     const RowCount re{counters, 0, cap};
-    const RowCount ra{nullptr, A, A};
+    const RowCount ra{agent_rows, A, A};
     const int nsm = sm_count();
     int32_t rc;
     // 1. edge features + message layer 1
@@ -104,7 +105,7 @@ extern "C" __attribute__((visibility("default"))) int32_t gcbf_gnn_forward(const
     GCBF_REQUIRE((((uintptr_t)params | (uintptr_t)workspace) & 15) == 0, "params/workspace must be 16-byte aligned");
     GCBF_REQUIRE(params_t == nullptr || (((uintptr_t)params_t) & 15) == 0, "params_t must be 16-byte aligned");
     return gnn_forward_impl(desc, out_dim, params, params_t, agent, goal, hits, row_start, row_deg, edge_recv, edge_src,
-                            counters, clip_all, out, workspace, (cudaStream_t)stream);
+                            counters, clip_all, out, workspace, (cudaStream_t)stream, nullptr);
 }
 
 // ---- building blocks exported for unit tests and for bench.py's isolated kernel timing ----

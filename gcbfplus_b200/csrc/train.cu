@@ -23,7 +23,7 @@ int32_t build_prepared(const ParamLayout& L, const float* P, float* out, cudaStr
 int32_t gnn_forward_impl(const gcbf_env_desc* d, int out_dim, const float* P, const float* PT, const float* agent, const float* goal,
                          const float* hits, const int32_t* row_start, const int32_t* row_deg,
                          const int32_t* edge_recv, const int32_t* edge_src, const int32_t* counters, int clip_all,
-                         float* out, float* ws, cudaStream_t st);
+                         float* out, float* ws, cudaStream_t st, const int32_t* agent_rows = nullptr);
 
 // ------------------------------------------------------------------------------------ act + dynamics (forward)
 // a = 2 pi + u_ref ; u = clip_action(a) ; x' = agent_step_euler(x, u)   (gcbf_plus.py:386-391)
@@ -518,18 +518,15 @@ edge_grad_gather_kernel(const int A, const int edge_cap, const int32_t* __restri
     for (int c = 0; c < ED; ++c) d_es[(size_t)a * ED + c] = s[c];
 }
 
-// d_es (edge-state grads of x') -> d pi.   x' = clip_state(x + xdot(x, u) dt), u = clip_action(a),
-// a = 2 pi + u_ref  (gcbf_plus.py:386-391; double_integrator.py:128-143,340-354 and twins).
-// d_pi = 2 (da_dyn + da_direct).
+// d_es (edge-state grads of x') -> d a.   x' = clip_state(x + xdot(x, u) dt), u = clip_action(a)
+// (gcbf_plus.py:386-391; double_integrator.py:128-143,340-354 and twins): the chain edge state -> state ->
+// clip_state -> Euler -> clip_action of agent `a`, shared by the train step and the policy refinement.
 template <int KIND>
-__global__ void dyn_bwd_kernel(const gcbf_env_desc d, const float* __restrict__ agent, const float* __restrict__ goal,
-                               const float* __restrict__ action, const float* __restrict__ xnext,
-                               const float* __restrict__ d_es, const float* __restrict__ da_direct,
-                               float* __restrict__ d_pi) {
+__device__ __forceinline__ void dyn_chain_dev(const gcbf_env_desc& d, const float* agent, const float* goal,
+                                              const float* action, const float* xnext, const float* d_es, const int a,
+                                              float* g) {
     using T = EnvTraits<KIND>;
     constexpr int SD = T::SD, NU = T::NU, ED = T::ED;
-    const int a = blockIdx.x * blockDim.x + threadIdx.x;
-    if (a >= d.n_graphs * d.n_agents) return;
     float dx[SD], xn[SD], de[ED];
 #pragma unroll
     for (int c = 0; c < ED; ++c) de[c] = d_es[(size_t)a * ED + c];
@@ -577,9 +574,23 @@ __global__ void dyn_bwd_kernel(const gcbf_env_desc d, const float* __restrict__ 
 #pragma unroll
     for (int c = 0; c < NU; ++c) {
         const float act = action[(size_t)a * NU + c];
-        const float g = (act > -d.u_lim && act < d.u_lim) ? du[c] : 0.f;  // clip_action
-        d_pi[(size_t)a * NU + c] = 2.f * (g + da_direct[(size_t)a * NU + c]);
+        g[c] = (act > -d.u_lim && act < d.u_lim) ? du[c] : 0.f;  // clip_action
     }
+}
+
+// train step: a = 2 pi + u_ref, so d_pi = 2 (da_dyn + da_direct).
+template <int KIND>
+__global__ void dyn_bwd_kernel(const gcbf_env_desc d, const float* __restrict__ agent, const float* __restrict__ goal,
+                               const float* __restrict__ action, const float* __restrict__ xnext,
+                               const float* __restrict__ d_es, const float* __restrict__ da_direct,
+                               float* __restrict__ d_pi) {
+    constexpr int NU = EnvTraits<KIND>::NU;
+    const int a = blockIdx.x * blockDim.x + threadIdx.x;
+    if (a >= d.n_graphs * d.n_agents) return;
+    float g[NU];
+    dyn_chain_dev<KIND>(d, agent, goal, action, xnext, d_es, a, g);
+#pragma unroll
+    for (int c = 0; c < NU; ++c) d_pi[(size_t)a * NU + c] = 2.f * (g[c] + da_direct[(size_t)a * NU + c]);
 }
 
 // ------------------------------------------------------------------------------------ one network backward
@@ -601,6 +612,7 @@ struct BwdArgs {
     float* je;             // [cap, 8] when d_es is wanted or the per-edge blocks are the result: d out[recv] / d feat_e
     float* part;           // PART_FLOATS: per-CTA partials of the weight-gradient reductions (when G is set)
     int use_tc;            // 1: backward-data GEMMs on the wgmma path
+    const int32_t* agent_rows = nullptr;   // optional device row count of the agent-row GEMMs (default: every agent)
 };
 
 // ---- the parameter-gradient kernels followed by the ordered sum of their per-CTA partials
@@ -703,7 +715,7 @@ static int32_t gnn_backward_impl(const BwdArgs& b, cudaStream_t st) {
     const int A = d->n_graphs * d->n_agents, cap = d->edge_cap;
     const GnnWs W = make_ws(cap, A);
     const RowCount re{b.counters, 0, cap};
-    const RowCount ra{nullptr, A, A};
+    const RowCount ra{b.agent_rows, A, A};
     const int nsm = sm_count();
     const float* fw = b.fw;
     float* gw = b.gw;
@@ -937,6 +949,7 @@ __global__ void polyak_kernel(float* __restrict__ tgt, const float* __restrict__
 
 }  // namespace gcbf
 #include "qp.cuh"
+#include "refine.cuh"
 namespace gcbf {
 
 // ------------------------------------------------------------------------------------ QP label workspace layout
@@ -1352,6 +1365,128 @@ extern "C" __attribute__((visibility("default"))) int32_t gcbf_qp_labels(
 #undef QP_LAUNCH
     count_launch();
     RC(check_launch("qp_solve_kernel"));
+#undef RC
+    return 0;
+}
+
+// ------------------------------------------------------------------------------------ online policy refinement
+extern "C" __attribute__((visibility("default"))) int32_t gcbf_refine_prepare(int32_t edge_dim, int32_t use_tensor_cores,
+                                                                              const float* cbf_params, float* prepared,
+                                                                              void* stream) {
+    GCBF_REQUIRE(cbf_params && prepared && (edge_dim == 2 || edge_dim == 4 || edge_dim == 6),
+                 "gcbf_refine_prepare: bad argument");
+    GCBF_REQUIRE((((uintptr_t)cbf_params | (uintptr_t)prepared) & 15) == 0, "buffers must be 16-byte aligned");
+    const ParamLayout Lc = make_layout(edge_dim, 1);
+    cudaStream_t st = (cudaStream_t)stream;
+    if (use_tensor_cores) return build_prepared(Lc, cbf_params, prepared, st);
+    return build_transposes(Lc, make_trans_layout(Lc), cbf_params, prepared, st);
+}
+
+extern "C" __attribute__((visibility("default"))) int64_t gcbf_refine_workspace_floats(const gcbf_env_desc* desc) {
+    if (!desc || desc->edge_cap <= 0 || desc->n_graphs <= 0 || desc->n_agents <= 0 || desc->env_kind < 0 ||
+        desc->env_kind > 3)
+        return -1;
+    return make_refine_ws(desc).total;
+}
+
+extern "C" __attribute__((visibility("default"))) int32_t gcbf_refine_actions(
+    const gcbf_env_desc* desc, float alpha, float lr, int32_t max_iter, int32_t use_tensor_cores,
+    const float* cbf_params, const float* cbf_prepared, const float* pi, const float* agent, const float* goal,
+    const float* hits, const int32_t* row_start, const int32_t* row_deg, const int32_t* edge_recv,
+    const int32_t* edge_src, const int32_t* counters, float* action, float* value, int32_t* iters, float* workspace,
+    int64_t workspace_floats, void* stream) {
+    GCBF_REQUIRE(desc && cbf_params && cbf_prepared && pi && agent && goal && hits && row_start && row_deg &&
+                     edge_recv && edge_src && counters && action && workspace, "gcbf_refine_actions: NULL pointer argument");
+    GCBF_REQUIRE(desc->env_kind >= 0 && desc->env_kind <= 3 && desc->edge_cap > 0 && desc->n_graphs > 0 &&
+                     desc->n_agents > 0 && desc->dt > 0.f, "gcbf_refine_actions: bad descriptor");
+    GCBF_REQUIRE(max_iter > 0 && isfinite(lr) && isfinite(alpha), "gcbf_refine_actions: bad settings (max_iter %d)",
+                 max_iter);
+    const RefineWs R = make_refine_ws(desc);
+    GCBF_REQUIRE(workspace_floats >= R.total, "refine workspace too small: %lld < %lld floats",
+                 (long long)workspace_floats, (long long)R.total);
+    GCBF_REQUIRE((((uintptr_t)workspace | (uintptr_t)cbf_params | (uintptr_t)cbf_prepared) & 15) == 0,
+                 "buffers must be 16-byte aligned");
+    cudaStream_t st = (cudaStream_t)stream;
+    const gcbf_env_desc* d = desc;
+    const int nu = env_nu(d->env_kind);
+    const int G = d->n_graphs, N = d->n_agents, A = G * N;
+    const int blocks = (A + 127) / 128;
+    float* ws = workspace;
+    int32_t* active = reinterpret_cast<int32_t*>(ws + R.active);
+    int32_t* upd = reinterpret_cast<int32_t*>(ws + R.upd);
+    int32_t* rows = reinterpret_cast<int32_t*>(ws + R.rows);
+    const float* PT = cbf_prepared;
+    int32_t rc;
+#define RC(x) do { if ((rc = (x))) return rc; } while (0)
+    auto forward = [&](const float* x, int clip_all, const int32_t* cnt, const int32_t* arows, float* out) -> int32_t {
+        return gnn_forward_impl(d, 1, cbf_params, use_tensor_cores ? PT : nullptr, x, goal, hits, row_start, row_deg,
+                                edge_recv, edge_src, cnt, clip_all, out, ws + R.fw, st, arows);
+    };
+    // 1. h = cbf(g) on the graph's own edge features
+    RC(forward(agent, 0, counters, nullptr, ws + R.h));
+    // 2. h(g'(u_ref)), every edge feature recomputed and norm-clipped (forward_graph)
+    GCBF_DISPATCH_ENV(d->env_kind, {
+        refine_next_state_kernel<KIND><<<blocks, 128, 0, st>>>(*d, nullptr, agent, goal, nullptr, ws + R.ur, ws + R.xn);
+    });
+    count_launch();
+    RC(check_launch("refine_next_state_kernel"));
+    RC(forward(ws + R.xn, 1, counters, nullptr, ws + R.hn));
+    // 3. per-agent selection of the starting action; every graph active
+    if (nu == 2)
+        refine_init_kernel<2><<<blocks, 128, 0, st>>>(G, A, alpha, d->dt, ws + R.h, ws + R.hn, ws + R.ur, pi, counters,
+                                                      action, active, rows);
+    else
+        refine_init_kernel<3><<<blocks, 128, 0, st>>>(G, A, alpha, d->dt, ws + R.h, ws + R.hn, ws + R.ur, pi, counters,
+                                                      action, active, rows);
+    count_launch();
+    RC(check_launch("refine_init_kernel"));
+    // 4. the refinement steps: data-only backward of h' into the edge-state gradient of x' (same as the QP labels'
+    //    Jacobian pass, gathered per agent), then the chain into the action
+    BwdArgs b;
+    b.d = d;
+    b.out_dim = 1;
+    b.P = cbf_params;
+    b.PT = PT;
+    b.fw = ws + R.fw;
+    b.gw = ws + R.gw;
+    b.out = ws + R.hn;
+    b.d_out = ws + R.dhn;
+    b.roww = nullptr;
+    b.G = nullptr;
+    b.agent = ws + R.xn;
+    b.goal = goal;
+    b.hits = hits;
+    b.row_start = row_start;
+    b.row_deg = row_deg;
+    b.edge_recv = edge_recv;
+    b.edge_src = edge_src;
+    b.counters = rows;
+    b.agent_rows = rows + 1;
+    b.clip_all = 1;
+    b.d_es = ws + R.d_es;
+    b.je = ws + R.je;
+    b.part = nullptr;
+    b.use_tc = use_tensor_cores;
+    for (int it = 0; it < max_iter; ++it) {
+        GCBF_DISPATCH_ENV(d->env_kind, {
+            refine_next_state_kernel<KIND><<<blocks, 128, 0, st>>>(*d, rows, agent, goal, action, nullptr, ws + R.xn);
+        });
+        count_launch();
+        RC(check_launch("refine_next_state_kernel"));
+        RC(forward(ws + R.xn, 1, rows, rows + 1, ws + R.hn));
+        refine_value_kernel<<<G, REFINE_VALUE_THREADS, 0, st>>>(N, env_sd(d->env_kind), alpha, d->dt, it, max_iter,
+                                                                ws + R.h, ws + R.hn, ws + R.xn, ws + R.dhn, active,
+                                                                upd, value, iters);
+        count_launch();
+        RC(check_launch("refine_value_kernel"));
+        RC(gnn_backward_impl(b, st));
+        GCBF_DISPATCH_ENV(d->env_kind, {
+            refine_update_kernel<KIND><<<blocks, 128, 0, st>>>(*d, lr, agent, goal, ws + R.xn, ws + R.d_es, active, upd,
+                                                               counters, rows, action);
+        });
+        count_launch();
+        RC(check_launch("refine_update_kernel"));
+    }
 #undef RC
     return 0;
 }

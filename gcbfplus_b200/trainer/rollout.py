@@ -10,6 +10,9 @@ Two device paths with the same arithmetic (bit-identical results, tests/test_gpu
 No host sync inside the loop on either path.
 The CBF-QP baselines (algo/cbf_qp.py) run on the CUDA-graph path: per step the pairwise CBFs + QP solve (2 launches),
 env.step with the QP action as input, and the graph build of the next state.
+The `actor_refine` policy (GCBF+ with online policy refinement, algo/refine.py) runs on the same path: per step the
+policy forward, the refinement of its action against the CBF (gcbf_refine_actions), env.step with the refined action as
+input, and the graph build of the next state.
 """
 from __future__ import annotations
 
@@ -22,6 +25,8 @@ import torch
 from .. import _lib
 from ..algo.cbf_qp import BASELINES, iter_stats
 from ..algo.params import NetParams
+from ..algo.refine import (REFINE_LR, REFINE_MAX_ITER, launch_refine, planes_buffer, prepare_planes,
+                           refine_workspace, require_one_layer_refine)
 from ..utils.graph import SwarmGraph
 from .data import Rollout
 
@@ -53,13 +58,19 @@ class _Chain:
             self.qp_ws = torch.empty(int(n_qp), dtype=f32, device=dev)
             self.qp_r = torch.empty(E, N, 3, dtype=f32, device=dev)
             self.qp_iters = torch.zeros(eng.T, eng.controller._n_solves(E, N), dtype=i32, device=dev)
+        if eng.policy == "actor_refine":
+            # refinement workspace and the per-step iteration record of every graph
+            self.refine_ws = refine_workspace(env, self.desc)
+            self.refine_iters = torch.zeros(eng.T, E, dtype=i32, device=dev)
 
 
 class RolloutEngine:
     def __init__(self, env, n_envs: int, T: Optional[int] = None, n_obs: Optional[int] = None,
                  use_cuda_graph: bool = True, policy: str = "actor", persistent: Optional[bool] = None):
-        """policy: 'actor' (a = 2 pi + u_ref, algo.step), 'u_ref' (test.py --u-ref), or a CBF-QP baseline: a
-        DecShareCBF / CentralizedCBF object, or its name ('dec_share_cbf' / 'centralized_cbf': built with alpha = 1)."""
+        """policy: 'actor' (a = 2 pi + u_ref, algo.step), 'actor_refine' (that action refined against the CBF,
+        GCBFPlus.online_policy_refinement; set_cbf_params() gives the CBF), 'u_ref' (test.py --u-ref), or a CBF-QP
+        baseline: a DecShareCBF / CentralizedCBF object, or its name ('dec_share_cbf' / 'centralized_cbf': built with
+        alpha = 1)."""
         self.env = env
         self.E = n_envs
         self.T = T or env.max_episode_steps
@@ -70,13 +81,17 @@ class RolloutEngine:
         elif policy in BASELINES:
             self.controller = BASELINES[policy](env, env.node_dim, env.edge_dim, env.state_dim, env.action_dim,
                                                 env.num_agents)
-        elif policy not in ("actor", "u_ref"):
+        elif policy not in ("actor", "actor_refine", "u_ref"):
             raise ValueError(f"unknown rollout policy {policy!r}")
         if self.controller is None and not getattr(env, "enable_stop", True):
             raise ValueError("the actor / u_ref rollouts apply the DubinsCar stop mask; env.enable_stop is False "
                              "(set by DecShareCBF)")
         self.policy = policy
         self.use_cuda_graph = use_cuda_graph
+        # actor_refine: a copy of the CBF, its prepared planes and the refinement settings (set_cbf_params)
+        self.cbf_params: Optional[NetParams] = None
+        self._refine_planes: Optional[torch.Tensor] = None
+        self.refine_alpha, self.refine_lr, self.refine_max_iter = 1.0, REFINE_LR, REFINE_MAX_ITER
         dev = env.device
         E, T, N = self.E, self.T, env.num_agents
         sd, nu, R, pd = env.state_dim, env.action_dim, env.n_hits, env.pos_dim
@@ -164,6 +179,9 @@ class RolloutEngine:
                 stream)
             _lib.check(rc, "gcbf_rollout_step_l")
             return
+        if self.policy == "actor_refine":
+            self._step_refine(ch, t, stream)
+            return
         if self.policy == "actor":      # algo.step + env.step + get_graph(next) in one call (6 launches)
             rc = env.lib.gcbf_rollout_step(
                 C.byref(d), self.params_buf.data_ptr(), self.infer_blob.data_ptr(), self.use_tc,
@@ -190,6 +208,30 @@ class RolloutEngine:
                                    None, ch.row_start[b].data_ptr(), ch.row_deg[b].data_ptr(), ch.edge_src[b].data_ptr(),
                                    self.actions[t, ch.e0].data_ptr(), self.agent[t + 1, ch.e0].data_ptr(),
                                    self.rewards[t, ch.e0:].data_ptr(), self.costs[t, ch.e0:].data_ptr(), mode, stream)
+        _lib.check(rc, "gcbf_env_step")
+        self._build(ch, t + 1, stream)
+
+    def _step_refine(self, ch: _Chain, t: int, stream: int) -> None:
+        """policy forward -> refined action (gcbf_refine_actions, iterations recorded per graph) -> env.step with it as
+        input -> graph build of the next state."""
+        env, d = self.env, ch.desc
+        if self.cbf_params is None:
+            raise RuntimeError("the actor_refine policy needs the CBF: call set_cbf_params() before run()")
+        b = t % 2
+        args = (self.agent[t, ch.e0], self.goal[ch.e0], self.hits[t, ch.e0], ch.row_start[b], ch.row_deg[b],
+                ch.edge_recv[b], ch.edge_src[b], ch.counters[t])
+        rc = env.lib.gcbf_gnn_infer(C.byref(d), _lib.NET_ACTOR, env.action_dim, self.params_buf.data_ptr(),
+                                    self.infer_blob.data_ptr(), self.use_tc, *[_lib.ptr(x) for x in args], 0,
+                                    ch.pi.data_ptr(), ch.ws.data_ptr(), ch.ws.numel(), stream)
+        _lib.check(rc, "gcbf_gnn_infer")
+        launch_refine(env, d, self.refine_alpha, self.refine_lr, self.refine_max_iter, self.use_tc, self.cbf_params,
+                      self._refine_planes, ch.pi, *args, self.actions[t, ch.e0], None,
+                      ch.refine_iters[t], ch.refine_ws, stream)
+        obs = self.obstacles[ch.e0].data_ptr() if self.O > 0 else None
+        rc = env.lib.gcbf_env_step(C.byref(d), self.agent[t, ch.e0].data_ptr(), self.goal[ch.e0].data_ptr(), obs,
+                                   None, ch.row_start[b].data_ptr(), ch.row_deg[b].data_ptr(), ch.edge_src[b].data_ptr(),
+                                   self.actions[t, ch.e0].data_ptr(), self.agent[t + 1, ch.e0].data_ptr(),
+                                   self.rewards[t, ch.e0:].data_ptr(), self.costs[t, ch.e0:].data_ptr(), 1, stream)
         _lib.check(rc, "gcbf_env_step")
         self._build(ch, t + 1, stream)
 
@@ -228,6 +270,9 @@ class RolloutEngine:
         kernel implements one layer, so a deeper actor runs on the step-by-step path; a one-layer actor gets the path
         the constructor chose for it, whatever actors the engine ran before."""
         env, dev, nu = self.env, self.env.device, self.env.action_dim
+        if n_layers > 1 and self.policy == "actor_refine":
+            raise NotImplementedError("online policy refinement implements gnn_layers = 1; the actor has %d GNN layers"
+                                      % n_layers)
         if n_layers > 1 and self._persistent_requested:
             raise ValueError("the persistent rollout implements one GNN layer; this actor has %d" % n_layers)
         if n_layers > 1 and not self.use_tc:
@@ -292,6 +337,36 @@ class RolloutEngine:
             self.launches_per_run = int(lib.gcbf_launch_count() - n0)
         if check:
             self.check_overflow()
+
+    def set_cbf_params(self, params: NetParams, alpha: float = 1.0, lr: float = REFINE_LR,
+                       max_iter: int = REFINE_MAX_ITER) -> None:
+        """actor_refine: the CBF the actions are refined against and the refinement's alpha / step size / iteration
+        cap.  The parameters are COPIED (like set_params): after they change, call set_cbf_params again."""
+        if self.policy != "actor_refine":
+            raise RuntimeError("set_cbf_params() is for the actor_refine policy")
+        require_one_layer_refine(params, "CBF")
+        if int(max_iter) < 1:
+            raise ValueError(f"max_iter must be >= 1, got {max_iter}")
+        settings = (float(alpha), float(lr), int(max_iter))
+        if self.cbf_params is None:
+            self.cbf_params = params.clone()
+            self._refine_planes = planes_buffer(params)
+        else:       # in place: a captured rollout keeps reading the same buffers
+            self.cbf_params.flat.copy_(params.flat)
+        prepare_planes(self.cbf_params, self._refine_planes, self.use_tc,
+                       torch.cuda.current_stream(self.env.device).cuda_stream)
+        if settings != (self.refine_alpha, self.refine_lr, self.refine_max_iter):
+            self._graph = None      # the settings are baked into the captured launches
+        self.refine_alpha, self.refine_lr, self.refine_max_iter = settings
+
+    def refine_stats(self) -> dict:
+        """actor_refine: median / max refinement iterations and the graph-steps that stopped at the cap, over every
+        graph-step of the last run() (reads the device record once; call after run())."""
+        if self.policy != "actor_refine":
+            raise RuntimeError("refine_stats() needs the actor_refine policy")
+        st = iter_stats(self.chains[0].refine_iters.reshape(-1))
+        st["graph_steps"] = st.pop("solves")
+        return st
 
     def qp_stats(self) -> dict:
         """CBF-QP baselines: median / max iterations and capped solves over every solve of the last run() (reads the

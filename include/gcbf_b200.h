@@ -371,6 +371,36 @@ int32_t gcbf_qp_labels(const gcbf_env_desc* desc, float alpha, int32_t use_tenso
                        float* u_qp, float* aux, int32_t* iters, float* workspace, int64_t workspace_floats,
                        void* stream);
 
+/* ---------------------------------------------------------------- online policy refinement
+ * gcbf_refine_actions replaces GCBF.online_policy_refinement (gcbfplus/algo/gcbf.py:161-201, inherited by GCBFPlus)
+ * for a batch of G graphs, each with its own stopping rule:
+ *   h = cbf(g);  v_ref = relu(-(cbf(forward_graph(g, u_ref)) - h) / dt - alpha h)   (per agent)
+ *   a = where(v_ref > 0, 2 pi + u_ref, u_ref);  i = 0, val = 1
+ *   while val > 0 and i < max_iter:  val = mean_agents relu(-(cbf(forward_graph(g, a)) - h) / dt - alpha h),
+ *                                    a -= lr * d val / d a,  i += 1
+ * (the reference's constants: lr = 0.1, max_iter = 30).  The gradient runs through clip_action, the Euler step,
+ * clip_state and the recomputed edge features with the train step's conventions (relu'(0) = 0, zero gradient outside
+ * the clip limits, the DubinsCar stop mask).  The launch sequence is fixed (capturable in a CUDA graph, no host sync);
+ * once every graph has stopped the remaining iterations run with zero device row counts.  One-layer CBF only.
+ *   cbf_params / cbf_prepared: the CBF parameters and gcbf_refine_prepare's planes of them (rebuild them whenever
+ *     the parameters change): the tf32 planes (use_tensor_cores != 0) or the transposed weights of the strict-fp32
+ *     SIMT path;
+ *     gcbf_params_t_count(edge_dim, 1) floats
+ *   pi [A, nu]: the actor output (policy.get_action);  graph arrays as gcbf_qp_labels takes them
+ *   action [A, nu] (out): the refined actions;  value [G] or NULL: the last loop value of each graph
+ *   iters [G] or NULL: iterations taken, bit 30 set when the graph stopped at max_iter with value > 0
+ *   workspace: gcbf_refine_workspace_floats(desc) floats.
+ * Deterministic: the same inputs on the same GPU model give bit-identical action, value and iters. */
+int32_t gcbf_refine_prepare(int32_t edge_dim, int32_t use_tensor_cores, const float* cbf_params, float* prepared,
+                            void* stream);
+int64_t gcbf_refine_workspace_floats(const gcbf_env_desc* desc);
+int32_t gcbf_refine_actions(const gcbf_env_desc* desc, float alpha, float lr, int32_t max_iter,
+                            int32_t use_tensor_cores, const float* cbf_params, const float* cbf_prepared,
+                            const float* pi, const float* agent, const float* goal, const float* hits,
+                            const int32_t* row_start, const int32_t* row_deg, const int32_t* edge_recv,
+                            const int32_t* edge_src, const int32_t* counters, float* action, float* value,
+                            int32_t* iters, float* workspace, int64_t workspace_floats, void* stream);
+
 /* ---------------------------------------------------------------- CBF-QP baseline controllers
  * Replace the reference's hand-written baselines for a batch of G graphs: the pairwise CBFs
  * (gcbfplus/algo/utils.py:44-349, get_pwise_cbf_fn :413-439, k = 3), DecShareCBF.get_qp_action

@@ -5,7 +5,9 @@ contour grids the reference hands to its renderer (test.py:125-131, trainer/util
 <path>/cbf_contours/epi<k>_agent<id>.npz (b_xs, b_ys, bb_h per time step).  --nojit-rollout is accepted: the
 reference needs it to survive n >= 512 with dense graphs (env/base.py:191-259); the sparse rollout engine has no such limit.
 --algo centralized_cbf | dec_share_cbf without --path runs the CBF-QP baseline controllers (test.py:88-103) with
-alpha = --alpha and writes to ./logs/<env>/<algo>."""
+alpha = --alpha and writes to ./logs/<env>/<algo>.
+--online-refine (with --path) refines every action of the trained GCBF+ policy against its CBF
+(GCBFPlus.online_policy_refinement, gcbf.py:161-201) and prints the refinement's iteration statistics."""
 import argparse
 import os
 
@@ -23,6 +25,7 @@ def test(args):
     print(f"> Running test.py {args}")
     if args.cpu:
         raise SystemExit("--cpu: gcbfplus_b200 is the sm_90a CUDA path only (no CPU fallback by design)")
+    check_refine_flags(args)
     np.random.seed(args.seed)
     config = None
     if not args.u_ref and args.path is not None:
@@ -58,7 +61,7 @@ def test(args):
             loss_safe_coef=config.loss_safe_coef, loss_h_dot_coef=config.loss_h_dot_coef, max_grad_norm=2.0,
             seed=config.seed)
         algo.load(model_path, step)
-        policy = "actor"
+        policy = "actor_refine" if args.online_refine else "actor"
         path = args.path
     else:
         assert args.env is not None
@@ -68,6 +71,8 @@ def test(args):
     eng = RolloutEngine(env, n_epi, T=env.max_episode_steps, policy=policy)
     if algo is not None and not baseline:
         eng.set_params(algo.actor_params)
+        if args.online_refine:
+            eng.set_cbf_params(algo.cbf_params, alpha=algo.alpha)
     # test.py:117-119,158: test_keys = split(PRNGKey(seed), 1000)[:epi][offset:]; episode i resets with
     # split(test_keys[i])[0].  All episodes run as one batch here.
     from gcbfplus_b200.utils import jrandom as jr
@@ -96,6 +101,13 @@ def test(args):
         if st["capped"]:
             print(f"WARNING: {st['capped']} QP solve(s) hit the iteration cap ({algo.max_iter}); their actions are the "
                   "capped iterates, not the exact QP minimisers")
+    if args.online_refine:
+        st = eng.refine_stats()
+        print(f"refinement iterations: median {st['iters_median']:.0f}, max {st['iters_max']}, "
+              f"capped {st['capped']} of {st['graph_steps']} graph-steps")
+        if st["capped"]:
+            print(f"WARNING: {st['capped']} graph-step(s) hit the refinement cap ({eng.refine_max_iter} iterations) "
+                  "with the CBF condition still violated; their actions are the capped iterates")
     if args.log:
         with open(os.path.join(path, "test_log.csv"), "a") as f:
             f.write(f"{env.num_agents},{args.epi},{env.max_episode_steps},{env.area_size},{env.params['n_obs']},"
@@ -114,6 +126,19 @@ def test(args):
         print("video rendering is out of scope of the CUDA hot path (SURVEY.md section 2, row 17); skipped")
 
 
+def check_refine_flags(args) -> None:
+    """--online-refine refines a trained GCBF+ policy: it needs --path and excludes --u-ref and the baselines."""
+    if not args.online_refine:
+        return
+    if args.u_ref:
+        raise SystemExit("--online-refine refines a trained GCBF+ policy; it cannot be combined with --u-ref")
+    if args.path is None:
+        if args.algo in BASELINES:
+            raise SystemExit(f"--online-refine refines a trained GCBF+ policy; it cannot be combined with the "
+                             f"{args.algo} baseline")
+        raise SystemExit("--online-refine needs a trained GCBF+ run (--path)")
+
+
 # the reference's command line (test.py:239-266), table-driven like train.py
 FLAGS = [
     (("-n", "--num-agents"), int, None), (("--obs",), int, 0), (("--area-size",), float, "required"),
@@ -122,6 +147,7 @@ FLAGS = [
     (("--cpu",), "flag", False), (("--u-ref",), "flag", False), (("--env",), str, None), (("--algo",), str, None),
     (("--step",), int, None), (("--epi",), int, 5), (("--offset",), int, 0), (("--no-video",), "flag", False),
     (("--nojit-rollout",), "flag", False), (("--log",), "flag", False), (("--dpi",), int, 100),
+    (("--online-refine",), "flag", False),
 ]
 
 
