@@ -267,17 +267,22 @@ def _cat(parts):
     return {k: torch.cat([p[k] for p in parts], dim=0) for k in parts[0]}
 
 
+def init_update_state(algo) -> None:
+    """Build what update() keeps between calls, if it is not there yet: the optimizer state and both replay buffers."""
+    if algo._trainer_state is None:
+        algo._trainer_state = TrainState(algo)
+    if not hasattr(algo, "buffer"):
+        algo.buffer = MaskedReplayBuffer(size=algo.buffer_size)
+        algo.unsafe_buffer = MaskedReplayBuffer(size=algo.buffer_size // 2)
+
+
 def update(algo, rollout: Rollout, step: int) -> dict:
     """GCBFPlus.update (gcbf_plus.py:282-297) + sample_batch (:232-280) + update_nets (:198-230),
     with the replay kept on the device (SURVEY 8f2).  Action labels: the CBF-QP of every graph in the
     batch, solved on the device with the TARGET cbf (get_b_u_qp, :193-213) -- `batch_u_qp`."""
     env = algo._env
     require_one_layer(algo.cbf_params.n_layers, "update()")
-    if algo._trainer_state is None:
-        algo._trainer_state = TrainState(algo)
-    if not hasattr(algo, "buffer"):
-        algo.buffer = MaskedReplayBuffer(size=algo.buffer_size)
-        algo.unsafe_buffer = MaskedReplayBuffer(size=algo.buffer_size // 2)
+    init_update_state(algo)
     safe, unsafe = label_rollout(algo, rollout)
     new = _flatten_bt(rollout, safe, unsafe)
     b, T = rollout.length, rollout.time_horizon

@@ -4,6 +4,7 @@ from __future__ import annotations
 
 import os
 from time import time
+from typing import Optional
 
 import numpy as np
 
@@ -11,13 +12,17 @@ from .. import dist as gdist
 from ..algo.train import require_one_layer
 from ..utils import jrandom as jr
 from .rollout import RolloutEngine
+from .train_state import load_train_state, save_run_state
 from .utils import eval_metrics, rollout
 
 
 class Trainer:
 
     def __init__(self, env, env_test, algo, n_env_train: int, n_env_test: int, log_dir: str, seed: int, params: dict,
-                 save_log: bool = True):
+                 save_log: bool = True, state_dir: Optional[str] = None, resume_from: Optional[str] = None):
+        """state_dir: every rank saves its training state there with every model save (trainer/train_state.py).
+        resume_from: this rank's saved state file; train() restores it after building its rollout engines and
+        continues from its step."""
         # reject a network the train step cannot train before any directory, checkpoint or rollout is made
         require_one_layer(algo.cbf_params.n_layers, "Trainer")
         self.env = env
@@ -49,6 +54,9 @@ class Trainer:
         self.update_steps = 0
         self.key = jr.PRNGKey(seed)                                   # trainer.py:62 key stream
         self.history = []
+        self.start_step = 0
+        self.state_dir = state_dir
+        self.resume_from = resume_from
 
     @staticmethod
     def _check_params(params: dict) -> bool:
@@ -80,7 +88,10 @@ class Trainer:
         train_engine = RolloutEngine(self.env, hi - lo)
         test_engine = RolloutEngine(self.env_test, self.n_env_test)
         test_keys = jr.split(jr.PRNGKey(self.seed), 1_000)[:self.n_env_test]       # trainer.py:99-100
-        for step in range(0, self.steps + 1):
+        if self.resume_from is not None:
+            # after the engines: they were built with the edge capacity the run started with, which the state may grow
+            load_train_state(self, self.resume_from)
+        for step in range(self.start_step, self.steps + 1):
             if step % self.eval_interval == 0:
                 ro = rollout(self.env_test, test_engine, self.algo.actor_params, test_keys)
                 info = eval_metrics(self.env_test, ro)
@@ -94,6 +105,8 @@ class Trainer:
                           f"finish: {info['eval/finish']:6.2f}")
                 if self.save_log and rank == 0 and step % self.save_interval == 0:
                     self.algo.save(os.path.join(self.model_dir), step)
+                if self.state_dir is not None and step % self.save_interval == 0:
+                    save_run_state(self, self.state_dir, step)
             key_x0, self.key = jr.split(self.key)                     # trainer.py:134-136
             ro = rollout(self.env, train_engine, self.algo.actor_params, jr.split(key_x0, self.n_env_train)[lo:hi])
             update_info = self.algo.update(ro, step)
