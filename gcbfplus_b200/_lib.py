@@ -45,14 +45,9 @@ _SIGNATURES = {
     "gcbf_last_error_string": (C.c_char_p, []),
     "gcbf_version": (C.c_int32, []),
     "gcbf_launch_count": (C.c_int64, []),
-    "gcbf_param_count": (C.c_int32, [C.c_int32, C.c_int32]),
-    "gcbf_param_offsets": (C.c_int32, [C.c_int32, C.c_int32, C.POINTER(C.c_int32)]),
     "gcbf_param_count_l": (C.c_int32, [C.c_int32, C.c_int32, C.c_int32]),
     "gcbf_param_offsets_l": (C.c_int32, [C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_int32)]),
     "gcbf_graph_build": (C.c_int32, [C.POINTER(EnvDesc)] + [_P] * 9 + [C.c_int32, _P]),
-    "gcbf_gnn_workspace_floats": (C.c_int64, [C.POINTER(EnvDesc), C.c_int32]),
-    "gcbf_gnn_forward": (C.c_int32, [C.POINTER(EnvDesc), C.c_int32, C.c_int32] + [_P] * 10 + [C.c_int32, _P, _P,
-                                     C.c_int64, _P]),
     "gcbf_gnn_workspace_floats_l": (C.c_int64, [C.POINTER(EnvDesc), C.c_int32, C.c_int32]),
     "gcbf_gnn_forward_l": (C.c_int32, [C.POINTER(EnvDesc), C.c_int32, C.c_int32, C.c_int32] + [_P] * 10 +
                            [C.c_int32, _P, _P, C.c_int64, _P]),
@@ -64,15 +59,11 @@ _SIGNATURES = {
     "gcbf_prepare_infer": (C.c_int32, [C.c_int32, C.c_int32, _P, _P, _P]),
     "gcbf_gnn_infer": (C.c_int32, [C.POINTER(EnvDesc), C.c_int32, C.c_int32, _P, _P, C.c_int32] + [_P] * 8 +
                        [C.c_int32, _P, _P, C.c_int64, _P]),
-    "gcbf_rollout_workspace_floats": (C.c_int64, [C.POINTER(EnvDesc)]),
-    "gcbf_rollout_step": (C.c_int32, [C.POINTER(EnvDesc), _P, _P, C.c_int32] + [_P] * 21 + [C.c_int64, _P]),
     "gcbf_rollout_step_select": (C.c_int32, [C.POINTER(EnvDesc), _P, _P, C.c_int32] + [_P] * 21 + [C.c_int64, C.c_int32, _P]),
     "gcbf_rollout_persistent_workspace_floats": (C.c_int64, [C.POINTER(EnvDesc)]),
     "gcbf_rollout_persistent_supported": (C.c_int32, [C.POINTER(EnvDesc)]),
     "gcbf_rollout_persistent_max_clusters": (C.c_int32, [C.c_int32]),
     "gcbf_rollout_persistent": (C.c_int32, [C.POINTER(EnvDesc), C.c_int32] + [_P] * 12 + [C.c_int64, _P, _P]),
-    "gcbf_params_t_count": (C.c_int32, [C.c_int32, C.c_int32]),
-    "gcbf_prepare_params": (C.c_int32, [C.c_int32, C.c_int32, _P, _P, _P]),
     "gcbf_env_step": (C.c_int32, [C.POINTER(EnvDesc)] + [_P] * 11 + [C.c_int32, _P]),
     "gcbf_act": (C.c_int32, [C.POINTER(EnvDesc)] + [_P] * 5),
     "gcbf_masks": (C.c_int32, [C.POINTER(EnvDesc)] + [_P] * 9),
@@ -172,10 +163,6 @@ def sqrt_threshold(r: float) -> float:
 
 def param_offsets(edge_dim: int, out_dim: int, n_layers: int = 1):
     """W, b offsets of the Dense layers in forward order (gcbf_param_offsets_l): 2 * (9 n_layers + 3) entries."""
-    if n_layers == 1:
-        arr = (C.c_int32 * 24)()
-        check(load().gcbf_param_offsets(edge_dim, out_dim, arr), "gcbf_param_offsets")
-        return list(arr)
     arr = (C.c_int32 * (2 * (9 * n_layers + 3)))()
     check(load().gcbf_param_offsets_l(edge_dim, out_dim, n_layers, arr), "gcbf_param_offsets_l")
     return list(arr)

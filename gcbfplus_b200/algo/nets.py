@@ -26,7 +26,7 @@ class GnnRunner:
         if ws is None or ws.device != device:
             n = self.env.lib.gcbf_gnn_workspace_floats_l(C.byref(desc), out_dim, n_layers)
             if n <= 0:
-                raise RuntimeError("gcbf_gnn_workspace_floats failed")
+                raise RuntimeError("gcbf_gnn_workspace_floats_l failed")
             ws = torch.empty(int(n), dtype=torch.float32, device=device)
             self._ws[key] = ws
         return ws

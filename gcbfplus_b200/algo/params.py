@@ -3,9 +3,9 @@
 Layout of one network (CBF or actor) = the 12 Dense layers in forward order
 (gcbfplus/nn/gnn.py:44-104, algo/module/cbf.py:12-53, algo/module/policy.py:63-128;
 names per SURVEY A.3), kernel [in, out] row-major then bias, each 16-byte aligned;
-offsets come from libgcbf_b200 (gcbf_param_offsets) so C and Python cannot drift.
+offsets come from libgcbf_b200 (gcbf_param_offsets_l) so C and Python cannot drift.
 With n_layers GNN layers (gnn.py:78-104) the 9 Dense layers of GNNLayer_0 .. GNNLayer_<n-1> come first, then the
-head (gcbf_param_offsets_l).
+head.
 Checkpoints keep the reference format: pickle of {'params': nested dict} with NumPy leaves
 (gcbfplus/algo/gcbf.py:344-357); the reference's own pickles (jax.Array leaves) load
 through a stub unpickler, no JAX needed.
@@ -93,7 +93,7 @@ class NetParams:
         self.offsets = _lib.param_offsets(edge_dim, out_dim, n_layers)
         self.count = _lib.param_count(edge_dim, out_dim, n_layers)
         self.flat = torch.zeros(self.count, dtype=torch.float32, device=device)
-        self._flat_t = None   # transposed GEMM weights for the tensor-core path (gcbf_prepare_params)
+        self._flat_t = None   # tf32 planes of the GEMM weights for the tensor-core path (gcbf_prepare_params_l)
 
     def prepared(self, stream: int = None):
         """Transposed GEMM weights (K-major B operands of the wgmma path), recomputed from `flat`.

@@ -25,8 +25,9 @@ def require_one_layer_refine(params: NetParams, what: str) -> None:
 
 
 def planes_buffer(params: NetParams) -> torch.Tensor:
-    """A buffer for the CBF's prepared planes (gcbf_params_t_count(edge_dim, 1) floats: enough for either GEMM path)."""
-    n = _lib.load().gcbf_params_t_count(params.edge_dim, 1)
+    """A buffer for the CBF's prepared planes (gcbf_params_t_count_l(edge_dim, 1, 1) floats: enough for either GEMM
+    path)."""
+    n = _lib.load().gcbf_params_t_count_l(params.edge_dim, 1, 1)
     return torch.empty(int(n), dtype=torch.float32, device=params.flat.device)
 
 

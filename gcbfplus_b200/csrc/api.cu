@@ -41,26 +41,8 @@ int sm_count() {
 }  // namespace gcbf
 
 extern "C" __attribute__((visibility("default"))) const char* gcbf_last_error_string(void) { return gcbf::g_err; }
-extern "C" __attribute__((visibility("default"))) int32_t gcbf_version(void) { return 100; }
+extern "C" __attribute__((visibility("default"))) int32_t gcbf_version(void) { return 101; }
 extern "C" __attribute__((visibility("default"))) int64_t gcbf_launch_count(void) { return gcbf::g_launches.load(); }
-
-extern "C" __attribute__((visibility("default"))) int32_t gcbf_param_count(int32_t edge_dim, int32_t out_dim) {
-    if (edge_dim < 1 || edge_dim > 6 || out_dim < 1 || out_dim > 4) return -1;
-    return gcbf::make_layout(edge_dim, out_dim).total;
-}
-
-extern "C" __attribute__((visibility("default"))) int32_t gcbf_param_offsets(int32_t edge_dim, int32_t out_dim, int32_t* off) {
-    if (edge_dim < 1 || edge_dim > 6 || out_dim < 1 || out_dim > 4 || !off) {
-        gcbf::set_error("gcbf_param_offsets: bad argument");
-        return -1;
-    }
-    gcbf::ParamLayout L = gcbf::make_layout(edge_dim, out_dim);
-    for (int i = 0; i < 12; ++i) {
-        off[2 * i] = L.w[i];
-        off[2 * i + 1] = L.b[i];
-    }
-    return 0;
-}
 
 extern "C" __attribute__((visibility("default"))) int32_t gcbf_param_count_l(int32_t edge_dim, int32_t out_dim,
                                                                              int32_t n_layers) {

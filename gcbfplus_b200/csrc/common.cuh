@@ -132,6 +132,10 @@ inline DeepLayout make_deep_layout(int edge_dim, int out_dim, int n_layers) {
     return D;
 }
 
+// tf32(x) rounded to nearest (13 low mantissa bits cleared, so the tensor core's own fp32->tf32 conversion is exact);
+// the hi / lo planes of the 3xTF32 GEMMs are rn_tf32(x) and rn_tf32(x - hi).
+__device__ __forceinline__ float rn_tf32(float x) { return __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xFFFFE000u); }
+
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

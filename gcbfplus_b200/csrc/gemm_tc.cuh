@@ -186,9 +186,7 @@ __device__ __forceinline__ void mma_k8_rs(float (&d)[64], const uint32_t (&a_hi)
 __device__ __forceinline__ int frag_row0(int wt) { return 16 * (wt >> 5) + ((wt & 31) >> 2); }
 __device__ __forceinline__ int frag_col(int wt, int i) { return 8 * (i >> 2) + 2 * (wt & 3) + (i & 1); }
 
-// hi = tf32(x) rounded to nearest (13 low mantissa bits cleared, so the tensor core's own fp32->tf32
-// conversion is exact), lo = tf32(x - hi): |x - hi - lo| <= 2^-24 |x|.
-__device__ __forceinline__ float rn_tf32(float x) { return __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xFFFFE000u); }
+// hi = rn_tf32(x), lo = rn_tf32(x - hi): |x - hi - lo| <= 2^-24 |x|.
 __device__ __forceinline__ void split_tf32(const float4& v, float4& h, float4& l) {
     h.x = rn_tf32(v.x); h.y = rn_tf32(v.y); h.z = rn_tf32(v.z); h.w = rn_tf32(v.w);
     l.x = rn_tf32(v.x - h.x); l.y = rn_tf32(v.y - h.y); l.z = rn_tf32(v.z - h.z); l.w = rn_tf32(v.w - h.w);
@@ -232,7 +230,7 @@ __device__ __forceinline__ void frag_relu_dot(const float (&d)[64], const float*
         }
 }
 
-// Weights are split once per parameter update (gcbf_prepare_params); activations are split in shared memory.
+// Weights are split once per parameter update (gcbf_prepare_params_l); activations are split in shared memory.
 static __global__ void split_tf32_kernel(const float* __restrict__ in, float* __restrict__ hi, float* __restrict__ lo, int n) {
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
         const float x = in[i];

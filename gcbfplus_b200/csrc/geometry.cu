@@ -12,6 +12,7 @@
 
 #include "common.cuh"
 #include "geometry_dev.cuh"
+#include "internal.cuh"
 
 namespace gcbf {
 
@@ -560,13 +561,6 @@ static int32_t check_desc(const gcbf_env_desc* d) {
         GCBF_REQUIRE(d->n_rays >= d->n_hits, "3-D env needs n_rays >= n_hits");
     return 0;
 }
-
-namespace gcbf {
-int32_t graph_build_impl(const gcbf_env_desc* desc, const float* agent, const float* obstacles, const float* ray_table,
-                         float* hits, int32_t* row_start, int32_t* row_deg, int32_t* edge_recv, int32_t* edge_src,
-                         int32_t* counters, int32_t flags, const TailArgs& tail, float* reward, float* cost, void* stream);
-
-}  // namespace gcbf
 
 extern "C" __attribute__((visibility("default"))) int32_t gcbf_graph_build(const gcbf_env_desc* desc, const float* agent, const float* obstacles,
                                     const float* ray_table, float* hits, int32_t* row_start, int32_t* row_deg,

@@ -5,108 +5,9 @@
 #include "gemm_tc_prod.cuh"
 #include "translayout.cuh"
 #include "smalljobs.cuh"
+#include "internal.cuh"
 
 using namespace gcbf;
-
-namespace gcbf {
-
-// Dense layer i of the network: Y = epi(X @ W_i + b_i).  With PT (transposed weights, see
-// translayout.cuh) the wgmma tensor-core kernel is used, otherwise the strict-fp32 SIMT kernel.
-static int32_t dense_fwd(int epi, const ParamLayout& L, const TransLayout& TL, int li, const float* P, const float* PT,
-                         const float* X, float* Y, const float* bias2, RowCount rc, cudaStream_t st) {
-    const int row_off = (li == L_UPD0) ? 3 * 256 : 0;   // update/Dense_0: rows 3..130 multiply the aggregated message
-    const int K = (li == L_UPD0) ? 128 : L.in[li];
-    if (PT) {   // PT = prepared parameters (PreparedLayout): tf32-split transposed weights
-        const PreparedLayout Q = make_prepared_layout(L, TL);
-        return tc::launch_gemm_tc(epi, false, X, PT + Q.pt_hi + TL.w[li], PT + Q.pt_lo + TL.w[li], P + L.b[li], bias2, Y,
-                                  nullptr, rc, K, L.out[li], st);
-    }
-    return launch_gemm_nn(epi, false, X, P + L.w[li] + row_off, P + L.b[li], bias2, Y, nullptr, rc, K, L.out[li], st);
-}
-
-int32_t gnn_forward_impl(const gcbf_env_desc* d, int out_dim, const float* P, const float* PT, const float* agent, const float* goal,
-                         const float* hits, const int32_t* row_start, const int32_t* row_deg,
-                         const int32_t* edge_recv, const int32_t* edge_src, const int32_t* counters, int clip_all,
-                         float* out, float* ws, cudaStream_t st, const int32_t* agent_rows) {
-    // agent_rows (optional): device row count of the agent-row GEMMs, like `counters` for the edge rows
-    const int ed = env_ed(d->env_kind);
-    const ParamLayout L = make_layout(ed, out_dim);
-    const TransLayout TL = make_trans_layout(L);
-    const int A = d->n_graphs * d->n_agents;
-    const int cap = d->edge_cap;
-    const GnnWs W = make_ws(cap, A);
-    const RowCount re{counters, 0, cap};
-    const RowCount ra{agent_rows, A, A};
-    const int nsm = sm_count();
-    int32_t rc;
-    // 1. edge features + message layer 1
-    {
-        const int grid = min((cap + 7) / 8, 4 * nsm);
-        GCBF_DISPATCH_ENV(d->env_kind, {
-            edge_l1_kernel<KIND><<<grid, 256, 0, st>>>(*d, P + L.w[L_MSG0], P + L.b[L_MSG0], agent, goal, hits,
-                                                       edge_recv, edge_src, counters, clip_all, ws + W.feat,
-                                                       ws + W.x1);
-        });
-        count_launch();
-        if ((rc = check_launch("edge_l1_kernel"))) return rc;
-    }
-    // 2-5. message MLP tail + gate MLP
-    if ((rc = dense_fwd(EPI_BIAS, L, TL, L_MSG1, P, PT, ws + W.x1, ws + W.x2, nullptr, re, st))) return rc;
-    if ((rc = dense_fwd(EPI_BIAS, L, TL, L_MSGOUT, P, PT, ws + W.x2, ws + W.msg, nullptr, re, st))) return rc;
-    if ((rc = dense_fwd(EPI_BIAS_RELU, L, TL, L_ATT0, P, PT, ws + W.msg, ws + W.g1, nullptr, re, st))) return rc;
-    if ((rc = dense_fwd(EPI_BIAS, L, TL, L_ATT1, P, PT, ws + W.g1, ws + W.g2, nullptr, re, st))) return rc;
-    // 6. attention softmax + aggregation
-    {
-        const int grid = min((A + 7) / 8, 4 * nsm);
-        attn_aggregate_kernel<<<grid, 256, 0, st>>>(A, cap, ws + W.g2, ws + W.msg, P + L.w[L_GATE], P + L.b[L_GATE],
-                                                    row_start, row_deg, ws + W.att, ws + W.ag);
-        count_launch();
-        if ((rc = check_launch("attn_aggregate_kernel"))) return rc;
-    }
-    // 7-11. update MLP (agent one-hot [0,0,1] folded into the bias: row 2 of update/Dense_0) + head MLP
-    if ((rc = dense_fwd(EPI_BIAS_RELU, L, TL, L_UPD0, P, PT, ws + W.ag, ws + W.v1, P + L.w[L_UPD0] + 2 * 256, ra, st))) return rc;
-    if ((rc = dense_fwd(EPI_BIAS, L, TL, L_UPD1, P, PT, ws + W.v1, ws + W.v2, nullptr, ra, st))) return rc;
-    if ((rc = dense_fwd(EPI_BIAS, L, TL, L_UPDOUT, P, PT, ws + W.v2, ws + W.v3, nullptr, ra, st))) return rc;
-    if ((rc = dense_fwd(EPI_BIAS_RELU, L, TL, L_HEAD0, P, PT, ws + W.v3, ws + W.h1, nullptr, ra, st))) return rc;
-    if ((rc = dense_fwd(EPI_BIAS, L, TL, L_HEAD1, P, PT, ws + W.h1, ws + W.h2, nullptr, ra, st))) return rc;
-    // 12. output layer + tanh
-    {
-        const int grid = min((A + 7) / 8, 4 * nsm);
-        head_out_kernel<<<grid, 256, 0, st>>>(A, out_dim, ws + W.h2, P + L.w[L_OUT], P + L.b[L_OUT], out);
-        count_launch();
-        if ((rc = check_launch("head_out_kernel"))) return rc;
-    }
-    return 0;
-}
-
-}  // namespace gcbf
-
-extern "C" __attribute__((visibility("default"))) int64_t gcbf_gnn_workspace_floats(const gcbf_env_desc* desc, int32_t out_dim) {
-    (void)out_dim;
-    if (!desc || desc->edge_cap <= 0 || desc->n_graphs <= 0 || desc->n_agents <= 0) return -1;
-    return make_ws(desc->edge_cap, (int64_t)desc->n_graphs * desc->n_agents).total;
-}
-
-extern "C" __attribute__((visibility("default"))) int32_t gcbf_gnn_forward(const gcbf_env_desc* desc, int32_t net_kind, int32_t out_dim, const float* params,
-                                    const float* params_t, const float* agent, const float* goal, const float* hits,
-                                    const int32_t* row_start, const int32_t* row_deg, const int32_t* edge_recv,
-                                    const int32_t* edge_src, const int32_t* counters, int32_t clip_all, float* out,
-                                    float* workspace, int64_t workspace_floats, void* stream) {
-    GCBF_REQUIRE(desc && params && agent && goal && hits && row_start && row_deg && edge_recv && edge_src && counters &&
-                     out && workspace, "gcbf_gnn_forward: NULL pointer argument");
-    GCBF_REQUIRE(desc->env_kind >= 0 && desc->env_kind <= 3, "bad env_kind");
-    GCBF_REQUIRE(net_kind == GCBF_NET_CBF || net_kind == GCBF_NET_ACTOR, "bad net_kind %d", net_kind);
-    GCBF_REQUIRE(out_dim >= 1 && out_dim <= 4, "bad out_dim %d", out_dim);
-    GCBF_REQUIRE(net_kind != GCBF_NET_CBF || out_dim == 1, "CBF net has out_dim 1");
-    GCBF_REQUIRE(desc->edge_cap > 0, "edge_cap must be positive");
-    const int64_t need = make_ws(desc->edge_cap, (int64_t)desc->n_graphs * desc->n_agents).total;
-    GCBF_REQUIRE(workspace_floats >= need, "workspace too small: %lld < %lld floats", (long long)workspace_floats,
-                 (long long)need);
-    GCBF_REQUIRE((((uintptr_t)params | (uintptr_t)workspace) & 15) == 0, "params/workspace must be 16-byte aligned");
-    GCBF_REQUIRE(params_t == nullptr || (((uintptr_t)params_t) & 15) == 0, "params_t must be 16-byte aligned");
-    return gnn_forward_impl(desc, out_dim, params, params_t, agent, goal, hits, row_start, row_deg, edge_recv, edge_src,
-                            counters, clip_all, out, workspace, (cudaStream_t)stream, nullptr);
-}
 
 // ---- building blocks exported for unit tests and for bench.py's isolated kernel timing ----
 extern "C" __attribute__((visibility("default"))) int32_t gcbf_gemm_nn(int32_t epi, int32_t accum, const float* A,
@@ -160,86 +61,6 @@ extern "C" __attribute__((visibility("default"))) int32_t gcbf_gemm_tc(int32_t e
                                     RowCount{m_ptr, m_fixed, m_cap}, K, N, (cudaStream_t)stream, ndot);
 }
 
-// Transposed GEMM weights of one network (the K-major B operands of the tensor-core path).
-extern "C" __attribute__((visibility("default"))) int32_t gcbf_params_t_count(int32_t edge_dim, int32_t out_dim) {
-    if (edge_dim < 1 || edge_dim > 6 || out_dim < 1 || out_dim > 4) return -1;
-    const ParamLayout L = make_layout(edge_dim, out_dim);
-    return make_prepared_layout(L, make_trans_layout(L)).total;
-}
-
-namespace gcbf {
-// Builds the prepared-parameter blob (PreparedLayout) of one network.
-// One launch builds the whole prepared blob: the transposed tf32 planes of the 9 GEMM weights (32 x 32 tiles through
-// shared memory, split on the way out) and the split planes of the untransposed parameters (the blocks after the tiles).
-struct PrepJobs {
-    int n;
-    int src[12], dst[12], rows[12], cols[12], tile0[13];
-};
-static __global__ void __launch_bounds__(256)
-prepare_kernel(const PrepJobs J, const float* __restrict__ P, float* __restrict__ pt_hi, float* __restrict__ pt_lo,
-               float* __restrict__ p_hi, float* __restrict__ p_lo, const int n_params) {
-    const int n_tiles = J.tile0[J.n];
-    if ((int)blockIdx.x < n_tiles) {
-        __shared__ float tile[32][33];
-        int j = 0;
-        while (j + 1 < J.n && (int)blockIdx.x >= J.tile0[j + 1]) ++j;
-        const int t = blockIdx.x - J.tile0[j];
-        const int rows = J.rows[j], cols = J.cols[j];
-        const int tiles_c = (cols + 31) / 32;
-        const int c0 = (t % tiles_c) * 32, r0 = (t / tiles_c) * 32;
-        const float* in = P + J.src[j];
-        const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
-        for (int i = ty; i < 32; i += 8) {
-            const int r = r0 + i, c = c0 + tx;
-            if (r < rows && c < cols) tile[i][tx] = in[(size_t)r * cols + c];
-        }
-        __syncthreads();
-        for (int i = ty; i < 32; i += 8) {
-            const int c = c0 + i, r = r0 + tx;
-            if (r < rows && c < cols) {
-                const float x = tile[tx][i];
-                const float h = tc::rn_tf32(x);
-                pt_hi[J.dst[j] + (size_t)c * rows + r] = h;
-                pt_lo[J.dst[j] + (size_t)c * rows + r] = tc::rn_tf32(x - h);
-            }
-        }
-        return;
-    }
-    const int nb = gridDim.x - n_tiles;
-    for (int i = (blockIdx.x - n_tiles) * 256 + threadIdx.x; i < n_params; i += nb * 256) {
-        const float x = P[i];
-        const float h = tc::rn_tf32(x);
-        p_hi[i] = h;
-        p_lo[i] = tc::rn_tf32(x - h);
-    }
-}
-
-int32_t build_prepared(const ParamLayout& L, const float* P, float* out, cudaStream_t st) {
-    const TransLayout TL = make_trans_layout(L);
-    const PreparedLayout Q = make_prepared_layout(L, TL);
-    PrepJobs J;
-    J.n = 0;
-    int tiles = 0;
-    for (int i = 0; i < 12; ++i) {
-        if (TL.w[i] < 0) continue;
-        const int rows = (i == L_UPD0) ? 128 : L.in[i];
-        J.src[J.n] = L.w[i] + (i == L_UPD0 ? 3 * 256 : 0);
-        J.dst[J.n] = TL.w[i];
-        J.rows[J.n] = rows;
-        J.cols[J.n] = L.out[i];
-        J.tile0[J.n] = tiles;
-        tiles += ((rows + 31) / 32) * ((L.out[i] + 31) / 32);
-        ++J.n;
-    }
-    J.tile0[J.n] = tiles;
-    const int split_blocks = min((L.total + 255) / 256, 2 * sm_count());
-    prepare_kernel<<<tiles + split_blocks, 256, 0, st>>>(J, P, out + Q.pt_hi, out + Q.pt_lo, out + Q.p_hi, out + Q.p_lo,
-                                                         L.total);
-    count_launch();
-    return check_launch("prepare_kernel");
-}
-}  // namespace gcbf
-
 extern "C" __attribute__((visibility("default"))) int32_t gcbf_split_tf32(const float* in, float* hi, float* lo, int32_t n,
                                                                           void* stream) {
     GCBF_REQUIRE(in && hi && lo && n > 0, "gcbf_split_tf32: bad argument");
@@ -247,14 +68,6 @@ extern "C" __attribute__((visibility("default"))) int32_t gcbf_split_tf32(const 
     count_launch();
     return check_launch("split_tf32_kernel");
 }
-extern "C" __attribute__((visibility("default"))) int32_t gcbf_prepare_params(int32_t edge_dim, int32_t out_dim,
-                                                                              const float* params, float* params_t,
-                                                                              void* stream) {
-    GCBF_REQUIRE(edge_dim >= 1 && edge_dim <= 6 && out_dim >= 1 && out_dim <= 4 && params && params_t,
-                 "gcbf_prepare_params: bad argument");
-    return build_prepared(make_layout(edge_dim, out_dim), params, params_t, (cudaStream_t)stream);
-}
-
 extern "C" __attribute__((visibility("default"))) int32_t gcbf_gemm_tn_tc(const float* X, int32_t ldx, const float* dY,
                                                                           float* C, const float* roww,
                                                                           const int32_t* row2agent,
@@ -336,8 +149,7 @@ int32_t gnn_infer_impl(const gcbf_env_desc* d, int out_dim, const float* P, cons
                               const float* agent, const float* goal, const float* hits, const int32_t* row_start,
                               const int32_t* row_deg, const int32_t* edge_recv, const int32_t* edge_src,
                               const int32_t* counters, int clip_all, float* out, float* ws, cudaStream_t st,
-                              float* z_out = nullptr, int* z_parts = nullptr, int32_t* zero_counter = nullptr,
-                              int select = 0xF, int keep_activations = 0) {
+                              float* z_out, int* z_parts, int32_t* zero_counter, int select, int keep_activations) {
     // keep_activations (folded train step): the unfused launch sequence, every layer output left in the workspace
     // (feat, x1, msg, g1, att, ag, v1, h1) for the backward pass; GEMMs still on the tensor-core path when use_tc
     // select (gcbf_rollout_step_select, measurement hook): bit 0 edge message (+ chained gate) kernel, bit 1 attention
@@ -471,12 +283,6 @@ extern "C" __attribute__((visibility("default"))) int32_t gcbf_gnn_infer(
 // clip, Euler, reward / cost terms -> LiDAR + neighbour lists of the next state (+ reward / cost reduction).
 // 5 kernel launches (tensor-core path).
 // ---------------------------------------------------------------------------------------------------
-namespace gcbf {
-int32_t graph_build_impl(const gcbf_env_desc* desc, const float* agent, const float* obstacles, const float* ray_table,
-                         float* hits, int32_t* row_start, int32_t* row_deg, int32_t* edge_recv, int32_t* edge_src,
-                         int32_t* counters, int32_t flags, const TailArgs& tail, float* reward, float* cost, void* stream);
-}  // namespace gcbf
-
 extern "C" __attribute__((visibility("default"))) int32_t gcbf_rollout_step_select(
     const gcbf_env_desc* desc, const float* actor_params, const float* infer_blob, int32_t use_tensor_cores,
     const float* agent, const float* goal, const float* obstacles, const float* ray_table, const float* hits,
@@ -487,11 +293,11 @@ extern "C" __attribute__((visibility("default"))) int32_t gcbf_rollout_step_sele
     GCBF_REQUIRE(desc && actor_params && infer_blob && agent && goal && ray_table && hits && row_start && row_deg &&
                      edge_recv && edge_src && counters && action && next_agent && next_hits && next_row_start &&
                      next_row_deg && next_edge_recv && next_edge_src && next_counters && reward && cost && workspace,
-                 "gcbf_rollout_step: NULL pointer argument");
+                 "gcbf_rollout_step_select: NULL pointer argument");
     GCBF_REQUIRE(next_row_start != row_start && next_row_deg != row_deg && next_edge_recv != edge_recv &&
                      next_edge_src != edge_src && next_counters != counters,
-                 "gcbf_rollout_step: the next graph must not alias the current one (double-buffer the edge lists)");
-    GCBF_REQUIRE(desc->env_kind >= 0 && desc->env_kind <= 3 && desc->edge_cap > 0, "gcbf_rollout_step: bad descriptor");
+                 "gcbf_rollout_step_select: the next graph must not alias the current one (double-buffer the edge lists)");
+    GCBF_REQUIRE(desc->env_kind >= 0 && desc->env_kind <= 3 && desc->edge_cap > 0, "gcbf_rollout_step_select: bad descriptor");
     GCBF_REQUIRE(desc->n_obs == 0 || obstacles, "obstacles is NULL but n_obs > 0");
     const int nu = env_nu(desc->env_kind);
     const int64_t A = (int64_t)desc->n_graphs * desc->n_agents;
@@ -534,105 +340,49 @@ extern "C" __attribute__((visibility("default"))) int32_t gcbf_rollout_step_sele
                             next_edge_src, next_counters, 1 | ((select & 2) ? 4 : 0), tl, reward, cost, stream);
 }
 
-extern "C" __attribute__((visibility("default"))) int32_t gcbf_rollout_step(
-    const gcbf_env_desc* desc, const float* actor_params, const float* infer_blob, int32_t use_tensor_cores,
-    const float* agent, const float* goal, const float* obstacles, const float* ray_table, const float* hits,
-    const int32_t* row_start, const int32_t* row_deg, const int32_t* edge_recv, const int32_t* edge_src,
-    const int32_t* counters, float* action, float* next_agent, float* next_hits, int32_t* next_row_start,
-    int32_t* next_row_deg, int32_t* next_edge_recv, int32_t* next_edge_src, int32_t* next_counters, float* reward,
-    float* cost, float* workspace, int64_t workspace_floats, void* stream) {
-    return gcbf_rollout_step_select(desc, actor_params, infer_blob, use_tensor_cores, agent, goal, obstacles, ray_table,
-                                    hits, row_start, row_deg, edge_recv, edge_src, counters, action, next_agent, next_hits,
-                                    next_row_start, next_row_deg, next_edge_recv, next_edge_src, next_counters, reward, cost,
-                                    workspace, workspace_floats, GCBF_STEP_ALL, stream);
-}
-
-extern "C" __attribute__((visibility("default"))) int64_t gcbf_rollout_workspace_floats(const gcbf_env_desc* desc) {
-    if (!desc || desc->edge_cap <= 0 || desc->n_graphs <= 0 || desc->n_agents <= 0) return -1;
-    const int64_t A = (int64_t)desc->n_graphs * desc->n_agents;
-    return make_ws(desc->edge_cap, A).total + 8 * A + 16;
-}
-
 // =====================================================================================================
-// Networks with n_layers > 1 (gnn.py:78-104), tensor-core path, unfolded weights.
+// Unfolded forward of an n_layers-deep network (gnn.py:78-104; n_layers = 1 is the reference's one-layer GNN): the
+// GEMMs read the tf32 planes of PlaneLayout (tensor-core path) or, at n_layers = 1, the parameters themselves
+// (strict-fp32 SIMT path).
 // Edges and their features are the same in every layer; only the node features change.  Receivers are always agents,
 // so goal and hit nodes never receive a message: their layer output is update_l([y_{l-1} | 0]), one constant row per
-// layer for "goal" and one for "hit".  They ride along as node rows A and A + 1 of every node-level GEMM.
+// layer for "goal" and one for "hit".  They ride along as node rows A and A + 1 of the node-level GEMMs of every layer
+// that a later layer reads.
 // From layer 1 on, the first message layer W1 = [We; Ws; Wr] is split: pre1_e = feat_e We + S[src_e] + R[recv_e] + b1
 // with the node-level products S = y Ws and R = y Wr, so the edge kernel gathers two 256-wide rows instead of running a
 // K = ed + 256 GEMM per edge.
 // =====================================================================================================
 namespace gcbf {
 
-// Transposed tf32 hi / lo planes of every GEMM weight of a deep network (gcbf_prepare_params_l): slot i < 12 is
-// Dense layer i of ParamLayout layer[l] (L_MSG0 holds Ws, DEEP_WR holds Wr at l >= 1; the head lives in layer 0's
-// slots); -1 where the weight is not a GEMM operand.  hi at t[l][i], lo at t[l][i] + rows * cols.
-constexpr int DEEP_WR = 12;
-struct DeepPlanes {
-    int t[GCBF_MAX_LAYERS][13], src[GCBF_MAX_LAYERS][13], rows[GCBF_MAX_LAYERS][13], cols[GCBF_MAX_LAYERS][13];
-    int total;
-};
-static DeepPlanes make_deep_planes(const DeepLayout& D, int ed) {
-    DeepPlanes Q;
-    int off = 0;
-    for (int l = 0; l < D.n_layers; ++l) {
-        const ParamLayout& L = D.layer[l];
-        for (int i = 0; i < 13; ++i) {
-            int src = -1, rows = 0;
-            if (i == L_MSG0 || i == DEEP_WR) {
-                if (l > 0) { src = L.w[L_MSG0] + (ed + (i == DEEP_WR ? 128 : 0)) * 256; rows = 128; }
-            } else if (i == L_UPD0) {
-                src = L.w[i] + (l == 0 ? 3 * 256 : 0);
-                rows = l == 0 ? 128 : 256;
-            } else if (i == L_HEAD0 || i == L_HEAD1) {
-                if (l == 0) { src = L.w[i]; rows = L.in[i]; }
-            } else if (i != L_GATE && i != L_OUT) {
-                src = L.w[i];
-                rows = L.in[i];
-            }
-            const int cols = (i == DEEP_WR) ? 256 : L.out[i];
-            Q.src[l][i] = src;
-            Q.rows[l][i] = rows;
-            Q.cols[l][i] = cols;
-            Q.t[l][i] = src < 0 ? -1 : off;
-            if (src >= 0) off += 2 * rows * cols;
-        }
-    }
-    Q.total = off;
-    return Q;
-}
-
-static int32_t build_deep_planes(int ed, int out_dim, int n_layers, const float* P, float* PT, cudaStream_t st) {
-    const DeepLayout D = make_deep_layout(ed, out_dim, n_layers);
-    const DeepPlanes Q = make_deep_planes(D, ed);
+int32_t build_planes(int ed, int out_dim, int n_layers, const float* P, float* PT, cudaStream_t st) {
+    const PlaneLayout Q = make_plane_layout(make_deep_layout(ed, out_dim, n_layers), ed);
     PlaneJobList PJ;
     for (int l = 0; l < n_layers; ++l) {
         for (int i = 0; i < 13; ++i) {
             if (Q.t[l][i] < 0) continue;
-            PJ.add(P + Q.src[l][i], Q.rows[l][i], Q.cols[l][i], true, PT + Q.t[l][i],
-                   PT + Q.t[l][i] + Q.rows[l][i] * Q.cols[l][i]);
+            const int rows = Q.rows[l][i], cols = Q.cols[l][i], n = rows * cols;
+            PJ.add(P + Q.src[l][i], rows, cols, true, PT + Q.t[l][i], PT + Q.t[l][i] + n);
+            if (Q.s[i] >= 0) PJ.add(P + Q.src[l][i], rows, cols, false, PT + Q.s[i], PT + Q.s[i] + n);
         }
-        if (int32_t rc = PJ.launch(st)) return rc;   // <= 11 jobs per layer
+        if (int32_t rc = PJ.launch(st)) return rc;   // one launch per layer: 18 jobs at n_layers = 1, <= 11 after
     }
     return 0;
 }
 
-// Workspace of the deep forward: the one-layer activations with A + 2 node rows, S | R and the update input [y | ag].
+// Workspace of the unfolded forward: the activations of make_ws (the layout the backward reads) and, at n_layers > 1,
+// with A + 2 node rows, plus S | R and the update input [y | ag].
 struct DeepWs {
     GnnWs g;
     int64_t s, r, cat, total;
 };
-static DeepWs make_deep_ws(int64_t cap, int64_t A) {
+static DeepWs make_deep_ws(int64_t cap, int64_t A, int n_layers) {
     DeepWs W;
-    W.g = make_ws(cap, A + 2);
-    int64_t o = W.g.total;
-    W.s = o;
-    o += (A + 2) * 256;
-    W.r = o;
-    o += (A + 2) * 256;
-    W.cat = o;
-    o += (A + 2) * 256;
-    W.total = o;
+    const int64_t nodes = n_layers > 1 ? A + 2 : A, node_block = n_layers > 1 ? nodes * 256 : 0;
+    W.g = make_ws(cap, nodes);
+    W.s = W.g.total;
+    W.r = W.s + node_block;
+    W.cat = W.r + node_block;
+    W.total = W.cat + node_block;
     return W;
 }
 
@@ -701,31 +451,34 @@ node_concat_kernel(const int A, const float* __restrict__ Y, const float* __rest
     }
 }
 
-// Forward of an n_layers-deep network.  out != nullptr: tanh(head) [A, out_dim]; else z_out [1][A][4] receives the
-// output layer's pre-activations without bias (the rollout step's policy tail adds the bias and the tanh).
-int32_t gnn_forward_deep(const gcbf_env_desc* d, int out_dim, int n_layers, const float* P, const float* PT,
-                         const float* agent, const float* goal, const float* hits, const int32_t* row_start,
-                         const int32_t* row_deg, const int32_t* edge_recv, const int32_t* edge_src,
-                         const int32_t* counters, int clip_all, float* out, float* z_out, float* ws, cudaStream_t st) {
+int32_t gnn_forward(const gcbf_env_desc* d, int out_dim, int n_layers, const float* P, const float* PT,
+                    const float* agent, const float* goal, const float* hits, const int32_t* row_start,
+                    const int32_t* row_deg, const int32_t* edge_recv, const int32_t* edge_src, const int32_t* counters,
+                    int clip_all, float* out, float* z_out, float* ws, cudaStream_t st, const int32_t* agent_rows) {
     const int ed = env_ed(d->env_kind);
     const DeepLayout D = make_deep_layout(ed, out_dim, n_layers);
-    const DeepPlanes Q = make_deep_planes(D, ed);
+    const PlaneLayout Q = make_plane_layout(D, ed);
     const int A = d->n_graphs * d->n_agents, cap = d->edge_cap;
-    const DeepWs DW = make_deep_ws(cap, A);
+    const DeepWs DW = make_deep_ws(cap, A, n_layers);
     const GnnWs& W = DW.g;
     const RowCount re{counters, 0, cap};
-    const RowCount ra{nullptr, A, A};
+    const RowCount ra{agent_rows, A, A};
     const RowCount ra2{nullptr, A + 2, A + 2};
     const int nsm = sm_count();
     int32_t rc;
+    // Y = epi(X W + bias (+ bias2)) with W the weight in slot i of layer l
     auto gemm = [&](int epi, int l, int i, const float* X, const float* bias, const float* bias2, float* Y,
                     RowCount rows) -> int32_t {
         const int K = Q.rows[l][i], N = Q.cols[l][i];
-        return tc::launch_gemm_tc(epi, false, X, PT + Q.t[l][i], PT + Q.t[l][i] + K * N, bias, bias2, Y, nullptr, rows,
-                                  K, N, st);
+        if (PT)
+            return tc::launch_gemm_tc(epi, false, X, PT + Q.t[l][i], PT + Q.t[l][i] + K * N, bias, bias2, Y, nullptr,
+                                      rows, K, N, st);
+        return launch_gemm_nn(epi, false, X, P + Q.src[l][i], bias, bias2, Y, nullptr, rows, K, N, st);
     };
     for (int l = 0; l < n_layers; ++l) {
         const ParamLayout& L = D.layer[l];
+        const bool carry = l + 1 < n_layers;   // a later layer reads the goal / hit rows of this one
+        const RowCount rn = carry ? ra2 : ra;
         const int egrid = min((cap + 7) / 8, 4 * nsm);
         if (l == 0) {
             GCBF_DISPATCH_ENV(d->env_kind, {
@@ -761,17 +514,19 @@ int32_t gnn_forward_deep(const gcbf_env_desc* d, int out_dim, int n_layers, cons
             // agent one-hot [0,0,1] folded into the bias: row 2 of update/Dense_0
             if ((rc = gemm(EPI_BIAS_RELU, l, L_UPD0, ws + W.ag, P + L.b[L_UPD0], P + L.w[L_UPD0] + 2 * 256, ws + W.v1,
                            ra))) return rc;
-            const_rows_l0_kernel<<<1, 256, 0, st>>>(A, P + L.w[L_UPD0], P + L.b[L_UPD0], ws + W.v1);
-            count_launch();
-            if ((rc = check_launch("const_rows_l0_kernel"))) return rc;
+            if (carry) {
+                const_rows_l0_kernel<<<1, 256, 0, st>>>(A, P + L.w[L_UPD0], P + L.b[L_UPD0], ws + W.v1);
+                count_launch();
+                if ((rc = check_launch("const_rows_l0_kernel"))) return rc;
+            }
         } else {
             node_concat_kernel<<<min((A + 2 + 3) / 4, 4 * nsm), 256, 0, st>>>(A, ws + W.v3, ws + W.ag, ws + DW.cat);
             count_launch();
             if ((rc = check_launch("node_concat_kernel"))) return rc;
-            if ((rc = gemm(EPI_BIAS_RELU, l, L_UPD0, ws + DW.cat, P + L.b[L_UPD0], nullptr, ws + W.v1, ra2))) return rc;
+            if ((rc = gemm(EPI_BIAS_RELU, l, L_UPD0, ws + DW.cat, P + L.b[L_UPD0], nullptr, ws + W.v1, rn))) return rc;
         }
-        if ((rc = gemm(EPI_BIAS, l, L_UPD1, ws + W.v1, P + L.b[L_UPD1], nullptr, ws + W.v2, ra2))) return rc;
-        if ((rc = gemm(EPI_BIAS, l, L_UPDOUT, ws + W.v2, P + L.b[L_UPDOUT], nullptr, ws + W.v3, ra2))) return rc;
+        if ((rc = gemm(EPI_BIAS, l, L_UPD1, ws + W.v1, P + L.b[L_UPD1], nullptr, ws + W.v2, rn))) return rc;
+        if ((rc = gemm(EPI_BIAS, l, L_UPDOUT, ws + W.v2, P + L.b[L_UPDOUT], nullptr, ws + W.v3, rn))) return rc;
     }
     const ParamLayout& L = D.layer[0];
     if ((rc = gemm(EPI_BIAS_RELU, 0, L_HEAD0, ws + W.v3, P + L.b[L_HEAD0], nullptr, ws + W.h1, ra))) return rc;
@@ -793,12 +548,15 @@ static bool deep_dims_ok(int32_t edge_dim, int32_t out_dim, int32_t n_layers) {
     return edge_dim >= 1 && edge_dim <= 6 && out_dim >= 1 && out_dim <= 4 && n_layers >= 1 &&
            n_layers <= gcbf::GCBF_MAX_LAYERS;
 }
+static bool ws_dims_ok(const gcbf_env_desc* desc, int32_t n_layers) {
+    return desc && desc->edge_cap > 0 && desc->n_graphs > 0 && desc->n_agents > 0 && n_layers >= 1 &&
+           n_layers <= gcbf::GCBF_MAX_LAYERS;
+}
 
 extern "C" __attribute__((visibility("default"))) int32_t gcbf_params_t_count_l(int32_t edge_dim, int32_t out_dim,
                                                                                 int32_t n_layers) {
     if (!deep_dims_ok(edge_dim, out_dim, n_layers)) return -1;
-    if (n_layers == 1) return gcbf_params_t_count(edge_dim, out_dim);
-    return make_deep_planes(make_deep_layout(edge_dim, out_dim, n_layers), edge_dim).total;
+    return make_plane_layout(make_deep_layout(edge_dim, out_dim, n_layers), edge_dim).total;
 }
 
 extern "C" __attribute__((visibility("default"))) int32_t gcbf_prepare_params_l(int32_t edge_dim, int32_t out_dim,
@@ -806,16 +564,14 @@ extern "C" __attribute__((visibility("default"))) int32_t gcbf_prepare_params_l(
                                                                                 float* params_t, void* stream) {
     GCBF_REQUIRE(deep_dims_ok(edge_dim, out_dim, n_layers) && params && params_t, "gcbf_prepare_params_l: bad argument");
     GCBF_REQUIRE((((uintptr_t)params | (uintptr_t)params_t) & 15) == 0, "gcbf_prepare_params_l: 16-byte alignment required");
-    if (n_layers == 1) return gcbf_prepare_params(edge_dim, out_dim, params, params_t, stream);
-    return build_deep_planes(edge_dim, out_dim, n_layers, params, params_t, (cudaStream_t)stream);
+    return build_planes(edge_dim, out_dim, n_layers, params, params_t, (cudaStream_t)stream);
 }
 
 extern "C" __attribute__((visibility("default"))) int64_t gcbf_gnn_workspace_floats_l(const gcbf_env_desc* desc,
                                                                                      int32_t out_dim, int32_t n_layers) {
-    if (n_layers == 1) return gcbf_gnn_workspace_floats(desc, out_dim);
-    if (!desc || desc->edge_cap <= 0 || desc->n_graphs <= 0 || desc->n_agents <= 0 || n_layers < 1 ||
-        n_layers > gcbf::GCBF_MAX_LAYERS) return -1;
-    return make_deep_ws(desc->edge_cap, (int64_t)desc->n_graphs * desc->n_agents).total;
+    (void)out_dim;
+    if (!ws_dims_ok(desc, n_layers)) return -1;
+    return make_deep_ws(desc->edge_cap, (int64_t)desc->n_graphs * desc->n_agents, n_layers).total;
 }
 
 extern "C" __attribute__((visibility("default"))) int32_t gcbf_gnn_forward_l(
@@ -825,33 +581,29 @@ extern "C" __attribute__((visibility("default"))) int32_t gcbf_gnn_forward_l(
     float* out, float* workspace, int64_t workspace_floats, void* stream) {
     GCBF_REQUIRE(n_layers >= 1 && n_layers <= GCBF_MAX_LAYERS, "gcbf_gnn_forward_l: n_layers %d outside [1, %d]",
                  n_layers, GCBF_MAX_LAYERS);
-    if (n_layers == 1)
-        return gcbf_gnn_forward(desc, net_kind, out_dim, params, params_t, agent, goal, hits, row_start, row_deg,
-                                edge_recv, edge_src, counters, clip_all, out, workspace, workspace_floats, stream);
     GCBF_REQUIRE(desc && params && agent && goal && hits && row_start && row_deg && edge_recv && edge_src && counters &&
                      out && workspace, "gcbf_gnn_forward_l: NULL pointer argument");
-    GCBF_REQUIRE(params_t, "gcbf_gnn_forward_l: n_layers > 1 runs on the tensor-core path only (params_t from "
-                           "gcbf_prepare_params_l); the strict-fp32 SIMT path implements n_layers = 1");
+    GCBF_REQUIRE(n_layers == 1 || params_t, "gcbf_gnn_forward_l: n_layers > 1 runs on the tensor-core path only "
+                                            "(params_t from gcbf_prepare_params_l); the strict-fp32 SIMT path "
+                                            "implements n_layers = 1");
     GCBF_REQUIRE(desc->env_kind >= 0 && desc->env_kind <= 3, "bad env_kind");
     GCBF_REQUIRE(net_kind == GCBF_NET_CBF || net_kind == GCBF_NET_ACTOR, "bad net_kind %d", net_kind);
     GCBF_REQUIRE(out_dim >= 1 && out_dim <= 4 && (net_kind != GCBF_NET_CBF || out_dim == 1), "bad out_dim %d", out_dim);
     GCBF_REQUIRE(desc->edge_cap > 0, "edge_cap must be positive");
-    const int64_t need = make_deep_ws(desc->edge_cap, (int64_t)desc->n_graphs * desc->n_agents).total;
+    const int64_t need = make_deep_ws(desc->edge_cap, (int64_t)desc->n_graphs * desc->n_agents, n_layers).total;
     GCBF_REQUIRE(workspace_floats >= need, "workspace too small: %lld < %lld floats", (long long)workspace_floats,
                  (long long)need);
     GCBF_REQUIRE((((uintptr_t)params | (uintptr_t)params_t | (uintptr_t)workspace) & 15) == 0,
                  "params/params_t/workspace must be 16-byte aligned");
-    return gnn_forward_deep(desc, out_dim, n_layers, params, params_t, agent, goal, hits, row_start, row_deg, edge_recv,
-                            edge_src, counters, clip_all, out, nullptr, workspace, (cudaStream_t)stream);
+    return gnn_forward(desc, out_dim, n_layers, params, params_t, agent, goal, hits, row_start, row_deg, edge_recv,
+                       edge_src, counters, clip_all, out, nullptr, workspace, (cudaStream_t)stream);
 }
 
 extern "C" __attribute__((visibility("default"))) int64_t gcbf_rollout_workspace_floats_l(const gcbf_env_desc* desc,
                                                                                          int32_t n_layers) {
-    if (n_layers == 1) return gcbf_rollout_workspace_floats(desc);
-    if (!desc || desc->edge_cap <= 0 || desc->n_graphs <= 0 || desc->n_agents <= 0 || n_layers < 1 ||
-        n_layers > gcbf::GCBF_MAX_LAYERS) return -1;
+    if (!ws_dims_ok(desc, n_layers)) return -1;
     const int64_t A = (int64_t)desc->n_graphs * desc->n_agents;
-    return make_deep_ws(desc->edge_cap, A).total + 8 * A + 16;
+    return make_deep_ws(desc->edge_cap, A, n_layers).total + 8 * A + 16;
 }
 
 extern "C" __attribute__((visibility("default"))) int32_t gcbf_rollout_step_l(
@@ -864,10 +616,11 @@ extern "C" __attribute__((visibility("default"))) int32_t gcbf_rollout_step_l(
     GCBF_REQUIRE(n_layers >= 1 && n_layers <= GCBF_MAX_LAYERS, "gcbf_rollout_step_l: n_layers %d outside [1, %d]",
                  n_layers, GCBF_MAX_LAYERS);
     if (n_layers == 1)
-        return gcbf_rollout_step(desc, actor_params, infer_blob, use_tensor_cores, agent, goal, obstacles, ray_table,
-                                 hits, row_start, row_deg, edge_recv, edge_src, counters, action, next_agent, next_hits,
-                                 next_row_start, next_row_deg, next_edge_recv, next_edge_src, next_counters, reward,
-                                 cost, workspace, workspace_floats, stream);
+        return gcbf_rollout_step_select(desc, actor_params, infer_blob, use_tensor_cores, agent, goal, obstacles,
+                                        ray_table, hits, row_start, row_deg, edge_recv, edge_src, counters, action,
+                                        next_agent, next_hits, next_row_start, next_row_deg, next_edge_recv,
+                                        next_edge_src, next_counters, reward, cost, workspace, workspace_floats,
+                                        GCBF_STEP_ALL, stream);
     GCBF_REQUIRE(desc && actor_params && infer_blob && agent && goal && ray_table && hits && row_start && row_deg &&
                      edge_recv && edge_src && counters && action && next_agent && next_hits && next_row_start &&
                      next_row_deg && next_edge_recv && next_edge_src && next_counters && reward && cost && workspace,
@@ -880,7 +633,7 @@ extern "C" __attribute__((visibility("default"))) int32_t gcbf_rollout_step_l(
     GCBF_REQUIRE(desc->n_obs == 0 || obstacles, "obstacles is NULL but n_obs > 0");
     const int nu = env_nu(desc->env_kind);
     const int64_t A = (int64_t)desc->n_graphs * desc->n_agents;
-    const DeepWs W = make_deep_ws(desc->edge_cap, A);
+    const DeepWs W = make_deep_ws(desc->edge_cap, A, n_layers);
     GCBF_REQUIRE(workspace_floats >= W.total + 8 * A + 8, "workspace too small: %lld < %lld floats",
                  (long long)workspace_floats, (long long)(W.total + 8 * A + 8));
     GCBF_REQUIRE((((uintptr_t)workspace | (uintptr_t)actor_params | (uintptr_t)infer_blob) & 15) == 0,
@@ -888,8 +641,8 @@ extern "C" __attribute__((visibility("default"))) int32_t gcbf_rollout_step_l(
     cudaStream_t st = (cudaStream_t)stream;
     const DeepLayout D = make_deep_layout(env_ed(desc->env_kind), nu, n_layers);
     float* z = workspace + ((W.total + 3) & ~(int64_t)3);    // [1][A][4] output-layer pre-activations
-    if (int32_t rc = gnn_forward_deep(desc, nu, n_layers, actor_params, infer_blob, agent, goal, hits, row_start,
-                                      row_deg, edge_recv, edge_src, counters, 0, nullptr, z, workspace, st)) return rc;
+    if (int32_t rc = gnn_forward(desc, nu, n_layers, actor_params, infer_blob, agent, goal, hits, row_start, row_deg,
+                                 edge_recv, edge_src, counters, 0, nullptr, z, workspace, st)) return rc;
     TailArgs tl;
     tl.z = z;
     tl.parts = 1;

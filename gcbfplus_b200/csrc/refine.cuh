@@ -1,6 +1,6 @@
 // refine.cuh -- online policy refinement of GCBF+ (gcbfplus/algo/gcbf.py:161-201) for a batch of G graphs.
 // Included at the end of train.cu: it runs on the train step's pieces -- the CBF forward with saved activations
-// (gnn_forward_impl), its data-only backward into the per-agent edge-state gradient (gnn_backward_impl with G = nullptr)
+// (gnn_forward), its data-only backward into the per-agent edge-state gradient (gnn_backward_impl with G = nullptr)
 // and the chain edge state -> state -> clip_state -> Euler -> clip_action (dyn_chain_dev).
 //
 // Per graph, h = cbf(g) is a constant and the action is refined by gradient steps on

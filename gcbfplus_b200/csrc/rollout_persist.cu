@@ -1,6 +1,6 @@
 // rollout_persist.cu -- the whole closed-loop rollout of trainer/utils.py:25-55 as ONE persistent kernel: one
 // thread-block CLUSTER per environment, a loop over the T env-steps inside the kernel, cluster barriers where the
-// 5-launch path (gcbf_rollout_step) has kernel boundaries.
+// 5-launch path (gcbf_rollout_step_l) has kernel boundaries.
 //
 // Why: environments are independent graphs, and at BASELINE's configs[2] (16 envs x 512 agents) every kernel of the
 // 5-launch env-step is a single wave whose duration is its per-CTA latency chain plus ~4 us of launch / prologue

@@ -127,9 +127,7 @@ struct SmallJobList {
 };
 
 // ---- tf32 hi / lo planes of a [rows, cols] matrix, straight or transposed, several matrices per launch
-__device__ __forceinline__ float sj_rn_tf32(float x) { return __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xFFFFE000u); }
-
-constexpr int PLANE_MAX_JOBS = 16;
+constexpr int PLANE_MAX_JOBS = 18;   // the planes of a one-layer network (PlaneLayout): 9 transposed + 9 straight
 struct PlaneJobs {
     int n;
     int tile0[PLANE_MAX_JOBS + 1];
@@ -153,9 +151,9 @@ static __global__ void __launch_bounds__(256) plane_jobs_kernel(const PlaneJobs 
             const int r = r0 + i, c = c0 + tx;
             if (r < rows && c < cols) {
                 const float x = in[(size_t)r * cols + c];
-                const float h = sj_rn_tf32(x);
+                const float h = rn_tf32(x);
                 J.hi[j][(size_t)r * cols + c] = h;
-                J.lo[j][(size_t)r * cols + c] = sj_rn_tf32(x - h);
+                J.lo[j][(size_t)r * cols + c] = rn_tf32(x - h);
             }
         }
         return;
@@ -169,9 +167,9 @@ static __global__ void __launch_bounds__(256) plane_jobs_kernel(const PlaneJobs 
         const int c = c0 + i, r = r0 + tx;
         if (r < rows && c < cols) {
             const float x = tile[tx][i];
-            const float h = sj_rn_tf32(x);
+            const float h = rn_tf32(x);
             J.hi[j][(size_t)c * rows + r] = h;
-            J.lo[j][(size_t)c * rows + r] = sj_rn_tf32(x - h);
+            J.lo[j][(size_t)c * rows + r] = rn_tf32(x - h);
         }
     }
 }

@@ -16,14 +16,9 @@
 #include "gnn.cuh"
 #include "translayout.cuh"
 #include "smalljobs.cuh"
+#include "internal.cuh"
 
 namespace gcbf {
-
-int32_t build_prepared(const ParamLayout& L, const float* P, float* out, cudaStream_t st);
-int32_t gnn_forward_impl(const gcbf_env_desc* d, int out_dim, const float* P, const float* PT, const float* agent, const float* goal,
-                         const float* hits, const int32_t* row_start, const int32_t* row_deg,
-                         const int32_t* edge_recv, const int32_t* edge_src, const int32_t* counters, int clip_all,
-                         float* out, float* ws, cudaStream_t st, const int32_t* agent_rows = nullptr);
 
 // ------------------------------------------------------------------------------------ act + dynamics (forward)
 // a = 2 pi + u_ref ; u = clip_action(a) ; x' = agent_step_euler(x, u)   (gcbf_plus.py:386-391)
@@ -598,7 +593,7 @@ struct BwdArgs {
     const gcbf_env_desc* d;
     int out_dim;
     const float* P;        // parameters
-    const float* PT;       // transposed GEMM weights (make_trans_layout)
+    const float* PT;       // backward-data B operands: tf32 planes (build_planes) or, SIMT, W^T (TransLayout)
     const float* fw;       // forward workspace (saved activations)
     float* gw;             // gradient workspace (same layout)
     const float* out;      // network output (tanh applied) [A, out_dim]
@@ -693,18 +688,15 @@ static int32_t dense_bwd_weight(const BwdArgs& b, const float* X, int ldx, const
     return launch_colsum(dY, db, b.roww, row2agent, rc, N, A, st, b.part, db2);
 }
 
-// dX = epi(dY @ W_i^T) (+= if accum).  SIMT: B = W^T from PT; tensor core: Bt = W itself (K-major).
-static int32_t dense_bwd_data(const BwdArgs& b, const ParamLayout& L, const TransLayout& TL, int li, int epi, bool accum,
+// dX = epi(dY @ W_i^T) (+= if accum) with the B operand at b.PT + boff[li].  Tensor core: the straight tf32 planes of
+// W_i (PlaneLayout.s, W itself is the K-major operand); SIMT: W_i^T (TransLayout).
+static int32_t dense_bwd_data(const BwdArgs& b, const ParamLayout& L, const int* boff, int li, int epi, bool accum,
                               const float* dY, float* dX, const float* aux, RowCount rc, cudaStream_t st) {
     const int N = (li == L_UPD0) ? 128 : L.in[li];
     const int K = L.out[li];
-    if (b.use_tc) {   // b.PT = prepared blob: the W planes are the K-major B operand of dX = dY @ W^T
-        const PreparedLayout Q = make_prepared_layout(L, TL);
-        const int off = L.w[li] + (li == L_UPD0 ? 3 * 256 : 0);
-        return tc::launch_gemm_tc(epi, accum, dY, b.PT + Q.p_hi + off, b.PT + Q.p_lo + off, nullptr, nullptr, dX, aux, rc,
-                                  K, N, st);
-    }
-    return launch_gemm_nn(epi, accum, dY, b.PT + TL.w[li], nullptr, nullptr, dX, aux, rc, K, N, st);
+    const float* B = b.PT + boff[li];
+    if (b.use_tc) return tc::launch_gemm_tc(epi, accum, dY, B, B + K * N, nullptr, nullptr, dX, aux, rc, K, N, st);
+    return launch_gemm_nn(epi, accum, dY, B, nullptr, nullptr, dX, aux, rc, K, N, st);
 }
 
 static int32_t gnn_backward_impl(const BwdArgs& b, cudaStream_t st) {
@@ -712,6 +704,8 @@ static int32_t gnn_backward_impl(const BwdArgs& b, cudaStream_t st) {
     const int ed = env_ed(d->env_kind);
     const ParamLayout L = make_layout(ed, b.out_dim);
     const TransLayout TL = make_trans_layout(L);
+    const PlaneLayout Q = make_plane_layout(make_deep_layout(ed, b.out_dim, 1), ed);
+    const int* boff = b.use_tc ? Q.s : TL.w;
     const int A = d->n_graphs * d->n_agents, cap = d->edge_cap;
     const GnnWs W = make_ws(cap, A);
     const RowCount re{b.counters, 0, cap};
@@ -729,30 +723,30 @@ static int32_t gnn_backward_impl(const BwdArgs& b, cudaStream_t st) {
                     wgrad ? Gz + L.w[L_OUT] : nullptr, wgrad ? Gz + L.b[L_OUT] : nullptr, 0, st));
     // ---- head MLP
     WG(dense_bwd_weight(b, fw + W.h1, 256, gw + W.h2, b.G + L.w[L_HEAD1], b.G + L.b[L_HEAD1], nullptr, nullptr, ra, 256, 256, A, st));
-    RC(dense_bwd_data(b, L, TL, L_HEAD1, EPI_RELU_MASK, false, gw + W.h2, gw + W.h1, fw + W.h1, ra, st));
+    RC(dense_bwd_data(b, L, boff, L_HEAD1, EPI_RELU_MASK, false, gw + W.h2, gw + W.h1, fw + W.h1, ra, st));
     WG(dense_bwd_weight(b, fw + W.v3, 128, gw + W.h1, b.G + L.w[L_HEAD0], b.G + L.b[L_HEAD0], nullptr, nullptr, ra, 128, 256, A, st));
-    RC(dense_bwd_data(b, L, TL, L_HEAD0, EPI_NONE, false, gw + W.h1, gw + W.v3, nullptr, ra, st));
+    RC(dense_bwd_data(b, L, boff, L_HEAD0, EPI_NONE, false, gw + W.h1, gw + W.v3, nullptr, ra, st));
     // ---- update MLP
     WG(dense_bwd_weight(b, fw + W.v2, 256, gw + W.v3, b.G + L.w[L_UPDOUT], b.G + L.b[L_UPDOUT], nullptr, nullptr, ra, 256, 128, A, st));
-    RC(dense_bwd_data(b, L, TL, L_UPDOUT, EPI_NONE, false, gw + W.v3, gw + W.v2, nullptr, ra, st));
+    RC(dense_bwd_data(b, L, boff, L_UPDOUT, EPI_NONE, false, gw + W.v3, gw + W.v2, nullptr, ra, st));
     WG(dense_bwd_weight(b, fw + W.v1, 256, gw + W.v2, b.G + L.w[L_UPD1], b.G + L.b[L_UPD1], nullptr, nullptr, ra, 256, 256, A, st));
-    RC(dense_bwd_data(b, L, TL, L_UPD1, EPI_RELU_MASK, false, gw + W.v2, gw + W.v1, fw + W.v1, ra, st));
+    RC(dense_bwd_data(b, L, boff, L_UPD1, EPI_RELU_MASK, false, gw + W.v2, gw + W.v1, fw + W.v1, ra, st));
     WG(dense_bwd_weight(b, fw + W.ag, 128, gw + W.v1, b.G + L.w[L_UPD0] + 3 * 256, b.G + L.b[L_UPD0], b.G + L.w[L_UPD0] + 2 * 256, nullptr, ra, 128, 256, A, st));
-    RC(dense_bwd_data(b, L, TL, L_UPD0, EPI_NONE, false, gw + W.v1, gw + W.ag, nullptr, ra, st));
+    RC(dense_bwd_data(b, L, boff, L_UPD0, EPI_NONE, false, gw + W.v1, gw + W.ag, nullptr, ra, st));
     // ---- attention + aggregation
     RC(attn_aggregate_bwd(b, min((A + 7) / 8, 2 * nsm), gw + W.ag, fw + W.msg, fw + W.g2, fw + W.att, b.P + L.w[L_GATE],
                           gw + W.msg, gw + W.g2, wgrad ? Gz + L.w[L_GATE] : nullptr, wgrad ? Gz + L.b[L_GATE] : nullptr, 0,
                           st));
     // ---- gate MLP (edge rows; dW weighted by the receiver's weight)
     WG(dense_bwd_weight(b, fw + W.g1, 128, gw + W.g2, b.G + L.w[L_ATT1], b.G + L.b[L_ATT1], nullptr, b.edge_recv, re, 128, 128, A, st));
-    RC(dense_bwd_data(b, L, TL, L_ATT1, EPI_RELU_MASK, false, gw + W.g2, gw + W.g1, fw + W.g1, re, st));
+    RC(dense_bwd_data(b, L, boff, L_ATT1, EPI_RELU_MASK, false, gw + W.g2, gw + W.g1, fw + W.g1, re, st));
     WG(dense_bwd_weight(b, fw + W.msg, 128, gw + W.g1, b.G + L.w[L_ATT0], b.G + L.b[L_ATT0], nullptr, b.edge_recv, re, 128, 128, A, st));
-    RC(dense_bwd_data(b, L, TL, L_ATT0, EPI_NONE, true, gw + W.g1, gw + W.msg, nullptr, re, st));
+    RC(dense_bwd_data(b, L, boff, L_ATT0, EPI_NONE, true, gw + W.g1, gw + W.msg, nullptr, re, st));
     // ---- message MLP
     WG(dense_bwd_weight(b, fw + W.x2, 256, gw + W.msg, b.G + L.w[L_MSGOUT], b.G + L.b[L_MSGOUT], nullptr, b.edge_recv, re, 256, 128, A, st));
-    RC(dense_bwd_data(b, L, TL, L_MSGOUT, EPI_NONE, false, gw + W.msg, gw + W.x2, nullptr, re, st));
+    RC(dense_bwd_data(b, L, boff, L_MSGOUT, EPI_NONE, false, gw + W.msg, gw + W.x2, nullptr, re, st));
     WG(dense_bwd_weight(b, fw + W.x1, 256, gw + W.x2, b.G + L.w[L_MSG1], b.G + L.b[L_MSG1], nullptr, b.edge_recv, re, 256, 256, A, st));
-    RC(dense_bwd_data(b, L, TL, L_MSG1, EPI_RELU_MASK, false, gw + W.x2, gw + W.x1, fw + W.x1, re, st));
+    RC(dense_bwd_data(b, L, boff, L_MSG1, EPI_RELU_MASK, false, gw + W.x2, gw + W.x1, fw + W.x1, re, st));
     // ---- edge layer 1
     RC(edge_l1_bwd(b, L, gw + W.x1, fw + W.feat, wgrad, st));
 #undef WG
@@ -769,14 +763,6 @@ static int32_t gnn_backward_impl(const BwdArgs& b, cudaStream_t st) {
 // weights (accumulated over the passes of a network in `Gf`, InferLayout offsets) are un-folded onto the flax
 // parameters at the end by the chain rule of the products (unfold_jobs: two launches of small products for both networks).
 // Same function, same gradient; only the rounding differs (~1e-6 relative, like the rollout's folded forward).
-int32_t prepare_infer_pair(int ed, int out_a, const float* Pa, float* blob_a, int out_b, const float* Pb, float* blob_b,
-                           cudaStream_t st);
-int32_t gnn_infer_impl(const gcbf_env_desc* d, int out_dim, const float* P, const float* blob, int use_tc,
-                       const float* agent, const float* goal, const float* hits, const int32_t* row_start,
-                       const int32_t* row_deg, const int32_t* edge_recv, const int32_t* edge_src,
-                       const int32_t* counters, int clip_all, float* out, float* ws, cudaStream_t st, float* z_out,
-                       int* z_parts, int32_t* zero_counter, int select, int keep_activations);
-
 static int32_t gnn_backward_folded(const BwdArgs& b, const float* blob, float* Gf, cudaStream_t st) {
     const gcbf_env_desc* d = b.d;
     const int ed = env_ed(d->env_kind);
@@ -960,13 +946,12 @@ static QpWs make_qp_ws(const gcbf_env_desc* d) {
     const int ed = env_ed(d->env_kind);
     const int64_t A = (int64_t)d->n_graphs * d->n_agents, cap = d->edge_cap;
     const GnnWs W = make_ws(d->edge_cap, A);
-    const ParamLayout Lc = make_layout(ed, 1);
     QpWs t;
     int64_t o = 0;
     auto take = [&](int64_t n) { int64_t r = o; o += (n + 7) & ~(int64_t)7; return r; };   // 32-byte slots: 256-bit epilogue stores
     t.ws0 = take(W.total);
     t.gws = take(W.total);
-    t.pt_cbf = take(make_prepared_layout(Lc, make_trans_layout(Lc)).total);
+    t.pt_cbf = take(make_plane_layout(make_deep_layout(ed, 1, 1), ed).total);   // also holds the SIMT TransLayout
     t.h = take(A);
     t.ones = take(A);
     t.je = take(cap * 8);
@@ -1125,8 +1110,8 @@ extern "C" __attribute__((visibility("default"))) int32_t gcbf_train_step(
         if (use_tc)
             return gnn_infer_impl(d, out_dim, params, blob, 1, x, goal, hits, row_start, row_deg, edge_recv, edge_src,
                                   counters, clip_all, out, fws, st, nullptr, nullptr, nullptr, 0xF, 1);
-        return gnn_forward_impl(d, out_dim, params, nullptr, x, goal, hits, row_start, row_deg, edge_recv, edge_src,
-                                counters, clip_all, out, fws, st);
+        return gnn_forward(d, out_dim, 1, params, nullptr, x, goal, hits, row_start, row_deg, edge_recv, edge_src,
+                           counters, clip_all, out, nullptr, fws, st);
     };
     RC(forward(1, cbf_params, blob_c, agent, 0, ws + TW.h, ws + TW.ws0));
     RC(forward(nu, actor_params, blob_a, agent, 0, ws + TW.pi, ws + TW.ws1));
@@ -1297,11 +1282,11 @@ extern "C" __attribute__((visibility("default"))) int32_t gcbf_qp_labels(
     float* ws = workspace;
     int32_t rc;
 #define RC(x) do { if ((rc = (x))) return rc; } while (0)
-    if (use_tensor_cores) RC(build_prepared(Lc, cbf_params, ws + Q.pt_cbf, st));
+    if (use_tensor_cores) RC(build_planes(ed, 1, 1, cbf_params, ws + Q.pt_cbf, st));
     else RC(build_transposes(Lc, make_trans_layout(Lc), cbf_params, ws + Q.pt_cbf, st));
     // h = cbf(add_edge_feats(graph, x)): every edge feature norm-clipped (gcbf_plus.py:310-316)
-    RC(gnn_forward_impl(d, 1, cbf_params, use_tensor_cores ? ws + Q.pt_cbf : nullptr, agent, goal, hits, row_start, row_deg,
-                        edge_recv, edge_src, counters, 1, ws + Q.h, ws + Q.ws0, st));
+    RC(gnn_forward(d, 1, 1, cbf_params, use_tensor_cores ? ws + Q.pt_cbf : nullptr, agent, goal, hits, row_start, row_deg,
+                   edge_recv, edge_src, counters, 1, ws + Q.h, nullptr, ws + Q.ws0, st));
     fill_kernel<<<min((A + 255) / 256, 2 * sm_count()), 256, 0, st>>>(ws + Q.ones, A, 1.f);
     count_launch();
     RC(check_launch("fill_kernel"));
@@ -1378,7 +1363,7 @@ extern "C" __attribute__((visibility("default"))) int32_t gcbf_refine_prepare(in
     GCBF_REQUIRE((((uintptr_t)cbf_params | (uintptr_t)prepared) & 15) == 0, "buffers must be 16-byte aligned");
     const ParamLayout Lc = make_layout(edge_dim, 1);
     cudaStream_t st = (cudaStream_t)stream;
-    if (use_tensor_cores) return build_prepared(Lc, cbf_params, prepared, st);
+    if (use_tensor_cores) return build_planes(edge_dim, 1, 1, cbf_params, prepared, st);
     return build_transposes(Lc, make_trans_layout(Lc), cbf_params, prepared, st);
 }
 
@@ -1419,8 +1404,8 @@ extern "C" __attribute__((visibility("default"))) int32_t gcbf_refine_actions(
     int32_t rc;
 #define RC(x) do { if ((rc = (x))) return rc; } while (0)
     auto forward = [&](const float* x, int clip_all, const int32_t* cnt, const int32_t* arows, float* out) -> int32_t {
-        return gnn_forward_impl(d, 1, cbf_params, use_tensor_cores ? PT : nullptr, x, goal, hits, row_start, row_deg,
-                                edge_recv, edge_src, cnt, clip_all, out, ws + R.fw, st, arows);
+        return gnn_forward(d, 1, 1, cbf_params, use_tensor_cores ? PT : nullptr, x, goal, hits, row_start, row_deg,
+                           edge_recv, edge_src, cnt, clip_all, out, nullptr, ws + R.fw, st, arows);
     };
     // 1. h = cbf(g) on the graph's own edge features
     RC(forward(agent, 0, counters, nullptr, ws + R.h));

@@ -1,5 +1,5 @@
-// translayout.cuh -- transposed copies of the GEMM weights of one network: the K-major B operands of
-// the tensor-core forward (Y = X @ W -> Bt = W^T) and the backward-data operands of the SIMT path.
+// translayout.cuh -- the GEMM weights of a network in the layouts the GEMMs read: transposed fp32 copies (TransLayout,
+// the backward-data operands of the SIMT path) and tf32 hi / lo planes (PlaneLayout, the tensor-core path).
 #pragma once
 #include "common.cuh"
 
@@ -54,22 +54,49 @@ static int32_t build_transposes(const ParamLayout& L, const TransLayout& T, cons
     return 0;
 }
 
-
-
-// "Prepared" parameters of one network for the tensor-core path (gcbf_prepare_params):
-//   [ W^T hi | W^T lo | W hi | W lo ]   (tf32 split planes; W^T in TransLayout order, W in ParamLayout order)
-// forward GEMMs read the W^T planes (K-major B operand), backward-data GEMMs the W planes.
-struct PreparedLayout {
-    int pt_hi, pt_lo, p_hi, p_lo, total;
+// tf32 hi / lo planes of the GEMM weights of an n_layers-deep network (gcbf_prepare_params_l): the one prepared-weights
+// format of the unfolded network.  Slot i < 12 is Dense layer i of DeepLayout layer[l] (L_MSG0 holds Ws, DEEP_WR holds
+// Wr at l >= 1; the head lives in layer 0's slots); layer 0's update/Dense_0 is its rows 3..130, which multiply the
+// aggregate.  src / rows / cols: the weight in the parameters.  Per slot:
+//   t[l][i]: W^T hi, then W^T lo at + rows * cols (K-major B operand of the forward); -1: not a GEMM operand;
+//   s[i] (n_layers = 1 only, else -1): W hi, then W lo (K-major B operand of the backward-data GEMM dX = dY W^T).
+constexpr int DEEP_WR = 12;
+struct PlaneLayout {
+    int t[GCBF_MAX_LAYERS][13], src[GCBF_MAX_LAYERS][13], rows[GCBF_MAX_LAYERS][13], cols[GCBF_MAX_LAYERS][13];
+    int s[13];
+    int total;
 };
-inline PreparedLayout make_prepared_layout(const ParamLayout& L, const TransLayout& T) {
-    PreparedLayout q;
-    q.pt_hi = 0;
-    q.pt_lo = T.total;
-    q.p_hi = 2 * T.total;
-    q.p_lo = 2 * T.total + L.total;
-    q.total = 2 * T.total + 2 * L.total;
-    return q;
+inline PlaneLayout make_plane_layout(const DeepLayout& D, int ed) {
+    PlaneLayout Q;
+    int off = 0;
+    for (int l = 0; l < D.n_layers; ++l) {
+        const ParamLayout& L = D.layer[l];
+        for (int i = 0; i < 13; ++i) {
+            int src = -1, rows = 0;
+            if (i == L_MSG0 || i == DEEP_WR) {
+                if (l > 0) { src = L.w[L_MSG0] + (ed + (i == DEEP_WR ? 128 : 0)) * 256; rows = 128; }
+            } else if (i == L_UPD0) {
+                src = L.w[i] + (l == 0 ? 3 * 256 : 0);
+                rows = l == 0 ? 128 : 256;
+            } else if (i == L_HEAD0 || i == L_HEAD1) {
+                if (l == 0) { src = L.w[i]; rows = L.in[i]; }
+            } else if (i != L_GATE && i != L_OUT) {
+                src = L.w[i];
+                rows = L.in[i];
+            }
+            const int cols = (i == DEEP_WR) ? 256 : L.out[i];
+            Q.src[l][i] = src;
+            Q.rows[l][i] = rows;
+            Q.cols[l][i] = cols;
+            Q.t[l][i] = src < 0 ? -1 : off;
+            if (src >= 0) off += 2 * rows * cols;
+            if (l > 0) continue;
+            Q.s[i] = (src < 0 || D.n_layers > 1) ? -1 : off;
+            if (Q.s[i] >= 0) off += 2 * rows * cols;
+        }
+    }
+    Q.total = off;
+    return Q;
 }
 
 }  // namespace gcbf

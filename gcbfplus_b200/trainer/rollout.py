@@ -4,9 +4,9 @@ and trainer/trainer.py:81-87.
 Two device paths with the same arithmetic (bit-identical results, tests/test_gpu_rollout.py):
 * persistent (default where supported: 2-D environments, n <= 512): ONE kernel launch for the whole T-step rollout, one
   thread-block cluster per environment looping over the steps (csrc/rollout_persist.cu);
-* 5-launch env-step (gcbf_rollout_step), the whole T-step loop captured in one CUDA graph: LinearDrone, n > 512,
-  GCBF_PERSISTENT=0, the u_ref policy, and actors with more than one GNN layer (gcbf_rollout_step_l; the engine takes
-  the depth from the network set_params() receives).
+* 5-launch env-step (gcbf_rollout_step_l), the whole T-step loop captured in one CUDA graph: LinearDrone, n > 512,
+  GCBF_PERSISTENT=0, the u_ref policy, and actors with more than one GNN layer (the engine takes the depth from the
+  network set_params() receives).
 No host sync inside the loop on either path.
 The CBF-QP baselines (algo/cbf_qp.py) run on the CUDA-graph path: per step the pairwise CBFs + QP solve (2 launches),
 env.step with the QP action as input, and the graph build of the next state.
@@ -44,13 +44,13 @@ class _Chain:
         cap = self.desc.edge_cap
         self.pi = torch.zeros(E, N, nu, dtype=f32, device=dev)
         # edge lists are double-buffered: step t reads half t % 2 while the graph of state t+1 is written into the
-        # other half (gcbf_rollout_step's fused tail + graph build reads the old lists for the step cost)
+        # other half (gcbf_rollout_step_l's fused tail + graph build reads the old lists for the step cost)
         self.row_start = torch.zeros(2, E * N, dtype=i32, device=dev)
         self.row_deg = torch.zeros(2, E * N, dtype=i32, device=dev)
         self.edge_recv = torch.zeros(2, cap, dtype=i32, device=dev)
         self.edge_src = torch.zeros(2, cap, dtype=i32, device=dev)
         self.counters = torch.zeros(eng.T + 1, 4, dtype=i32, device=dev)
-        n_ws = env.lib.gcbf_rollout_workspace_floats(C.byref(self.desc))
+        n_ws = env.lib.gcbf_rollout_workspace_floats_l(C.byref(self.desc), 1)
         self.ws = torch.empty(int(n_ws), dtype=f32, device=dev)
         if eng.controller is not None:
             # CBF-QP baseline: pairwise-CBF workspace, relaxations (scratch) and the per-step iteration record
@@ -166,7 +166,10 @@ class RolloutEngine:
         env, d = self.env, ch.desc
         obs = self.obstacles[ch.e0].data_ptr() if self.O > 0 else None
         b = t % 2
-        if self.policy == "actor" and self.n_layers > 1:
+        if self.policy == "actor_refine":
+            self._step_refine(ch, t, stream)
+            return
+        if self.policy == "actor":      # algo.step + env.step + get_graph(next) in one call
             rc = env.lib.gcbf_rollout_step_l(
                 C.byref(d), self.n_layers, self.params_buf.data_ptr(), self.infer_blob.data_ptr(), self.use_tc,
                 self.agent[t, ch.e0].data_ptr(), self.goal[ch.e0].data_ptr(), obs, env.ray_table.data_ptr(),
@@ -178,22 +181,6 @@ class RolloutEngine:
                 self.rewards[t, ch.e0:].data_ptr(), self.costs[t, ch.e0:].data_ptr(), ch.ws.data_ptr(), ch.ws.numel(),
                 stream)
             _lib.check(rc, "gcbf_rollout_step_l")
-            return
-        if self.policy == "actor_refine":
-            self._step_refine(ch, t, stream)
-            return
-        if self.policy == "actor":      # algo.step + env.step + get_graph(next) in one call (6 launches)
-            rc = env.lib.gcbf_rollout_step(
-                C.byref(d), self.params_buf.data_ptr(), self.infer_blob.data_ptr(), self.use_tc,
-                self.agent[t, ch.e0].data_ptr(), self.goal[ch.e0].data_ptr(), obs, env.ray_table.data_ptr(),
-                self.hits[t, ch.e0].data_ptr(), ch.row_start[b].data_ptr(), ch.row_deg[b].data_ptr(),
-                ch.edge_recv[b].data_ptr(), ch.edge_src[b].data_ptr(), ch.counters[t].data_ptr(),
-                self.actions[t, ch.e0].data_ptr(), self.agent[t + 1, ch.e0].data_ptr(),
-                self.hits[t + 1, ch.e0].data_ptr(), ch.row_start[1 - b].data_ptr(), ch.row_deg[1 - b].data_ptr(),
-                ch.edge_recv[1 - b].data_ptr(), ch.edge_src[1 - b].data_ptr(), ch.counters[t + 1].data_ptr(),
-                self.rewards[t, ch.e0:].data_ptr(), self.costs[t, ch.e0:].data_ptr(), ch.ws.data_ptr(), ch.ws.numel(),
-                stream)
-            _lib.check(rc, "gcbf_rollout_step")
             return
         mode = 2                        # u_ref policy
         if self.controller is not None:  # CBF-QP action, then env.step with it as input

@@ -95,13 +95,10 @@ int32_t gcbf_version(void);
 /* number of thread-block launches of this library's kernels since process start
  * (host-side counter; used by bench.py for "gpu_launches"). */
 int64_t gcbf_launch_count(void);
-/* size in floats of one network's flat parameter buffer and the offset table
- * (24 entries: W,b of the 12 Dense layers in forward order, see DESIGN.md). */
-int32_t gcbf_param_count(int32_t edge_dim, int32_t out_dim);
-int32_t gcbf_param_offsets(int32_t edge_dim, int32_t out_dim, int32_t* offsets24_host);
-/* The same for a network with n_layers GNN layers (gnn.py:78-104; 1 <= n_layers <= 8): W,b of the 9 Dense layers
- * of GNN layer 0, ..., of layer n_layers - 1, then of the 3 head layers (2 * (9 * n_layers + 3) entries).  From
- * layer 1 on, msg/Dense_0 is [ed + 256, 256] and update/Dense_0 is [256, 256].  n_layers = 1: the layout above. */
+/* size in floats of the flat parameter buffer of a network with n_layers GNN layers (gnn.py:78-104;
+ * 1 <= n_layers <= 8) and its offset table: W,b of the 9 Dense layers of GNN layer 0, ..., of layer n_layers - 1, then
+ * of the 3 head layers (2 * (9 * n_layers + 3) entries, forward order, see DESIGN.md; n_layers = 1: 24 entries, the
+ * reference's 12 Dense layers).  From layer 1 on, msg/Dense_0 is [ed + 256, 256] and update/Dense_0 is [256, 256]. */
 int32_t gcbf_param_count_l(int32_t edge_dim, int32_t out_dim, int32_t n_layers);
 int32_t gcbf_param_offsets_l(int32_t edge_dim, int32_t out_dim, int32_t n_layers, int32_t* offsets_host);
 
@@ -126,25 +123,13 @@ int32_t gcbf_graph_build(const gcbf_env_desc* desc, const float* agent, const fl
  * (gcbfplus/nn/gnn.py:44-104, nn/mlp.py:6-30, algo/module/cbf.py:12-53,
  * algo/module/policy.py:63-128), including env.add_edge_feats when clip_all = 1
  * (env/double_integrator.py:275-286).
- * params: flat fp32 buffer (gcbf_param_offsets).  out: [A, out_dim] (tanh applied).
- * params_t: NULL -> strict-fp32 SIMT GEMMs; else the transposed GEMM weights from
- * gcbf_prepare_params -> wgmma tensor-core GEMMs (3xTF32 split, fp32 accumulate; same tolerance).
- * workspace: gcbf_gnn_workspace_floats() floats; holds the saved activations
- * the backward pass reads. */
-int64_t gcbf_gnn_workspace_floats(const gcbf_env_desc* desc, int32_t out_dim);
-int32_t gcbf_params_t_count(int32_t edge_dim, int32_t out_dim);
-int32_t gcbf_prepare_params(int32_t edge_dim, int32_t out_dim, const float* params, float* params_t,
-                            void* stream);
-int32_t gcbf_gnn_forward(const gcbf_env_desc* desc, int32_t net_kind, int32_t out_dim,
-                         const float* params, const float* params_t, const float* agent, const float* goal,
-                         const float* hits,
-                         const int32_t* row_start, const int32_t* row_deg, const int32_t* edge_recv,
-                         const int32_t* edge_src, const int32_t* counters, int32_t clip_all, float* out,
-                         float* workspace, int64_t workspace_floats, void* stream);
-/* The same for n_layers GNN layers (params in the gcbf_param_offsets_l layout).  n_layers = 1 is the call above.
- * n_layers > 1 runs on the tensor-core path only (params_t from gcbf_prepare_params_l must not be NULL): from layer 1
- * on, S = y Ws and R = y Wr are node-level GEMMs and each edge gathers S[sender] + R[receiver]; goal and hit nodes,
- * which never receive a message, are one constant row each per layer. */
+ * params: flat fp32 buffer of n_layers GNN layers (gcbf_param_offsets_l).  out: [A, out_dim] (tanh applied).
+ * params_t: NULL -> strict-fp32 SIMT GEMMs (n_layers = 1 only); else the tf32 hi / lo planes of the GEMM weights from
+ * gcbf_prepare_params_l (gcbf_params_t_count_l floats) -> wgmma tensor-core GEMMs (3xTF32 split, fp32 accumulate;
+ * same tolerance).  From layer 1 on, S = y Ws and R = y Wr are node-level GEMMs and each edge gathers
+ * S[sender] + R[receiver]; goal and hit nodes, which never receive a message, are one constant row each per layer.
+ * workspace: gcbf_gnn_workspace_floats_l() floats; at n_layers = 1 it holds the saved activations the backward pass
+ * reads. */
 int64_t gcbf_gnn_workspace_floats_l(const gcbf_env_desc* desc, int32_t out_dim, int32_t n_layers);
 int32_t gcbf_params_t_count_l(int32_t edge_dim, int32_t out_dim, int32_t n_layers);
 int32_t gcbf_prepare_params_l(int32_t edge_dim, int32_t out_dim, int32_t n_layers, const float* params,
@@ -155,7 +140,7 @@ int32_t gcbf_gnn_forward_l(const gcbf_env_desc* desc, int32_t net_kind, int32_t 
                            const int32_t* edge_recv, const int32_t* edge_src, const int32_t* counters,
                            int32_t clip_all, float* out, float* workspace, int64_t workspace_floats, void* stream);
 
-/* Inference-only forward with FOLDED weights (rollouts; same functions replaced as gcbf_gnn_forward).
+/* Inference-only forward with FOLDED weights (rollouts; same functions replaced as gcbf_gnn_forward_l).
  * Each MLP block ends in two activation-free linear layers (nn/mlp.py:23-29, act_final=False), which are
  * multiplied together once per parameter update by gcbf_prepare_infer: 4 GEMMs instead of 9 per forward and
  * 2.4x fewer FLOPs; no activations are saved.  infer_blob: gcbf_infer_count() floats (folded weights, their
@@ -219,35 +204,9 @@ int32_t gcbf_reset_positions_ex(const gcbf_env_desc* desc, const uint32_t* keys,
  * The NEXT graph (next_row_start ... next_counters) must not alias the current one: callers
  * double-buffer the edge lists (the cost of the step reads the current lists while the next ones are
  * written).  counters / next_counters are the 4-int counter blocks of the current / next graph.
- * workspace: gcbf_rollout_workspace_floats(). */
-int64_t gcbf_rollout_workspace_floats(const gcbf_env_desc* desc);
-int32_t gcbf_rollout_step(const gcbf_env_desc* desc, const float* actor_params, const float* infer_blob,
-                          int32_t use_tensor_cores, const float* agent, const float* goal,
-                          const float* obstacles, const float* ray_table, const float* hits,
-                          const int32_t* row_start, const int32_t* row_deg, const int32_t* edge_recv,
-                          const int32_t* edge_src, const int32_t* counters, float* action,
-                          float* next_agent, float* next_hits, int32_t* next_row_start,
-                          int32_t* next_row_deg, int32_t* next_edge_recv, int32_t* next_edge_src,
-                          int32_t* next_counters, float* reward, float* cost, float* workspace,
-                          int64_t workspace_floats, void* stream);
-
-/* Measurement hook: the same step with only the launches whose bit is set in `select` enqueued (bench.py times every
- * kernel of the step alone, on the buffers a full step left behind, to find the dominant one and its roofline):
- * bit 0 edge features + message layer + chained gate layer, bit 1 segment softmax + aggregate, bit 2 update layer,
- * bit 3 folded update/head layer, bit 4 policy tail + graph build of the next state.  GCBF_STEP_ALL = gcbf_rollout_step. */
-#define GCBF_STEP_ALL 31
-int32_t gcbf_rollout_step_select(const gcbf_env_desc* desc, const float* actor_params, const float* infer_blob,
-                                 int32_t use_tensor_cores, const float* agent, const float* goal,
-                                 const float* obstacles, const float* ray_table, const float* hits,
-                                 const int32_t* row_start, const int32_t* row_deg, const int32_t* edge_recv,
-                                 const int32_t* edge_src, const int32_t* counters, float* action,
-                                 float* next_agent, float* next_hits, int32_t* next_row_start,
-                                 int32_t* next_row_deg, int32_t* next_edge_recv, int32_t* next_edge_src,
-                                 int32_t* next_counters, float* reward, float* cost, float* workspace,
-                                 int64_t workspace_floats, int32_t select, void* stream);
-/* The rollout step for an actor with n_layers GNN layers.  n_layers = 1 is gcbf_rollout_step.  n_layers > 1 (tensor-core
- * path only): infer_blob is the gcbf_prepare_params_l output, the policy forward runs layer by layer unfolded
- * (gcbf_gnn_forward_l) and the same policy tail + graph build kernel ends the step.
+ * n_layers > 1 (tensor-core path only): infer_blob is the gcbf_prepare_params_l output instead of the
+ * gcbf_prepare_infer one, the policy forward runs layer by layer unfolded (gcbf_gnn_forward_l) and the same policy
+ * tail + graph build kernel ends the step.
  * workspace: gcbf_rollout_workspace_floats_l(). */
 int64_t gcbf_rollout_workspace_floats_l(const gcbf_env_desc* desc, int32_t n_layers);
 int32_t gcbf_rollout_step_l(const gcbf_env_desc* desc, int32_t n_layers, const float* actor_params,
@@ -260,13 +219,29 @@ int32_t gcbf_rollout_step_l(const gcbf_env_desc* desc, int32_t n_layers, const f
                             float* reward, float* cost, float* workspace, int64_t workspace_floats,
                             void* stream);
 
+/* Measurement hook: the same step with only the launches whose bit is set in `select` enqueued (bench.py times every
+ * kernel of the step alone, on the buffers a full step left behind, to find the dominant one and its roofline):
+ * bit 0 edge features + message layer + chained gate layer, bit 1 segment softmax + aggregate, bit 2 update layer,
+ * bit 3 folded update/head layer, bit 4 policy tail + graph build of the next state.  GCBF_STEP_ALL = the whole step
+ * (gcbf_rollout_step_l at n_layers = 1; workspace: gcbf_rollout_workspace_floats_l(desc, 1)). */
+#define GCBF_STEP_ALL 31
+int32_t gcbf_rollout_step_select(const gcbf_env_desc* desc, const float* actor_params, const float* infer_blob,
+                                 int32_t use_tensor_cores, const float* agent, const float* goal,
+                                 const float* obstacles, const float* ray_table, const float* hits,
+                                 const int32_t* row_start, const int32_t* row_deg, const int32_t* edge_recv,
+                                 const int32_t* edge_src, const int32_t* counters, float* action,
+                                 float* next_agent, float* next_hits, int32_t* next_row_start,
+                                 int32_t* next_row_deg, int32_t* next_edge_recv, int32_t* next_edge_src,
+                                 int32_t* next_counters, float* reward, float* cost, float* workspace,
+                                 int64_t workspace_floats, int32_t select, void* stream);
+
 /* ---------------------------------------------------------------- persistent rollout (a8 whole scan)
  * The WHOLE rollout() of gcbfplus/trainer/utils.py:25-55 (reset excluded) in ONE kernel launch: one thread-block cluster
- * per environment loops over the n_steps env-steps; the kernel boundaries of gcbf_rollout_step become cluster barriers,
+ * per environment loops over the n_steps env-steps; the kernel boundaries of gcbf_rollout_step_l become cluster barriers,
  * pipeline / table setup is paid once per rollout (csrc/rollout_persist.cu).  Same arithmetic as
- * gcbf_rollout_step -> same bits.  Supported: SingleIntegrator / DoubleIntegrator / DubinsCar, n_agents <= 512,
+ * gcbf_rollout_step_l -> same bits.  Supported: SingleIntegrator / DoubleIntegrator / DubinsCar, n_agents <= 512,
  * n_obs <= 32, one obstacle set per environment, desc->edge_cap >= n_graphs * n_agents (it is split evenly over the
- * environments); gcbf_rollout_persistent_supported() tells, callers fall back to gcbf_rollout_step otherwise.
+ * environments); gcbf_rollout_persistent_supported() tells, callers fall back to gcbf_rollout_step_l otherwise.
  *   agent_rec [n_steps+1, G, N, sd]: slice 0 = initial states (input), slices 1.. written;  hits_rec [n_steps+1, G, N, R, pd]
  *   (all slices written, slice 0 = LiDAR of the initial states);  actions_rec [n_steps, G, N, nu];  rewards / costs
  *   [n_steps, G];  counters [n_steps+1, 4] (zeroed by the caller): [t][0] += edges of the graphs of state t, [t][1] |= overflow.
@@ -385,7 +360,7 @@ int32_t gcbf_qp_labels(const gcbf_env_desc* desc, float alpha, int32_t use_tenso
  *   cbf_params / cbf_prepared: the CBF parameters and gcbf_refine_prepare's planes of them (rebuild them whenever
  *     the parameters change): the tf32 planes (use_tensor_cores != 0) or the transposed weights of the strict-fp32
  *     SIMT path;
- *     gcbf_params_t_count(edge_dim, 1) floats
+ *     gcbf_params_t_count_l(edge_dim, 1, 1) floats
  *   pi [A, nu]: the actor output (policy.get_action);  graph arrays as gcbf_qp_labels takes them
  *   action [A, nu] (out): the refined actions;  value [G] or NULL: the last loop value of each graph
  *   iters [G] or NULL: iterations taken, bit 30 set when the graph stopped at max_iter with value > 0

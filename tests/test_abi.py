@@ -45,11 +45,11 @@ def test_param_layout_matches_reference_counts():
         assert _lib.param_count(ed, nu) >= want_actor
 
 
-def test_error_reporting_without_gpu():
+def test_layout_query_and_graph_build_report_errors_without_gpu():
     from gcbfplus_b200 import _lib
     lib = _lib.load()
     assert lib.gcbf_version() >= 100
-    rc = lib.gcbf_param_offsets(99, 1, (ctypes.c_int32 * 24)())
+    rc = lib.gcbf_param_offsets_l(99, 1, 1, (ctypes.c_int32 * 24)())
     assert rc < 0 and b"bad argument" in lib.gcbf_last_error_string()
     d = _lib.EnvDesc()
     d.env_kind = 7

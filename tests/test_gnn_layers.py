@@ -31,26 +31,29 @@ def test_specs_names_shapes_and_counts():
             assert layer["Dense_0"] == (256, 128) and layer["Dense_2"] == (256, 128) and layer["Dense_1"] == (128, 1)
 
 
+# the tf32 planes of the GEMM weights (gcbf_params_t_count_l): hi and lo of the transposed weights of every layer and, at
+# L = 1, of the straight ones the backward reads.  The 9 GEMM weights of a layer hold 360448 floats at any ed
+# (layer 0: update/Dense_0 rows 3..130 and the two hidden head layers; later layers: Ws and Wr instead).
+PLANE_FLOATS = {1: 4 * 360448, 2: 2 * 2 * 360448, 3: 2 * 3 * 360448}
+
+
+@pytest.mark.parametrize("L", [1, 2, 3])
 @pytest.mark.parametrize("ed,nu", [(2, 2), (4, 2), (6, 3)])
-def test_library_layout_follows_the_specs(ed, nu):
+def test_library_layout_and_planes_follow_the_specs(ed, nu, L):
     from gcbfplus_b200 import _lib
     from gcbfplus_b200.algo.params import layer_specs
     lib = _lib.load()
-    assert _lib.param_count(ed, nu, 1) == lib.gcbf_param_count(ed, nu)
-    assert _lib.param_offsets(ed, nu, 1) == _lib.param_offsets(ed, nu)
-    import ctypes
-    one = (ctypes.c_int32 * 24)()
-    assert lib.gcbf_param_offsets_l(ed, nu, 1, one) == 0 and list(one) == _lib.param_offsets(ed, nu)
-    for L in (2, 3):
-        specs = layer_specs(ed, nu, "actor", L)
-        offs = _lib.param_offsets(ed, nu, L)
-        assert len(offs) == 2 * len(specs) == 2 * (9 * L + 3)
-        assert all(o % 4 == 0 for o in offs) and offs == sorted(offs)
-        ends = offs[1:] + [_lib.param_count(ed, nu, L)]
-        for k, (_, fi, fo) in enumerate(specs):
-            assert ends[2 * k] - offs[2 * k] >= fi * fo and ends[2 * k] - offs[2 * k] < fi * fo + 4
-            assert ends[2 * k + 1] - offs[2 * k + 1] >= fo
+    specs = layer_specs(ed, nu, "actor", L)
+    offs = _lib.param_offsets(ed, nu, L)
+    assert len(offs) == 2 * len(specs) == 2 * (9 * L + 3)
+    assert all(o % 4 == 0 for o in offs) and offs == sorted(offs)
+    ends = offs[1:] + [_lib.param_count(ed, nu, L)]
+    for k, (_, fi, fo) in enumerate(specs):
+        assert ends[2 * k] - offs[2 * k] >= fi * fo and ends[2 * k] - offs[2 * k] < fi * fo + 4
+        assert ends[2 * k + 1] - offs[2 * k + 1] >= fo
+    assert lib.gcbf_params_t_count_l(ed, nu, L) == PLANE_FLOATS[L]
     assert lib.gcbf_param_count_l(ed, nu, 0) < 0 and lib.gcbf_param_count_l(ed, nu, 9) < 0
+    assert lib.gcbf_params_t_count_l(ed, nu, 0) < 0 and lib.gcbf_params_t_count_l(ed, nu, 9) < 0
 
 
 @pytest.mark.parametrize("L", [2, 3])
