@@ -37,6 +37,16 @@ struct TailArgs {
     float* next_agent;         // out [A, sd]
 };
 
+// ---- workspace layouts: consecutive slots, each rounded up to `align` floats (a power of two) --------------------
+struct WsSlots {
+    int64_t align, off = 0;
+    int64_t take(int64_t n) {
+        const int64_t r = off;
+        off += (n + align - 1) & ~(align - 1);
+        return r;
+    }
+};
+
 // ---- per-environment compile-time traits -------------------------------------------
 template <int KIND> struct EnvTraits;
 template <> struct EnvTraits<GCBF_ENV_SINGLE_INTEGRATOR> { static constexpr int SD = 2, ED = 2, NU = 2, PD = 2; };

@@ -9,6 +9,7 @@
 #pragma once
 #include "gemm_tc.cuh"
 #include "gnn.cuh"
+#include "internal.cuh"
 
 namespace gcbf {
 namespace tc {
@@ -272,20 +273,19 @@ constexpr int PROD_SMEM = STAGES * STG + 256 + L1_FLOATS * 4 + 1024;
 // MSG[e, :128] = relu-layer-1(edge e) @ W23 + b23: edge_l1 producer + folded message GEMM (K = 256, N = 128), with the
 // gate layer (K = N = 128, weights gate_Bt_*) and its folded gate vector chained in the same kernel: the logits are
 // written to chain.logits.
-inline int32_t launch_edge_msg(const gcbf_env_desc* d, const float* W1, const float* b1, const float* agent,
-                               const float* goal, const float* hits, const int32_t* edge_recv,
-                               const int32_t* edge_src, const int32_t* counters, int clip_all, const float* Bt_hi,
-                               const float* Bt_lo, const float* bias, float* msg, cudaStream_t st,
-                               const float* gate_Bt_hi, const float* gate_Bt_lo, const ChainArgs& chain) {
-    if (!counters) {
+inline int32_t launch_edge_msg(const gcbf_env_desc* d, const float* W1, const float* b1, const GraphRefs& g,
+                               int clip_all, const float* Bt_hi, const float* Bt_lo, const float* bias, float* msg,
+                               cudaStream_t st, const float* gate_Bt_hi, const float* gate_Bt_lo,
+                               const ChainArgs& chain) {
+    if (!g.counters) {
         set_error("launch_edge_msg: the chained gate GEMM needs the device edge counter");
         return -1;
     }
     ProdArgs pa;
     memset(&pa, 0, sizeof(pa));
     pa.d = *d;
-    pa.W1 = W1; pa.b1 = b1; pa.agent = agent; pa.goal = goal; pa.hits = hits;
-    pa.edge_recv = edge_recv; pa.edge_src = edge_src; pa.clip_all = clip_all;
+    pa.W1 = W1; pa.b1 = b1; pa.agent = g.agent; pa.goal = g.goal; pa.hits = g.hits;
+    pa.edge_recv = g.edge_recv; pa.edge_src = g.edge_src; pa.clip_all = clip_all;
     const int K = 256, N = 128;
     CUtensorMap tmB, tmBl, tmG, tmGl;
     if (int32_t r = make_map(&tmB, Bt_hi, N, K, N)) return r;
@@ -300,7 +300,7 @@ inline int32_t launch_edge_msg(const gcbf_env_desc* d, const float* W1, const fl
             cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, PROD_SMEM);
             attr_done = true;
         }
-        kern<<<grid, THREADS_NN, PROD_SMEM, st>>>(tmB, tmBl, tmG, tmGl, pa, bias, msg, counters, d->edge_cap, chain);
+        kern<<<grid, THREADS_NN, PROD_SMEM, st>>>(tmB, tmBl, tmG, tmGl, pa, bias, msg, g.counters, d->edge_cap, chain);
         count_launch();
         return check_launch("edge_chain_kernel");
     });

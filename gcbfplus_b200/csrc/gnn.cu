@@ -146,10 +146,8 @@ int32_t prepare_infer_pair(int ed, int out_a, const float* Pa, float* blob_a, in
 }
 
 int32_t gnn_infer_impl(const gcbf_env_desc* d, int out_dim, const float* P, const float* blob, int use_tc,
-                              const float* agent, const float* goal, const float* hits, const int32_t* row_start,
-                              const int32_t* row_deg, const int32_t* edge_recv, const int32_t* edge_src,
-                              const int32_t* counters, int clip_all, float* out, float* ws, cudaStream_t st,
-                              float* z_out, int* z_parts, int32_t* zero_counter, int select, int keep_activations) {
+                       const GraphRefs& g, int clip_all, float* out, float* ws, cudaStream_t st, float* z_out,
+                       int* z_parts, int32_t* zero_counter, int select, int keep_activations) {
     // keep_activations (folded train step): the unfused launch sequence, every layer output left in the workspace
     // (feat, x1, msg, g1, att, ag, v1, h1) for the backward pass; GEMMs still on the tensor-core path when use_tc
     // select (gcbf_rollout_step_select, measurement hook): bit 0 edge message (+ chained gate) kernel, bit 1 attention
@@ -161,7 +159,7 @@ int32_t gnn_infer_impl(const gcbf_env_desc* d, int out_dim, const float* P, cons
     const InferLayout I = make_infer_layout(out_dim);
     const int A = d->n_graphs * d->n_agents, cap = d->edge_cap;
     const GnnWs W = make_ws(cap, A);
-    const RowCount re{counters, 0, cap};
+    const RowCount re{g.counters, 0, cap};
     const RowCount ra{nullptr, A, A};
     const int nsm = sm_count();
     int32_t rc;
@@ -180,17 +178,17 @@ int32_t gnn_infer_impl(const gcbf_env_desc* d, int out_dim, const float* P, cons
             ch.avec = blob + I.a23;
             ch.cst = blob + I.c23;
             ch.logits = ws + W.att;
-            if ((rc = tc::launch_edge_msg(d, P + L.w[L_MSG0], P + L.b[L_MSG0], agent, goal, hits, edge_recv, edge_src,
-                                          counters, clip_all, blob + I.t_w23, blob + I.t_w23 + 256 * 128, blob + I.b23,
-                                          ws + W.msg, st, blob + I.t_a1, blob + I.t_a1 + 128 * 128, ch))) return rc;
+            if ((rc = tc::launch_edge_msg(d, P + L.w[L_MSG0], P + L.b[L_MSG0], g, clip_all, blob + I.t_w23,
+                                          blob + I.t_w23 + 256 * 128, blob + I.b23, ws + W.msg, st, blob + I.t_a1,
+                                          blob + I.t_a1 + 128 * 128, ch))) return rc;
         }
         // (measured: producing the aggregate inside the update GEMM (tc::launch_attn_upd) is slower than the
         //  separate warp-per-receiver kernel + TMA-fed GEMM: 36.6 us vs 13.2 + 11.7 us -- its N-split repeats
         //  the aggregation and the per-thread MSG gathers are latency-bound; the edge producer above is a win)
         if (select & 2) {
             const int grid = min((A + 7) / 8, 8 * nsm);   // 8 x 256 threads per SM: one receiver per warp in flight (latency-bound kernel)
-            attn_aggregate_kernel<<<grid, 256, 0, st>>>(A, cap, nullptr, ws + W.msg, blob + I.a23, blob + I.c23, row_start,
-                                                        row_deg, ws + W.att, ws + W.ag, zero_counter);
+            attn_aggregate_kernel<<<grid, 256, 0, st>>>(A, cap, nullptr, ws + W.msg, blob + I.a23, blob + I.c23,
+                                                        g.row_start, g.row_deg, ws + W.att, ws + W.ag, zero_counter);
             count_launch();
             if ((rc = check_launch("attn_aggregate_kernel"))) return rc;
         }
@@ -200,8 +198,9 @@ int32_t gnn_infer_impl(const gcbf_env_desc* d, int out_dim, const float* P, cons
         {
             const int grid = min((cap + 7) / 8, 4 * nsm);
             GCBF_DISPATCH_ENV(d->env_kind, {
-                edge_l1_kernel<KIND><<<grid, 256, 0, st>>>(*d, P + L.w[L_MSG0], P + L.b[L_MSG0], agent, goal, hits,
-                                                           edge_recv, edge_src, counters, clip_all, ws + W.feat, ws + W.x1);
+                edge_l1_kernel<KIND><<<grid, 256, 0, st>>>(*d, P + L.w[L_MSG0], P + L.b[L_MSG0], g.agent, g.goal,
+                                                           g.hits, g.edge_recv, g.edge_src, g.counters, clip_all,
+                                                           ws + W.feat, ws + W.x1);
             });
             count_launch();
             if ((rc = check_launch("edge_l1_kernel"))) return rc;
@@ -210,8 +209,8 @@ int32_t gnn_infer_impl(const gcbf_env_desc* d, int out_dim, const float* P, cons
         if ((rc = gemm(EPI_BIAS_RELU, ws + W.msg, P + L.w[L_ATT0], I.t_a1, 128, 128, P + L.b[L_ATT0], nullptr, ws + W.g1, re))) return rc;
         {
             const int grid = min((A + 7) / 8, 8 * nsm);
-            attn_aggregate_kernel<<<grid, 256, 0, st>>>(A, cap, ws + W.g1, ws + W.msg, blob + I.a23, blob + I.c23, row_start,
-                                                        row_deg, ws + W.att, ws + W.ag, zero_counter);
+            attn_aggregate_kernel<<<grid, 256, 0, st>>>(A, cap, ws + W.g1, ws + W.msg, blob + I.a23, blob + I.c23,
+                                                        g.row_start, g.row_deg, ws + W.att, ws + W.ag, zero_counter);
             count_launch();
             if ((rc = check_launch("attn_aggregate_kernel"))) return rc;
         }
@@ -265,79 +264,17 @@ extern "C" __attribute__((visibility("default"))) int32_t gcbf_gnn_infer(
     int32_t clip_all, float* out, float* workspace, int64_t workspace_floats, void* stream) {
     GCBF_REQUIRE(desc && params && infer_blob && agent && goal && hits && row_start && row_deg && edge_recv && edge_src &&
                      counters && out && workspace, "gcbf_gnn_infer: NULL pointer argument");
-    GCBF_REQUIRE(desc->env_kind >= 0 && desc->env_kind <= 3, "bad env_kind");
+    if (int32_t rc = check_graph_desc(desc, "gcbf_gnn_infer")) return rc;
     GCBF_REQUIRE(net_kind == GCBF_NET_CBF || net_kind == GCBF_NET_ACTOR, "bad net_kind %d", net_kind);
     GCBF_REQUIRE(out_dim >= 1 && out_dim <= 4 && (net_kind != GCBF_NET_CBF || out_dim == 1), "bad out_dim %d", out_dim);
-    GCBF_REQUIRE(desc->edge_cap > 0, "edge_cap must be positive");
     const int64_t need = make_ws(desc->edge_cap, (int64_t)desc->n_graphs * desc->n_agents).total;
     GCBF_REQUIRE(workspace_floats >= need, "workspace too small: %lld < %lld floats", (long long)workspace_floats,
                  (long long)need);
     GCBF_REQUIRE((((uintptr_t)params | (uintptr_t)workspace | (uintptr_t)infer_blob) & 15) == 0,
                  "params/infer_blob/workspace must be 16-byte aligned");
-    return gnn_infer_impl(desc, out_dim, params, infer_blob, use_tensor_cores, agent, goal, hits, row_start, row_deg,
-                          edge_recv, edge_src, counters, clip_all, out, workspace, (cudaStream_t)stream);
-}
-
-// ---------------------------------------------------------------------------------------------------
-// One closed-loop rollout step in a single call: policy forward (folded weights) -> a = 2 pi + u_ref,
-// clip, Euler, reward / cost terms -> LiDAR + neighbour lists of the next state (+ reward / cost reduction).
-// 5 kernel launches (tensor-core path).
-// ---------------------------------------------------------------------------------------------------
-extern "C" __attribute__((visibility("default"))) int32_t gcbf_rollout_step_select(
-    const gcbf_env_desc* desc, const float* actor_params, const float* infer_blob, int32_t use_tensor_cores,
-    const float* agent, const float* goal, const float* obstacles, const float* ray_table, const float* hits,
-    const int32_t* row_start, const int32_t* row_deg, const int32_t* edge_recv, const int32_t* edge_src,
-    const int32_t* counters, float* action, float* next_agent, float* next_hits, int32_t* next_row_start,
-    int32_t* next_row_deg, int32_t* next_edge_recv, int32_t* next_edge_src, int32_t* next_counters, float* reward,
-    float* cost, float* workspace, int64_t workspace_floats, int32_t select, void* stream) {
-    GCBF_REQUIRE(desc && actor_params && infer_blob && agent && goal && ray_table && hits && row_start && row_deg &&
-                     edge_recv && edge_src && counters && action && next_agent && next_hits && next_row_start &&
-                     next_row_deg && next_edge_recv && next_edge_src && next_counters && reward && cost && workspace,
-                 "gcbf_rollout_step_select: NULL pointer argument");
-    GCBF_REQUIRE(next_row_start != row_start && next_row_deg != row_deg && next_edge_recv != edge_recv &&
-                     next_edge_src != edge_src && next_counters != counters,
-                 "gcbf_rollout_step_select: the next graph must not alias the current one (double-buffer the edge lists)");
-    GCBF_REQUIRE(desc->env_kind >= 0 && desc->env_kind <= 3 && desc->edge_cap > 0, "gcbf_rollout_step_select: bad descriptor");
-    GCBF_REQUIRE(desc->n_obs == 0 || obstacles, "obstacles is NULL but n_obs > 0");
-    const int nu = env_nu(desc->env_kind);
-    const int64_t A = (int64_t)desc->n_graphs * desc->n_agents;
-    const GnnWs W = make_ws(desc->edge_cap, A);
-    const int64_t need = W.total + 8 * A + 8;
-    GCBF_REQUIRE(workspace_floats >= need, "workspace too small: %lld < %lld floats", (long long)workspace_floats,
-                 (long long)need);
-    GCBF_REQUIRE(((uintptr_t)workspace & 15) == 0, "workspace must be 16-byte aligned");
-    cudaStream_t st = (cudaStream_t)stream;
-    const InferLayout I = make_infer_layout(nu);
-    float* z = workspace + ((W.total + 3) & ~(int64_t)3);    // [2][A][4] output-layer partial sums
-    int32_t rc;
-    int parts = 1;
-    // 6 launches, no memset / copy node in between: {edge features + message layer}, {gate layer -> logits},
-    // {segment softmax + aggregate; clears the next edge counter}, {update layer}, {folded update/head layer + output
-    // layer partial sums}, {policy tail fused into the graph build of the next state}.
-    // (Programmatic dependent launch of this chain was built and measured: +1 % (inside a CUDA graph the
-    //  kernel-to-kernel gap is already ~1 us) and it was NOT safe as written -- a dependent kernel that starts early
-    //  can keep L1 / read-only-cache lines of buffers its predecessor rewrites (DubinsCar rollouts became
-    //  non-deterministic with only the edge-message GEMM launched that way).  Removed.)
-    GCBF_REQUIRE(select == GCBF_STEP_ALL || use_tensor_cores, "gcbf_rollout_step_select: partial steps need the tensor-core path");
-    if ((rc = gnn_infer_impl(desc, nu, actor_params, infer_blob, use_tensor_cores, agent, goal, hits, row_start, row_deg,
-                             edge_recv, edge_src, counters, 0, nullptr, workspace, st, z, &parts, next_counters,
-                             select & 0xF))) return rc;
-    if (!(select & 16)) return 0;
-    TailArgs tl;
-    tl.z = z;
-    tl.parts = parts;
-    tl.z_cap = (int)A;
-    tl.bHO = infer_blob + I.bho;
-    tl.agent_prev = agent;
-    tl.goal = goal;
-    tl.row_start_prev = row_start;
-    tl.row_deg_prev = row_deg;
-    tl.edge_src_prev = edge_src;
-    tl.action = action;
-    tl.next_agent = next_agent;
-    // the attention kernel cleared the next edge counter; a partial step without it lets the build clear it itself
-    return graph_build_impl(desc, nullptr, obstacles, ray_table, next_hits, next_row_start, next_row_deg, next_edge_recv,
-                            next_edge_src, next_counters, 1 | ((select & 2) ? 4 : 0), tl, reward, cost, stream);
+    const GraphRefs g{agent, goal, hits, row_start, row_deg, edge_recv, edge_src, counters};
+    return gnn_infer_impl(desc, out_dim, params, infer_blob, use_tensor_cores, g, clip_all, out, workspace,
+                          (cudaStream_t)stream);
 }
 
 // =====================================================================================================
@@ -378,11 +315,13 @@ struct DeepWs {
 static DeepWs make_deep_ws(int64_t cap, int64_t A, int n_layers) {
     DeepWs W;
     const int64_t nodes = n_layers > 1 ? A + 2 : A, node_block = n_layers > 1 ? nodes * 256 : 0;
+    WsSlots S{8};
     W.g = make_ws(cap, nodes);
-    W.s = W.g.total;
-    W.r = W.s + node_block;
-    W.cat = W.r + node_block;
-    W.total = W.cat + node_block;
+    S.take(W.g.total);
+    W.s = S.take(node_block);
+    W.r = S.take(node_block);
+    W.cat = S.take(node_block);
+    W.total = S.off;
     return W;
 }
 
@@ -452,16 +391,15 @@ node_concat_kernel(const int A, const float* __restrict__ Y, const float* __rest
 }
 
 int32_t gnn_forward(const gcbf_env_desc* d, int out_dim, int n_layers, const float* P, const float* PT,
-                    const float* agent, const float* goal, const float* hits, const int32_t* row_start,
-                    const int32_t* row_deg, const int32_t* edge_recv, const int32_t* edge_src, const int32_t* counters,
-                    int clip_all, float* out, float* z_out, float* ws, cudaStream_t st, const int32_t* agent_rows) {
+                    const GraphRefs& g, int clip_all, float* out, float* z_out, float* ws, cudaStream_t st,
+                    const int32_t* agent_rows) {
     const int ed = env_ed(d->env_kind);
     const DeepLayout D = make_deep_layout(ed, out_dim, n_layers);
     const PlaneLayout Q = make_plane_layout(D, ed);
     const int A = d->n_graphs * d->n_agents, cap = d->edge_cap;
     const DeepWs DW = make_deep_ws(cap, A, n_layers);
     const GnnWs& W = DW.g;
-    const RowCount re{counters, 0, cap};
+    const RowCount re{g.counters, 0, cap};
     const RowCount ra{agent_rows, A, A};
     const RowCount ra2{nullptr, A + 2, A + 2};
     const int nsm = sm_count();
@@ -482,9 +420,9 @@ int32_t gnn_forward(const gcbf_env_desc* d, int out_dim, int n_layers, const flo
         const int egrid = min((cap + 7) / 8, 4 * nsm);
         if (l == 0) {
             GCBF_DISPATCH_ENV(d->env_kind, {
-                edge_l1_kernel<KIND><<<egrid, 256, 0, st>>>(*d, P + L.w[L_MSG0], P + L.b[L_MSG0], agent, goal, hits,
-                                                            edge_recv, edge_src, counters, clip_all, ws + W.feat,
-                                                            ws + W.x1);
+                edge_l1_kernel<KIND><<<egrid, 256, 0, st>>>(*d, P + L.w[L_MSG0], P + L.b[L_MSG0], g.agent, g.goal,
+                                                            g.hits, g.edge_recv, g.edge_src, g.counters, clip_all,
+                                                            ws + W.feat, ws + W.x1);
             });
             count_launch();
             if ((rc = check_launch("edge_l1_kernel"))) return rc;
@@ -493,8 +431,8 @@ int32_t gnn_forward(const gcbf_env_desc* d, int out_dim, int n_layers, const flo
             if ((rc = gemm(EPI_NONE, l, DEEP_WR, ws + W.v3, nullptr, nullptr, ws + DW.r, ra))) return rc;
             GCBF_DISPATCH_ENV(d->env_kind, {
                 edge_deep_kernel<EnvTraits<KIND>::ED><<<egrid, 256, 0, st>>>(
-                    A, cap, P + L.w[L_MSG0], P + L.b[L_MSG0], ws + W.feat, ws + DW.s, ws + DW.r, edge_recv, edge_src,
-                    counters, ws + W.x1);
+                    A, cap, P + L.w[L_MSG0], P + L.b[L_MSG0], ws + W.feat, ws + DW.s, ws + DW.r, g.edge_recv,
+                    g.edge_src, g.counters, ws + W.x1);
             });
             count_launch();
             if ((rc = check_launch("edge_deep_kernel"))) return rc;
@@ -506,7 +444,7 @@ int32_t gnn_forward(const gcbf_env_desc* d, int out_dim, int n_layers, const flo
         {
             const int grid = min((A + 7) / 8, 4 * nsm);
             attn_aggregate_kernel<<<grid, 256, 0, st>>>(A, cap, ws + W.g2, ws + W.msg, P + L.w[L_GATE], P + L.b[L_GATE],
-                                                        row_start, row_deg, ws + W.att, ws + W.ag);
+                                                        g.row_start, g.row_deg, ws + W.att, ws + W.ag);
             count_launch();
             if ((rc = check_launch("attn_aggregate_kernel"))) return rc;
         }
@@ -549,8 +487,17 @@ static bool deep_dims_ok(int32_t edge_dim, int32_t out_dim, int32_t n_layers) {
            n_layers <= gcbf::GCBF_MAX_LAYERS;
 }
 static bool ws_dims_ok(const gcbf_env_desc* desc, int32_t n_layers) {
-    return desc && desc->edge_cap > 0 && desc->n_graphs > 0 && desc->n_agents > 0 && n_layers >= 1 &&
-           n_layers <= gcbf::GCBF_MAX_LAYERS;
+    return graph_sizes_ok(desc) && n_layers >= 1 && n_layers <= gcbf::GCBF_MAX_LAYERS;
+}
+
+// Workspace of the rollout step: the forward's (make_deep_ws) and, 16-byte aligned after it, the output layer's
+// partial sums z [2][A][4].
+struct StepWs {
+    int64_t z, total;
+};
+static StepWs make_step_ws(const gcbf_env_desc* d, int n_layers) {
+    const int64_t A = (int64_t)d->n_graphs * d->n_agents, fwd = make_deep_ws(d->edge_cap, A, n_layers).total;
+    return {(fwd + 3) & ~(int64_t)3, fwd + 8 * A + 16};
 }
 
 extern "C" __attribute__((visibility("default"))) int32_t gcbf_params_t_count_l(int32_t edge_dim, int32_t out_dim,
@@ -586,24 +533,95 @@ extern "C" __attribute__((visibility("default"))) int32_t gcbf_gnn_forward_l(
     GCBF_REQUIRE(n_layers == 1 || params_t, "gcbf_gnn_forward_l: n_layers > 1 runs on the tensor-core path only "
                                             "(params_t from gcbf_prepare_params_l); the strict-fp32 SIMT path "
                                             "implements n_layers = 1");
-    GCBF_REQUIRE(desc->env_kind >= 0 && desc->env_kind <= 3, "bad env_kind");
+    if (int32_t rc = check_graph_desc(desc, "gcbf_gnn_forward_l")) return rc;
     GCBF_REQUIRE(net_kind == GCBF_NET_CBF || net_kind == GCBF_NET_ACTOR, "bad net_kind %d", net_kind);
     GCBF_REQUIRE(out_dim >= 1 && out_dim <= 4 && (net_kind != GCBF_NET_CBF || out_dim == 1), "bad out_dim %d", out_dim);
-    GCBF_REQUIRE(desc->edge_cap > 0, "edge_cap must be positive");
     const int64_t need = make_deep_ws(desc->edge_cap, (int64_t)desc->n_graphs * desc->n_agents, n_layers).total;
     GCBF_REQUIRE(workspace_floats >= need, "workspace too small: %lld < %lld floats", (long long)workspace_floats,
                  (long long)need);
     GCBF_REQUIRE((((uintptr_t)params | (uintptr_t)params_t | (uintptr_t)workspace) & 15) == 0,
                  "params/params_t/workspace must be 16-byte aligned");
-    return gnn_forward(desc, out_dim, n_layers, params, params_t, agent, goal, hits, row_start, row_deg, edge_recv,
-                       edge_src, counters, clip_all, out, nullptr, workspace, (cudaStream_t)stream);
+    const GraphRefs g{agent, goal, hits, row_start, row_deg, edge_recv, edge_src, counters};
+    return gnn_forward(desc, out_dim, n_layers, params, params_t, g, clip_all, out, nullptr, workspace,
+                       (cudaStream_t)stream);
 }
 
 extern "C" __attribute__((visibility("default"))) int64_t gcbf_rollout_workspace_floats_l(const gcbf_env_desc* desc,
                                                                                          int32_t n_layers) {
     if (!ws_dims_ok(desc, n_layers)) return -1;
-    const int64_t A = (int64_t)desc->n_graphs * desc->n_agents;
-    return make_deep_ws(desc->edge_cap, A, n_layers).total + 8 * A + 16;
+    return make_step_ws(desc, n_layers).total;
+}
+
+// ---------------------------------------------------------------------------------------------------
+// One closed-loop rollout step in a single call: policy forward -> a = 2 pi + u_ref, clip, Euler, reward / cost terms
+// -> LiDAR + neighbour lists of the next state (+ reward / cost reduction).
+// n_layers = 1: the folded forward (gnn_infer_impl), 6 launches on the tensor-core path with no memset / copy node in
+// between: {edge features + message layer}, {gate layer -> logits}, {segment softmax + aggregate; clears the next edge
+// counter}, {update layer}, {folded update/head layer + output layer partial sums}, {policy tail fused into the graph
+// build of the next state}.  `select` (gcbf_rollout_step_select) skips launches of that chain.
+// n_layers > 1: the unfolded forward (gnn_forward) on the tensor-core path, then the same fused tail and build.
+// (Programmatic dependent launch of this chain was built and measured: +1 % (inside a CUDA graph the kernel-to-kernel
+//  gap is already ~1 us) and it was NOT safe as written -- a dependent kernel that starts early can keep L1 /
+//  read-only-cache lines of buffers its predecessor rewrites (DubinsCar rollouts became non-deterministic with only the
+//  edge-message GEMM launched that way).  Removed.)
+// ---------------------------------------------------------------------------------------------------
+static int32_t rollout_step(
+    const char* fn, const gcbf_env_desc* desc, int32_t n_layers, const float* actor_params, const float* infer_blob,
+    int32_t use_tensor_cores, const float* agent, const float* goal, const float* obstacles, const float* ray_table,
+    const float* hits, const int32_t* row_start, const int32_t* row_deg, const int32_t* edge_recv,
+    const int32_t* edge_src, const int32_t* counters, float* action, float* next_agent, float* next_hits,
+    int32_t* next_row_start, int32_t* next_row_deg, int32_t* next_edge_recv, int32_t* next_edge_src,
+    int32_t* next_counters, float* reward, float* cost, float* workspace, int64_t workspace_floats, int32_t select,
+    void* stream) {
+    GCBF_REQUIRE(n_layers >= 1 && n_layers <= GCBF_MAX_LAYERS, "%s: n_layers %d outside [1, %d]", fn, n_layers,
+                 GCBF_MAX_LAYERS);
+    GCBF_REQUIRE(desc && actor_params && infer_blob && agent && goal && ray_table && hits && row_start && row_deg &&
+                     edge_recv && edge_src && counters && action && next_agent && next_hits && next_row_start &&
+                     next_row_deg && next_edge_recv && next_edge_src && next_counters && reward && cost && workspace,
+                 "%s: NULL pointer argument", fn);
+    GCBF_REQUIRE(n_layers == 1 || use_tensor_cores, "%s: n_layers > 1 runs on the tensor-core path only", fn);
+    GCBF_REQUIRE(select == GCBF_STEP_ALL || use_tensor_cores, "%s: partial steps need the tensor-core path", fn);
+    GCBF_REQUIRE(next_row_start != row_start && next_row_deg != row_deg && next_edge_recv != edge_recv &&
+                     next_edge_src != edge_src && next_counters != counters,
+                 "%s: the next graph must not alias the current one (double-buffer the edge lists)", fn);
+    if (int32_t rc = check_graph_desc(desc, fn)) return rc;
+    GCBF_REQUIRE(desc->n_obs == 0 || obstacles, "obstacles is NULL but n_obs > 0");
+    const StepWs W = make_step_ws(desc, n_layers);
+    GCBF_REQUIRE(workspace_floats >= W.total, "workspace too small: %lld < %lld floats", (long long)workspace_floats,
+                 (long long)W.total);
+    const uintptr_t planes = n_layers > 1 ? (uintptr_t)actor_params | (uintptr_t)infer_blob : 0;   // PlaneLayout
+    GCBF_REQUIRE((((uintptr_t)workspace | planes) & 15) == 0, "%s: actor_params/infer_blob/workspace must be 16-byte "
+                                                              "aligned", fn);
+    cudaStream_t st = (cudaStream_t)stream;
+    const int nu = env_nu(desc->env_kind);
+    const GraphRefs g{agent, goal, hits, row_start, row_deg, edge_recv, edge_src, counters};
+    float* z = workspace + W.z;
+    TailArgs tl;
+    tl.z = z;
+    tl.parts = 1;
+    tl.z_cap = desc->n_graphs * desc->n_agents;
+    tl.agent_prev = agent;
+    tl.goal = goal;
+    tl.row_start_prev = row_start;
+    tl.row_deg_prev = row_deg;
+    tl.edge_src_prev = edge_src;
+    tl.action = action;
+    tl.next_agent = next_agent;
+    int32_t flags = 1;   // cast rays
+    if (n_layers == 1) {
+        if (int32_t rc = gnn_infer_impl(desc, nu, actor_params, infer_blob, use_tensor_cores, g, 0, nullptr, workspace,
+                                        st, z, &tl.parts, next_counters, select & 0xF)) return rc;
+        if (!(select & 16)) return 0;
+        tl.bHO = infer_blob + make_infer_layout(nu).bho;
+        // the attention kernel cleared the next edge counter; a partial step without it lets the build clear it
+        if (select & 2) flags |= 4;
+    } else {
+        if (int32_t rc = gnn_forward(desc, nu, n_layers, actor_params, infer_blob, g, 0, nullptr, z, workspace, st))
+            return rc;
+        tl.bHO = actor_params + make_deep_layout(env_ed(desc->env_kind), nu, n_layers).layer[0].b[L_OUT];
+    }
+    return graph_build_impl(desc, nullptr, obstacles, ray_table, next_hits, next_row_start, next_row_deg, next_edge_recv,
+                            next_edge_src, next_counters, flags, tl, reward, cost, stream);
 }
 
 extern "C" __attribute__((visibility("default"))) int32_t gcbf_rollout_step_l(
@@ -613,49 +631,21 @@ extern "C" __attribute__((visibility("default"))) int32_t gcbf_rollout_step_l(
     const int32_t* edge_src, const int32_t* counters, float* action, float* next_agent, float* next_hits,
     int32_t* next_row_start, int32_t* next_row_deg, int32_t* next_edge_recv, int32_t* next_edge_src,
     int32_t* next_counters, float* reward, float* cost, float* workspace, int64_t workspace_floats, void* stream) {
-    GCBF_REQUIRE(n_layers >= 1 && n_layers <= GCBF_MAX_LAYERS, "gcbf_rollout_step_l: n_layers %d outside [1, %d]",
-                 n_layers, GCBF_MAX_LAYERS);
-    if (n_layers == 1)
-        return gcbf_rollout_step_select(desc, actor_params, infer_blob, use_tensor_cores, agent, goal, obstacles,
-                                        ray_table, hits, row_start, row_deg, edge_recv, edge_src, counters, action,
-                                        next_agent, next_hits, next_row_start, next_row_deg, next_edge_recv,
-                                        next_edge_src, next_counters, reward, cost, workspace, workspace_floats,
-                                        GCBF_STEP_ALL, stream);
-    GCBF_REQUIRE(desc && actor_params && infer_blob && agent && goal && ray_table && hits && row_start && row_deg &&
-                     edge_recv && edge_src && counters && action && next_agent && next_hits && next_row_start &&
-                     next_row_deg && next_edge_recv && next_edge_src && next_counters && reward && cost && workspace,
-                 "gcbf_rollout_step_l: NULL pointer argument");
-    GCBF_REQUIRE(use_tensor_cores, "gcbf_rollout_step_l: n_layers > 1 runs on the tensor-core path only");
-    GCBF_REQUIRE(next_row_start != row_start && next_row_deg != row_deg && next_edge_recv != edge_recv &&
-                     next_edge_src != edge_src && next_counters != counters,
-                 "gcbf_rollout_step_l: the next graph must not alias the current one (double-buffer the edge lists)");
-    GCBF_REQUIRE(desc->env_kind >= 0 && desc->env_kind <= 3 && desc->edge_cap > 0, "gcbf_rollout_step_l: bad descriptor");
-    GCBF_REQUIRE(desc->n_obs == 0 || obstacles, "obstacles is NULL but n_obs > 0");
-    const int nu = env_nu(desc->env_kind);
-    const int64_t A = (int64_t)desc->n_graphs * desc->n_agents;
-    const DeepWs W = make_deep_ws(desc->edge_cap, A, n_layers);
-    GCBF_REQUIRE(workspace_floats >= W.total + 8 * A + 8, "workspace too small: %lld < %lld floats",
-                 (long long)workspace_floats, (long long)(W.total + 8 * A + 8));
-    GCBF_REQUIRE((((uintptr_t)workspace | (uintptr_t)actor_params | (uintptr_t)infer_blob) & 15) == 0,
-                 "actor_params/infer_blob/workspace must be 16-byte aligned");
-    cudaStream_t st = (cudaStream_t)stream;
-    const DeepLayout D = make_deep_layout(env_ed(desc->env_kind), nu, n_layers);
-    float* z = workspace + ((W.total + 3) & ~(int64_t)3);    // [1][A][4] output-layer pre-activations
-    if (int32_t rc = gnn_forward(desc, nu, n_layers, actor_params, infer_blob, agent, goal, hits, row_start, row_deg,
-                                 edge_recv, edge_src, counters, 0, nullptr, z, workspace, st)) return rc;
-    TailArgs tl;
-    tl.z = z;
-    tl.parts = 1;
-    tl.z_cap = (int)A;
-    tl.bHO = actor_params + D.layer[0].b[L_OUT];
-    tl.agent_prev = agent;
-    tl.goal = goal;
-    tl.row_start_prev = row_start;
-    tl.row_deg_prev = row_deg;
-    tl.edge_src_prev = edge_src;
-    tl.action = action;
-    tl.next_agent = next_agent;
-    // flags 1: cast rays; the build clears the next edge counter itself
-    return graph_build_impl(desc, nullptr, obstacles, ray_table, next_hits, next_row_start, next_row_deg, next_edge_recv,
-                            next_edge_src, next_counters, 1, tl, reward, cost, stream);
+    return rollout_step("gcbf_rollout_step_l", desc, n_layers, actor_params, infer_blob, use_tensor_cores, agent, goal,
+                        obstacles, ray_table, hits, row_start, row_deg, edge_recv, edge_src, counters, action,
+                        next_agent, next_hits, next_row_start, next_row_deg, next_edge_recv, next_edge_src,
+                        next_counters, reward, cost, workspace, workspace_floats, GCBF_STEP_ALL, stream);
+}
+
+extern "C" __attribute__((visibility("default"))) int32_t gcbf_rollout_step_select(
+    const gcbf_env_desc* desc, const float* actor_params, const float* infer_blob, int32_t use_tensor_cores,
+    const float* agent, const float* goal, const float* obstacles, const float* ray_table, const float* hits,
+    const int32_t* row_start, const int32_t* row_deg, const int32_t* edge_recv, const int32_t* edge_src,
+    const int32_t* counters, float* action, float* next_agent, float* next_hits, int32_t* next_row_start,
+    int32_t* next_row_deg, int32_t* next_edge_recv, int32_t* next_edge_src, int32_t* next_counters, float* reward,
+    float* cost, float* workspace, int64_t workspace_floats, int32_t select, void* stream) {
+    return rollout_step("gcbf_rollout_step_select", desc, 1, actor_params, infer_blob, use_tensor_cores, agent, goal,
+                        obstacles, ray_table, hits, row_start, row_deg, edge_recv, edge_src, counters, action,
+                        next_agent, next_hits, next_row_start, next_row_deg, next_edge_recv, next_edge_src,
+                        next_counters, reward, cost, workspace, workspace_floats, select, stream);
 }

@@ -17,22 +17,21 @@ struct GnnWs {
 };
 inline GnnWs make_ws(int64_t cap, int64_t A) {
     GnnWs w;
-    int64_t o = 0;
-    auto take = [&](int64_t n) { int64_t r = o; o += (n + 7) & ~(int64_t)7; return r; };   // 32-byte slots: 256-bit epilogue stores
-    w.feat = take(cap * FEAT_LD);
-    w.x1 = take(cap * 256);
-    w.x2 = take(cap * 256);
-    w.msg = take(cap * 128);
-    w.g1 = take(cap * 128);
-    w.g2 = take(cap * 128);
-    w.att = take(cap);
-    w.ag = take(A * 128);
-    w.v1 = take(A * 256);
-    w.v2 = take(A * 256);
-    w.v3 = take(A * 128);
-    w.h1 = take(A * 256);
-    w.h2 = take(A * 256);
-    w.total = o;
+    WsSlots S{8};   // 32-byte slots: 256-bit epilogue stores
+    w.feat = S.take(cap * FEAT_LD);
+    w.x1 = S.take(cap * 256);
+    w.x2 = S.take(cap * 256);
+    w.msg = S.take(cap * 128);
+    w.g1 = S.take(cap * 128);
+    w.g2 = S.take(cap * 128);
+    w.att = S.take(cap);
+    w.ag = S.take(A * 128);
+    w.v1 = S.take(A * 256);
+    w.v2 = S.take(A * 256);
+    w.v3 = S.take(A * 128);
+    w.h1 = S.take(A * 256);
+    w.h2 = S.take(A * 256);
+    w.total = S.off;
     return w;
 }
 
@@ -47,27 +46,26 @@ struct InferLayout {
 };
 inline InferLayout make_infer_layout(int out_dim) {
     InferLayout I;
-    int o = 0;
-    auto take = [&](int n) { int r = o; o += (n + 3) & ~3; return r; };
-    I.w23 = take(256 * 128);
-    I.b23 = take(128);
-    I.a23 = take(128);
-    I.c23 = take(4);
-    I.uh = take(256 * 256);
-    I.buh = take(256);
-    I.ho = take(256 * out_dim);
-    I.bho = take(4);
-    I.t_w23 = take(2 * 128 * 256);
-    I.t_a1 = take(2 * 128 * 128);
-    I.t_u1 = take(2 * 256 * 128);
-    I.t_uh = take(2 * 256 * 256);
-    I.q_u12 = take(256 * 128);
-    I.b_u12 = take(128);
-    I.p_w23 = take(2 * 256 * 128);
-    I.p_a1 = take(2 * 128 * 128);
-    I.p_u1 = take(2 * 128 * 256);
-    I.p_uh = take(2 * 256 * 256);
-    I.total = o;
+    WsSlots S{4};
+    I.w23 = S.take(256 * 128);
+    I.b23 = S.take(128);
+    I.a23 = S.take(128);
+    I.c23 = S.take(4);
+    I.uh = S.take(256 * 256);
+    I.buh = S.take(256);
+    I.ho = S.take(256 * out_dim);
+    I.bho = S.take(4);
+    I.t_w23 = S.take(2 * 128 * 256);
+    I.t_a1 = S.take(2 * 128 * 128);
+    I.t_u1 = S.take(2 * 256 * 128);
+    I.t_uh = S.take(2 * 256 * 256);
+    I.q_u12 = S.take(256 * 128);
+    I.b_u12 = S.take(128);
+    I.p_w23 = S.take(2 * 256 * 128);
+    I.p_a1 = S.take(2 * 128 * 128);
+    I.p_u1 = S.take(2 * 128 * 256);
+    I.p_uh = S.take(2 * 256 * 256);
+    I.total = S.off;
     return I;
 }
 

@@ -147,21 +147,20 @@ static RefineWs make_refine_ws(const gcbf_env_desc* d) {
     const int64_t A = (int64_t)d->n_graphs * d->n_agents, cap = d->edge_cap;
     const GnnWs W = make_ws(d->edge_cap, A);
     RefineWs t;
-    int64_t o = 0;
-    auto take = [&](int64_t n) { int64_t r = o; o += (n + 7) & ~(int64_t)7; return r; };   // 32-byte slots
-    t.fw = take(W.total);
-    t.gw = take(W.total);
-    t.h = take(A);
-    t.hn = take(A);
-    t.dhn = take(A);
-    t.ur = take(A * nu);
-    t.xn = take(A * sd);
-    t.d_es = take(A * ed);
-    t.je = take(cap * 8);
-    t.active = take(d->n_graphs);
-    t.upd = take(d->n_graphs);
-    t.rows = take(2);
-    t.total = o;
+    WsSlots S{8};   // 32-byte slots
+    t.fw = S.take(W.total);
+    t.gw = S.take(W.total);
+    t.h = S.take(A);
+    t.hn = S.take(A);
+    t.dhn = S.take(A);
+    t.ur = S.take(A * nu);
+    t.xn = S.take(A * sd);
+    t.d_es = S.take(A * ed);
+    t.je = S.take(cap * 8);
+    t.active = S.take(d->n_graphs);
+    t.upd = S.take(d->n_graphs);
+    t.rows = S.take(2);
+    t.total = S.off;
     return t;
 }
 

@@ -589,26 +589,34 @@ __global__ void dyn_bwd_kernel(const gcbf_env_desc d, const float* __restrict__ 
 }
 
 // ------------------------------------------------------------------------------------ one network backward
+// Built by aggregate initialisation, in this order.
 struct BwdArgs {
     const gcbf_env_desc* d;
+    GraphRefs g;           // the graph of the forward pass
+    float* gw;             // gradient workspace (make_ws layout)
+    float* part;           // PART_FLOATS: per-CTA partials of the weight-gradient reductions (when G is set)
+    int use_tc;            // 1: backward-data GEMMs on the wgmma path
     int out_dim;
     const float* P;        // parameters
-    const float* PT;       // backward-data B operands: tf32 planes (build_planes) or, SIMT, W^T (TransLayout)
+    const float* PT;       // backward-data B operands (prepare_bwd_operands)
     const float* fw;       // forward workspace (saved activations)
-    float* gw;             // gradient workspace (same layout)
     const float* out;      // network output (tanh applied) [A, out_dim]
     const float* d_out;    // upstream gradient wrt the output [A, out_dim]
     const float* roww;     // optional per-agent weights applied to every dW / db contribution
-    float* G;              // parameter gradient (accumulated)
-    const float *agent, *goal, *hits;
-    const int32_t *row_start, *row_deg, *edge_recv, *edge_src, *counters;
+    float* G;              // parameter gradient (accumulated); nullptr: data-only backward
     int clip_all;
     float* d_es;           // optional [A, ED] (written): gradient wrt the agents' edge states, gathered from `je`
     float* je;             // [cap, 8] when d_es is wanted or the per-edge blocks are the result: d out[recv] / d feat_e
-    float* part;           // PART_FLOATS: per-CTA partials of the weight-gradient reductions (when G is set)
-    int use_tc;            // 1: backward-data GEMMs on the wgmma path
     const int32_t* agent_rows = nullptr;   // optional device row count of the agent-row GEMMs (default: every agent)
 };
+
+// Backward-data B operands of a one-layer network: the straight tf32 planes (build_planes) on the tensor-core path,
+// W^T (TransLayout) on the SIMT path.
+static int32_t prepare_bwd_operands(int ed, int out_dim, int use_tc, const float* P, float* PT, cudaStream_t st) {
+    if (use_tc) return build_planes(ed, out_dim, 1, P, PT, st);
+    const ParamLayout L = make_layout(ed, out_dim);
+    return build_transposes(L, make_trans_layout(L), P, PT, st);
+}
 
 // ---- the parameter-gradient kernels followed by the ordered sum of their per-CTA partials
 static int grid_for_part(int grid, int64_t part_floats) {
@@ -633,8 +641,8 @@ static int32_t attn_aggregate_bwd(const BwdArgs& b, int grid, const float* dAG, 
                                   int mask_relu, cudaStream_t st) {
     const int A = b.d->n_graphs * b.d->n_agents;
     grid = grid_for_part(grid, 129);
-    attn_aggregate_bwd_kernel<<<grid, 256, 0, st>>>(A, b.d->edge_cap, dAG, MSG, G2, ATT, a3, b.row_start, b.row_deg,
-                                                    b.roww, dMSG, dG2, da3 ? b.part : nullptr, mask_relu);
+    attn_aggregate_bwd_kernel<<<grid, 256, 0, st>>>(A, b.d->edge_cap, dAG, MSG, G2, ATT, a3, b.g.row_start,
+                                                    b.g.row_deg, b.roww, dMSG, dG2, da3 ? b.part : nullptr, mask_relu);
     count_launch();
     if (int32_t rc = check_launch("attn_aggregate_bwd_kernel")) return rc;
     if (!da3) return 0;
@@ -650,9 +658,9 @@ static int32_t edge_l1_bwd(const BwdArgs& b, const ParamLayout& L, const float* 
         float* dW1 = b.G + L.w[L_MSG0];
         const int grid = grid_for_part(min(max(cap / 64, 1), 4 * nsm), edge_l1_part_floats(ed));   // chunks of 64 edges
         switch (ed) {
-            case 2: edge_l1_bwd_w_kernel<2><<<grid, 256, 0, st>>>(cap, A, b.counters, dY, feat, b.edge_src, b.edge_recv, b.roww, b.part); break;
-            case 4: edge_l1_bwd_w_kernel<4><<<grid, 256, 0, st>>>(cap, A, b.counters, dY, feat, b.edge_src, b.edge_recv, b.roww, b.part); break;
-            default: edge_l1_bwd_w_kernel<6><<<grid, 256, 0, st>>>(cap, A, b.counters, dY, feat, b.edge_src, b.edge_recv, b.roww, b.part); break;
+            case 2: edge_l1_bwd_w_kernel<2><<<grid, 256, 0, st>>>(cap, A, b.g.counters, dY, feat, b.g.edge_src, b.g.edge_recv, b.roww, b.part); break;
+            case 4: edge_l1_bwd_w_kernel<4><<<grid, 256, 0, st>>>(cap, A, b.g.counters, dY, feat, b.g.edge_src, b.g.edge_recv, b.roww, b.part); break;
+            default: edge_l1_bwd_w_kernel<6><<<grid, 256, 0, st>>>(cap, A, b.g.counters, dY, feat, b.g.edge_src, b.g.edge_recv, b.roww, b.part); break;
         }
         count_launch();
         if (int32_t rc = check_launch("edge_l1_bwd_w_kernel")) return rc;
@@ -664,16 +672,16 @@ static int32_t edge_l1_bwd(const BwdArgs& b, const ParamLayout& L, const float* 
     if (!b.je) return 0;
     const int grid = min((cap + 7) / 8, 4 * nsm);
     GCBF_DISPATCH_ENV(d->env_kind, {
-        edge_l1_bwd_x_kernel<KIND><<<grid, 256, 0, st>>>(*d, b.P + L.w[L_MSG0], dY, b.agent, b.goal, b.hits, b.edge_recv,
-                                                         b.edge_src, b.counters, b.clip_all, b.je);
+        edge_l1_bwd_x_kernel<KIND><<<grid, 256, 0, st>>>(*d, b.P + L.w[L_MSG0], dY, b.g.agent, b.g.goal, b.g.hits,
+                                                         b.g.edge_recv, b.g.edge_src, b.g.counters, b.clip_all, b.je);
     });
     count_launch();
     if (int32_t rc = check_launch("edge_l1_bwd_x_kernel")) return rc;
     if (!b.d_es) return 0;
     switch (ed) {
-        case 2: edge_grad_gather_kernel<2><<<(A + 127) / 128, 128, 0, st>>>(A, cap, b.row_start, b.row_deg, b.edge_src, b.je, b.d_es); break;
-        case 4: edge_grad_gather_kernel<4><<<(A + 127) / 128, 128, 0, st>>>(A, cap, b.row_start, b.row_deg, b.edge_src, b.je, b.d_es); break;
-        default: edge_grad_gather_kernel<6><<<(A + 127) / 128, 128, 0, st>>>(A, cap, b.row_start, b.row_deg, b.edge_src, b.je, b.d_es); break;
+        case 2: edge_grad_gather_kernel<2><<<(A + 127) / 128, 128, 0, st>>>(A, cap, b.g.row_start, b.g.row_deg, b.g.edge_src, b.je, b.d_es); break;
+        case 4: edge_grad_gather_kernel<4><<<(A + 127) / 128, 128, 0, st>>>(A, cap, b.g.row_start, b.g.row_deg, b.g.edge_src, b.je, b.d_es); break;
+        default: edge_grad_gather_kernel<6><<<(A + 127) / 128, 128, 0, st>>>(A, cap, b.g.row_start, b.g.row_deg, b.g.edge_src, b.je, b.d_es); break;
     }
     count_launch();
     return check_launch("edge_grad_gather_kernel");
@@ -708,7 +716,7 @@ static int32_t gnn_backward_impl(const BwdArgs& b, cudaStream_t st) {
     const int* boff = b.use_tc ? Q.s : TL.w;
     const int A = d->n_graphs * d->n_agents, cap = d->edge_cap;
     const GnnWs W = make_ws(cap, A);
-    const RowCount re{b.counters, 0, cap};
+    const RowCount re{b.g.counters, 0, cap};
     const RowCount ra{b.agent_rows, A, A};
     const int nsm = sm_count();
     const float* fw = b.fw;
@@ -738,14 +746,14 @@ static int32_t gnn_backward_impl(const BwdArgs& b, cudaStream_t st) {
                           gw + W.msg, gw + W.g2, wgrad ? Gz + L.w[L_GATE] : nullptr, wgrad ? Gz + L.b[L_GATE] : nullptr, 0,
                           st));
     // ---- gate MLP (edge rows; dW weighted by the receiver's weight)
-    WG(dense_bwd_weight(b, fw + W.g1, 128, gw + W.g2, b.G + L.w[L_ATT1], b.G + L.b[L_ATT1], nullptr, b.edge_recv, re, 128, 128, A, st));
+    WG(dense_bwd_weight(b, fw + W.g1, 128, gw + W.g2, b.G + L.w[L_ATT1], b.G + L.b[L_ATT1], nullptr, b.g.edge_recv, re, 128, 128, A, st));
     RC(dense_bwd_data(b, L, boff, L_ATT1, EPI_RELU_MASK, false, gw + W.g2, gw + W.g1, fw + W.g1, re, st));
-    WG(dense_bwd_weight(b, fw + W.msg, 128, gw + W.g1, b.G + L.w[L_ATT0], b.G + L.b[L_ATT0], nullptr, b.edge_recv, re, 128, 128, A, st));
+    WG(dense_bwd_weight(b, fw + W.msg, 128, gw + W.g1, b.G + L.w[L_ATT0], b.G + L.b[L_ATT0], nullptr, b.g.edge_recv, re, 128, 128, A, st));
     RC(dense_bwd_data(b, L, boff, L_ATT0, EPI_NONE, true, gw + W.g1, gw + W.msg, nullptr, re, st));
     // ---- message MLP
-    WG(dense_bwd_weight(b, fw + W.x2, 256, gw + W.msg, b.G + L.w[L_MSGOUT], b.G + L.b[L_MSGOUT], nullptr, b.edge_recv, re, 256, 128, A, st));
+    WG(dense_bwd_weight(b, fw + W.x2, 256, gw + W.msg, b.G + L.w[L_MSGOUT], b.G + L.b[L_MSGOUT], nullptr, b.g.edge_recv, re, 256, 128, A, st));
     RC(dense_bwd_data(b, L, boff, L_MSGOUT, EPI_NONE, false, gw + W.msg, gw + W.x2, nullptr, re, st));
-    WG(dense_bwd_weight(b, fw + W.x1, 256, gw + W.x2, b.G + L.w[L_MSG1], b.G + L.b[L_MSG1], nullptr, b.edge_recv, re, 256, 256, A, st));
+    WG(dense_bwd_weight(b, fw + W.x1, 256, gw + W.x2, b.G + L.w[L_MSG1], b.G + L.b[L_MSG1], nullptr, b.g.edge_recv, re, 256, 256, A, st));
     RC(dense_bwd_data(b, L, boff, L_MSG1, EPI_RELU_MASK, false, gw + W.x2, gw + W.x1, fw + W.x1, re, st));
     // ---- edge layer 1
     RC(edge_l1_bwd(b, L, gw + W.x1, fw + W.feat, wgrad, st));
@@ -770,7 +778,7 @@ static int32_t gnn_backward_folded(const BwdArgs& b, const float* blob, float* G
     const InferLayout I = make_infer_layout(b.out_dim);
     const int A = d->n_graphs * d->n_agents, cap = d->edge_cap;
     const GnnWs W = make_ws(cap, A);
-    const RowCount re{b.counters, 0, cap};
+    const RowCount re{b.g.counters, 0, cap};
     const RowCount ra{nullptr, A, A};
     const int nsm = sm_count();
     const float* fw = b.fw;
@@ -796,11 +804,11 @@ static int32_t gnn_backward_folded(const BwdArgs& b, const float* blob, float* G
     RC(attn_aggregate_bwd(b, min((A + 7) / 8, 6 * nsm), gw + W.ag, fw + W.msg, fw + W.g1, fw + W.att, blob + I.a23,
                           gw + W.msg, gw + W.g1, Gf + I.a23, Gf + I.c23, 1, st));
     // ---- g1 = relu(msg A1 + ba1)
-    RC(tc::launch_gemm_tn_tc(fw + W.msg, 128, gw + W.g1, b.G + L.w[L_ATT0], b.roww, b.edge_recv, re, 128, 128, A, st,
+    RC(tc::launch_gemm_tn_tc(fw + W.msg, 128, gw + W.g1, b.G + L.w[L_ATT0], b.roww, b.g.edge_recv, re, 128, 128, A, st,
                              b.G + L.b[L_ATT0], nullptr, b.part));
     RC(data(EPI_NONE, true, gw + W.g1, I.p_a1, 128, 128, gw + W.msg, nullptr, re));
     // ---- msg = x1 W23 + b23
-    RC(tc::launch_gemm_tn_tc(fw + W.x1, 256, gw + W.msg, Gf + I.w23, b.roww, b.edge_recv, re, 256, 128, A, st, Gf + I.b23,
+    RC(tc::launch_gemm_tn_tc(fw + W.x1, 256, gw + W.msg, Gf + I.w23, b.roww, b.g.edge_recv, re, 256, 128, A, st, Gf + I.b23,
                              nullptr, b.part));
     RC(data(EPI_RELU_MASK, false, gw + W.msg, I.p_w23, 128, 256, gw + W.x1, fw + W.x1, re));
     // ---- edge layer 1
@@ -947,21 +955,20 @@ static QpWs make_qp_ws(const gcbf_env_desc* d) {
     const int64_t A = (int64_t)d->n_graphs * d->n_agents, cap = d->edge_cap;
     const GnnWs W = make_ws(d->edge_cap, A);
     QpWs t;
-    int64_t o = 0;
-    auto take = [&](int64_t n) { int64_t r = o; o += (n + 7) & ~(int64_t)7; return r; };   // 32-byte slots: 256-bit epilogue stores
-    t.ws0 = take(W.total);
-    t.gws = take(W.total);
-    t.pt_cbf = take(make_plane_layout(make_deep_layout(ed, 1, 1), ed).total);   // also holds the SIMT TransLayout
-    t.h = take(A);
-    t.ones = take(A);
-    t.je = take(cap * 8);
-    t.qb = take(A);
-    t.qs = take(A * 4);
-    t.qe = take(cap * 4);
-    t.ur = take(A * 4);
-    t.qsc = take(A);
-    t.rev = take(cap);
-    t.total = o;
+    WsSlots S{8};   // 32-byte slots: 256-bit epilogue stores
+    t.ws0 = S.take(W.total);
+    t.gws = S.take(W.total);
+    t.pt_cbf = S.take(make_plane_layout(make_deep_layout(ed, 1, 1), ed).total);   // also holds the SIMT TransLayout
+    t.h = S.take(A);
+    t.ones = S.take(A);
+    t.je = S.take(cap * 8);
+    t.qb = S.take(A);
+    t.qs = S.take(A * 4);
+    t.qe = S.take(cap * 4);
+    t.ur = S.take(A * 4);
+    t.qsc = S.take(A);
+    t.rev = S.take(cap);
+    t.total = S.off;
     return t;
 }
 
@@ -986,39 +993,39 @@ static TrainWs make_train_ws(const gcbf_env_desc* d) {
     const int64_t A = (int64_t)d->n_graphs * d->n_agents;
     const GnnWs W = make_ws(d->edge_cap, A);
     TrainWs t;
-    int64_t o = 0;
-    auto up8 = [](int64_t n) { return (n + 7) & ~(int64_t)7; };   // 32-byte slots: 256-bit epilogue stores
-    auto take = [&](int64_t n) { int64_t r = o; o += up8(n); return r; };
+    WsSlots S{8};   // 32-byte slots: 256-bit epilogue stores
     auto take_net = [&](int out_dim) {
         const InferLayout I = make_infer_layout(out_dim);
+        WsSlots F{8};   // the folded step's region
+        F.take(I.total);
+        const int64_t gf = F.take(I.t_w23), scr = F.take(UNFOLD_SCRATCH);
         const int64_t simt = make_trans_layout(make_layout(ed, out_dim)).total;
-        const int64_t folded = up8(I.total) + up8(I.t_w23) + UNFOLD_SCRATCH;
         TrainNetWs n;
-        n.pt = take(simt > folded ? simt : folded);
-        n.gf = n.pt + up8(I.total);
-        n.scr = n.gf + up8(I.t_w23);
+        n.pt = S.take(simt > F.off ? simt : F.off);
+        n.gf = n.pt + gf;
+        n.scr = n.pt + scr;
         return n;
     };
-    t.ws0 = take(W.total);
-    t.ws1 = take(W.total);
-    t.ws2 = take(W.total);
-    t.gws = take(W.total);
+    t.ws0 = S.take(W.total);
+    t.ws1 = S.take(W.total);
+    t.ws2 = S.take(W.total);
+    t.gws = S.take(W.total);
     t.net_cbf = take_net(1);
     t.net_act = take_net(nu);
-    t.h = take(A);
-    t.hn = take(A);
-    t.pi = take(A * nu);
-    t.act = take(A * nu);
-    t.xn = take(A * sd);
-    t.d_es = take(A * ed);
-    t.je = take((int64_t)d->edge_cap * 8);
-    t.dh = take(A);
-    t.dhn = take(A);
-    t.da = take(A * nu);
-    t.dpi = take(A * nu);
-    t.lab = take(A);
-    t.part = take(PART_FLOATS);
-    t.total = o;
+    t.h = S.take(A);
+    t.hn = S.take(A);
+    t.pi = S.take(A * nu);
+    t.act = S.take(A * nu);
+    t.xn = S.take(A * sd);
+    t.d_es = S.take(A * ed);
+    t.je = S.take((int64_t)d->edge_cap * 8);
+    t.dh = S.take(A);
+    t.dhn = S.take(A);
+    t.da = S.take(A * nu);
+    t.dpi = S.take(A * nu);
+    t.lab = S.take(A);
+    t.part = S.take(PART_FLOATS);
+    t.total = S.off;
     return t;
 }
 
@@ -1027,10 +1034,7 @@ static TrainWs make_train_ws(const gcbf_env_desc* d) {
 using namespace gcbf;
 
 extern "C" __attribute__((visibility("default"))) int64_t gcbf_train_workspace_floats(const gcbf_env_desc* desc) {
-    if (!desc || desc->edge_cap <= 0 || desc->n_graphs <= 0 || desc->n_agents <= 0 || desc->env_kind < 0 ||
-        desc->env_kind > 3)
-        return -1;
-    return make_train_ws(desc).total;
+    return graph_desc_ok(desc) ? make_train_ws(desc).total : -1;
 }
 
 extern "C" __attribute__((visibility("default"))) int32_t gcbf_mask_counts(const uint8_t* safe_mask,
@@ -1056,8 +1060,7 @@ extern "C" __attribute__((visibility("default"))) int32_t gcbf_train_step(
     GCBF_REQUIRE(desc && hp_host && cbf_params && actor_params && agent && goal && hits && row_start && row_deg &&
                      edge_recv && edge_src && counters && safe_mask && unsafe_mask && u_qp && denoms && grad_cbf &&
                      grad_actor && stats && workspace, "gcbf_train_step: NULL pointer argument");
-    GCBF_REQUIRE(desc->env_kind >= 0 && desc->env_kind <= 3 && desc->edge_cap > 0 && desc->n_graphs > 0 &&
-                     desc->n_agents > 0, "gcbf_train_step: bad descriptor");
+    if (int32_t rc = check_graph_desc(desc, "gcbf_train_step")) return rc;
     const TrainWs TW = make_train_ws(desc);
     GCBF_REQUIRE(workspace_floats >= TW.total, "train workspace too small: %lld < %lld floats",
                  (long long)workspace_floats, (long long)TW.total);
@@ -1101,26 +1104,27 @@ extern "C" __attribute__((visibility("default"))) int32_t gcbf_train_step(
             return (int32_t)e;
         }
     } else {
-        RC(build_transposes(Lc, make_trans_layout(Lc), cbf_params, ws + TW.net_cbf.pt, st));
-        RC(build_transposes(La, make_trans_layout(La), actor_params, ws + TW.net_act.pt, st));
+        RC(prepare_bwd_operands(ed, 1, 0, cbf_params, blob_c, st));
+        RC(prepare_bwd_operands(ed, nu, 0, actor_params, blob_a, st));
     }
     // ---- forward: h = cbf(g), pi = actor(g), x' = f(x, clip(2 pi + u_ref)), h' = cbf(g')
-    auto forward = [&](int out_dim, const float* params, const float* blob, const float* x, int clip_all, float* out,
-                       float* fws) -> int32_t {
+    const GraphRefs g{agent, goal, hits, row_start, row_deg, edge_recv, edge_src, counters};
+    const GraphRefs gn = g.with_agent(ws + TW.xn);
+    auto forward = [&](int out_dim, const float* params, const float* blob, const GraphRefs& gr, int clip_all,
+                       float* out, float* fws) -> int32_t {
         if (use_tc)
-            return gnn_infer_impl(d, out_dim, params, blob, 1, x, goal, hits, row_start, row_deg, edge_recv, edge_src,
-                                  counters, clip_all, out, fws, st, nullptr, nullptr, nullptr, 0xF, 1);
-        return gnn_forward(d, out_dim, 1, params, nullptr, x, goal, hits, row_start, row_deg, edge_recv, edge_src,
-                           counters, clip_all, out, nullptr, fws, st);
+            return gnn_infer_impl(d, out_dim, params, blob, 1, gr, clip_all, out, fws, st, nullptr, nullptr, nullptr,
+                                  0xF, 1);
+        return gnn_forward(d, out_dim, 1, params, nullptr, gr, clip_all, out, nullptr, fws, st);
     };
-    RC(forward(1, cbf_params, blob_c, agent, 0, ws + TW.h, ws + TW.ws0));
-    RC(forward(nu, actor_params, blob_a, agent, 0, ws + TW.pi, ws + TW.ws1));
+    RC(forward(1, cbf_params, blob_c, g, 0, ws + TW.h, ws + TW.ws0));
+    RC(forward(nu, actor_params, blob_a, g, 0, ws + TW.pi, ws + TW.ws1));
     GCBF_DISPATCH_ENV(d->env_kind, {
         act_dyn_kernel<KIND><<<(A + 127) / 128, 128, 0, st>>>(*d, agent, goal, ws + TW.pi, ws + TW.act, ws + TW.xn);
     });
     count_launch();
     RC(check_launch("act_dyn_kernel"));
-    RC(forward(1, cbf_params, blob_c, ws + TW.xn, 1, ws + TW.hn, ws + TW.ws2));
+    RC(forward(1, cbf_params, blob_c, gn, 1, ws + TW.hn, ws + TW.ws2));
     // ---- losses and their derivatives wrt h, h', a
     {
         const int grid = min((A + 255) / 256, 2 * sm_count());
@@ -1134,35 +1138,14 @@ extern "C" __attribute__((visibility("default"))) int32_t gcbf_train_step(
         RC(check_launch("loss_kernel"));
         RC(launch_partial_sum(ws + TW.part, 10, grid, PartSegs().add(stats, 10), st));
     }
-    // ---- backward 1: cbf on g' (dW only from labelled receivers; dX from all) -> d_es
-    BwdArgs b;
-    b.d = d;
-    b.agent = ws + TW.xn;
-    b.goal = goal;
-    b.hits = hits;
-    b.row_start = row_start;
-    b.row_deg = row_deg;
-    b.edge_recv = edge_recv;
-    b.edge_src = edge_src;
-    b.counters = counters;
-    b.gw = ws + TW.gws;
-    b.out_dim = 1;
-    b.P = cbf_params;
-    b.PT = ws + TW.net_cbf.pt;
-    b.fw = ws + TW.ws2;
-    b.out = ws + TW.hn;
-    b.d_out = ws + TW.dhn;
-    b.roww = ws + TW.lab;
-    b.G = grad_cbf;
-    b.clip_all = 1;
-    b.d_es = ws + TW.d_es;
-    b.je = ws + TW.je;
-    b.part = ws + TW.part;
-    b.use_tc = use_tc;
-    auto backward = [&](const float* blob, float* gf) -> int32_t {
+    auto backward = [&](const BwdArgs& b, const float* blob, float* gf) -> int32_t {
         return use_tc ? gnn_backward_folded(b, blob, gf, st) : gnn_backward_impl(b, st);
     };
-    RC(backward(blob_c, gf_c));
+    float* const gw = ws + TW.gws;
+    float* const part = ws + TW.part;
+    // ---- backward 1: cbf on g' (dW only from labelled receivers; dX from all) -> d_es
+    RC(backward({d, gn, gw, part, use_tc, 1, cbf_params, blob_c, ws + TW.ws2, ws + TW.hn, ws + TW.dhn, ws + TW.lab,
+                 grad_cbf, 1, ws + TW.d_es, ws + TW.je}, blob_c, gf_c));
     // ---- through the Euler step / clips into the policy output
     GCBF_DISPATCH_ENV(d->env_kind, {
         dyn_bwd_kernel<KIND><<<(A + 127) / 128, 128, 0, st>>>(*d, agent, goal, ws + TW.act, ws + TW.xn, ws + TW.d_es,
@@ -1171,28 +1154,11 @@ extern "C" __attribute__((visibility("default"))) int32_t gcbf_train_step(
     count_launch();
     RC(check_launch("dyn_bwd_kernel"));
     // ---- backward 2: actor on g
-    b.agent = agent;
-    b.out_dim = nu;
-    b.P = actor_params;
-    b.PT = ws + TW.net_act.pt;
-    b.fw = ws + TW.ws1;
-    b.out = ws + TW.pi;
-    b.d_out = ws + TW.dpi;
-    b.roww = nullptr;
-    b.G = grad_actor;
-    b.clip_all = 0;
-    b.d_es = nullptr;
-    b.je = nullptr;
-    RC(backward(blob_a, gf_a));
+    RC(backward({d, g, gw, part, use_tc, nu, actor_params, blob_a, ws + TW.ws1, ws + TW.pi, ws + TW.dpi, nullptr,
+                 grad_actor, 0, nullptr, nullptr}, blob_a, gf_a));
     // ---- backward 3: cbf on g
-    b.out_dim = 1;
-    b.P = cbf_params;
-    b.PT = ws + TW.net_cbf.pt;
-    b.fw = ws + TW.ws0;
-    b.out = ws + TW.h;
-    b.d_out = ws + TW.dh;
-    b.G = grad_cbf;
-    RC(backward(blob_c, gf_c));
+    RC(backward({d, g, gw, part, use_tc, 1, cbf_params, blob_c, ws + TW.ws0, ws + TW.h, ws + TW.dh, nullptr, grad_cbf, 0,
+                 nullptr, nullptr}, blob_c, gf_c));
     if (use_tc) {
         SmallJobList JT, JU;      // both networks share the two un-fold launches
         unfold_jobs(ed, 1, cbf_params, blob_c, gf_c, grad_cbf, ws + TW.net_cbf.scr, JT, JU);
@@ -1242,16 +1208,13 @@ extern "C" __attribute__((visibility("default"))) int32_t gcbf_polyak(float* tgt
 
 // ------------------------------------------------------------------------------------ QP action labels
 extern "C" __attribute__((visibility("default"))) int64_t gcbf_qp_workspace_floats(const gcbf_env_desc* desc) {
-    if (!desc || desc->edge_cap <= 0 || desc->n_graphs <= 0 || desc->n_agents <= 0 || desc->env_kind < 0 ||
-        desc->env_kind > 3)
-        return -1;
-    return make_qp_ws(desc).total;
+    return graph_desc_ok(desc) ? make_qp_ws(desc).total : -1;
 }
 
 extern "C" __attribute__((visibility("default"))) int32_t gcbf_qp_workspace_layout(const gcbf_env_desc* desc,
                                                                                    int64_t* offsets8_host) {
-    GCBF_REQUIRE(desc && offsets8_host && desc->edge_cap > 0 && desc->n_graphs > 0 && desc->n_agents > 0 &&
-                     desc->env_kind >= 0 && desc->env_kind <= 3, "gcbf_qp_workspace_layout: bad argument");
+    GCBF_REQUIRE(offsets8_host, "gcbf_qp_workspace_layout: bad argument");
+    if (int32_t rc = check_graph_desc(desc, "gcbf_qp_workspace_layout")) return rc;
     const QpWs Q = make_qp_ws(desc);
     const int64_t o[8] = {Q.h, Q.je, Q.qb, Q.qs, Q.qe, Q.ur, Q.qsc, Q.rev};
     for (int i = 0; i < 8; ++i) offsets8_host[i] = o[i];
@@ -1265,8 +1228,7 @@ extern "C" __attribute__((visibility("default"))) int32_t gcbf_qp_labels(
     float* aux, int32_t* iters, float* workspace, int64_t workspace_floats, void* stream) {
     GCBF_REQUIRE(desc && cbf_params && agent && goal && hits && row_start && row_deg && edge_recv && edge_src &&
                      counters && u_qp && workspace, "gcbf_qp_labels: NULL pointer argument");
-    GCBF_REQUIRE(desc->env_kind >= 0 && desc->env_kind <= 3 && desc->edge_cap > 0 && desc->n_graphs > 0 &&
-                     desc->n_agents > 0, "gcbf_qp_labels: bad descriptor");
+    if (int32_t rc = check_graph_desc(desc, "gcbf_qp_labels")) return rc;
     GCBF_REQUIRE(desc->n_agents <= QP_MAX_AGENTS, "gcbf_qp_labels: n_agents %d > %d not supported", desc->n_agents,
                  QP_MAX_AGENTS);
     GCBF_REQUIRE(max_iter > 0 && tol >= 0.f, "gcbf_qp_labels: bad solver settings");
@@ -1278,44 +1240,20 @@ extern "C" __attribute__((visibility("default"))) int32_t gcbf_qp_labels(
     const gcbf_env_desc* d = desc;
     const int ed = env_ed(d->env_kind), nu = env_nu(d->env_kind);
     const int A = d->n_graphs * d->n_agents, N = d->n_agents;
-    const ParamLayout Lc = make_layout(ed, 1);
     float* ws = workspace;
+    const GraphRefs g{agent, goal, hits, row_start, row_deg, edge_recv, edge_src, counters};
     int32_t rc;
 #define RC(x) do { if ((rc = (x))) return rc; } while (0)
-    if (use_tensor_cores) RC(build_planes(ed, 1, 1, cbf_params, ws + Q.pt_cbf, st));
-    else RC(build_transposes(Lc, make_trans_layout(Lc), cbf_params, ws + Q.pt_cbf, st));
+    RC(prepare_bwd_operands(ed, 1, use_tensor_cores, cbf_params, ws + Q.pt_cbf, st));
     // h = cbf(add_edge_feats(graph, x)): every edge feature norm-clipped (gcbf_plus.py:310-316)
-    RC(gnn_forward(d, 1, 1, cbf_params, use_tensor_cores ? ws + Q.pt_cbf : nullptr, agent, goal, hits, row_start, row_deg,
-                   edge_recv, edge_src, counters, 1, ws + Q.h, nullptr, ws + Q.ws0, st));
+    RC(gnn_forward(d, 1, 1, cbf_params, use_tensor_cores ? ws + Q.pt_cbf : nullptr, g, 1, ws + Q.h, nullptr, ws + Q.ws0,
+                   st));
     fill_kernel<<<min((A + 255) / 256, 2 * sm_count()), 256, 0, st>>>(ws + Q.ones, A, 1.f);
     count_launch();
     RC(check_launch("fill_kernel"));
     // Jacobian: data-only backward with upstream 1, kept per edge
-    BwdArgs b;
-    b.d = d;
-    b.out_dim = 1;
-    b.P = cbf_params;
-    b.PT = ws + Q.pt_cbf;
-    b.fw = ws + Q.ws0;
-    b.gw = ws + Q.gws;
-    b.out = ws + Q.h;
-    b.d_out = ws + Q.ones;
-    b.roww = nullptr;
-    b.G = nullptr;
-    b.agent = agent;
-    b.goal = goal;
-    b.hits = hits;
-    b.row_start = row_start;
-    b.row_deg = row_deg;
-    b.edge_recv = edge_recv;
-    b.edge_src = edge_src;
-    b.counters = counters;
-    b.clip_all = 1;
-    b.d_es = nullptr;
-    b.je = ws + Q.je;
-    b.part = nullptr;
-    b.use_tc = use_tensor_cores;
-    RC(gnn_backward_impl(b, st));
+    RC(gnn_backward_impl({d, g, ws + Q.gws, nullptr, use_tensor_cores, 1, cbf_params, ws + Q.pt_cbf, ws + Q.ws0, ws + Q.h,
+                          ws + Q.ones, nullptr, nullptr, 1, nullptr, ws + Q.je}, st));
     int32_t* rev = reinterpret_cast<int32_t*>(ws + Q.rev);
     GCBF_DISPATCH_ENV(d->env_kind, {
         qp_assemble_kernel<KIND><<<(A + 127) / 128, 128, 0, st>>>(*d, alpha, agent, goal, ws + Q.h, ws + Q.je, row_start,
@@ -1361,17 +1299,11 @@ extern "C" __attribute__((visibility("default"))) int32_t gcbf_refine_prepare(in
     GCBF_REQUIRE(cbf_params && prepared && (edge_dim == 2 || edge_dim == 4 || edge_dim == 6),
                  "gcbf_refine_prepare: bad argument");
     GCBF_REQUIRE((((uintptr_t)cbf_params | (uintptr_t)prepared) & 15) == 0, "buffers must be 16-byte aligned");
-    const ParamLayout Lc = make_layout(edge_dim, 1);
-    cudaStream_t st = (cudaStream_t)stream;
-    if (use_tensor_cores) return build_planes(edge_dim, 1, 1, cbf_params, prepared, st);
-    return build_transposes(Lc, make_trans_layout(Lc), cbf_params, prepared, st);
+    return prepare_bwd_operands(edge_dim, 1, use_tensor_cores, cbf_params, prepared, (cudaStream_t)stream);
 }
 
 extern "C" __attribute__((visibility("default"))) int64_t gcbf_refine_workspace_floats(const gcbf_env_desc* desc) {
-    if (!desc || desc->edge_cap <= 0 || desc->n_graphs <= 0 || desc->n_agents <= 0 || desc->env_kind < 0 ||
-        desc->env_kind > 3)
-        return -1;
-    return make_refine_ws(desc).total;
+    return graph_desc_ok(desc) ? make_refine_ws(desc).total : -1;
 }
 
 extern "C" __attribute__((visibility("default"))) int32_t gcbf_refine_actions(
@@ -1382,8 +1314,8 @@ extern "C" __attribute__((visibility("default"))) int32_t gcbf_refine_actions(
     int64_t workspace_floats, void* stream) {
     GCBF_REQUIRE(desc && cbf_params && cbf_prepared && pi && agent && goal && hits && row_start && row_deg &&
                      edge_recv && edge_src && counters && action && workspace, "gcbf_refine_actions: NULL pointer argument");
-    GCBF_REQUIRE(desc->env_kind >= 0 && desc->env_kind <= 3 && desc->edge_cap > 0 && desc->n_graphs > 0 &&
-                     desc->n_agents > 0 && desc->dt > 0.f, "gcbf_refine_actions: bad descriptor");
+    if (int32_t rc = check_graph_desc(desc, "gcbf_refine_actions")) return rc;
+    GCBF_REQUIRE(desc->dt > 0.f, "gcbf_refine_actions: bad descriptor (dt %g)", (double)desc->dt);
     GCBF_REQUIRE(max_iter > 0 && isfinite(lr) && isfinite(alpha), "gcbf_refine_actions: bad settings (max_iter %d)",
                  max_iter);
     const RefineWs R = make_refine_ws(desc);
@@ -1403,19 +1335,24 @@ extern "C" __attribute__((visibility("default"))) int32_t gcbf_refine_actions(
     const float* PT = cbf_prepared;
     int32_t rc;
 #define RC(x) do { if ((rc = (x))) return rc; } while (0)
-    auto forward = [&](const float* x, int clip_all, const int32_t* cnt, const int32_t* arows, float* out) -> int32_t {
-        return gnn_forward(d, 1, 1, cbf_params, use_tensor_cores ? PT : nullptr, x, goal, hits, row_start, row_deg,
-                           edge_recv, edge_src, cnt, clip_all, out, nullptr, ws + R.fw, st, arows);
+    // g: the graph; gn: its edges over the next states x'; gr: the same with the refinement steps' device edge count
+    const GraphRefs g{agent, goal, hits, row_start, row_deg, edge_recv, edge_src, counters};
+    const GraphRefs gn = g.with_agent(ws + R.xn);
+    GraphRefs gr = gn;
+    gr.counters = rows;
+    auto forward = [&](const GraphRefs& on, int clip_all, const int32_t* arows, float* out) -> int32_t {
+        return gnn_forward(d, 1, 1, cbf_params, use_tensor_cores ? PT : nullptr, on, clip_all, out, nullptr, ws + R.fw,
+                           st, arows);
     };
     // 1. h = cbf(g) on the graph's own edge features
-    RC(forward(agent, 0, counters, nullptr, ws + R.h));
+    RC(forward(g, 0, nullptr, ws + R.h));
     // 2. h(g'(u_ref)), every edge feature recomputed and norm-clipped (forward_graph)
     GCBF_DISPATCH_ENV(d->env_kind, {
         refine_next_state_kernel<KIND><<<blocks, 128, 0, st>>>(*d, nullptr, agent, goal, nullptr, ws + R.ur, ws + R.xn);
     });
     count_launch();
     RC(check_launch("refine_next_state_kernel"));
-    RC(forward(ws + R.xn, 1, counters, nullptr, ws + R.hn));
+    RC(forward(gn, 1, nullptr, ws + R.hn));
     // 3. per-agent selection of the starting action; every graph active
     if (nu == 2)
         refine_init_kernel<2><<<blocks, 128, 0, st>>>(G, A, alpha, d->dt, ws + R.h, ws + R.hn, ws + R.ur, pi, counters,
@@ -1427,38 +1364,15 @@ extern "C" __attribute__((visibility("default"))) int32_t gcbf_refine_actions(
     RC(check_launch("refine_init_kernel"));
     // 4. the refinement steps: data-only backward of h' into the edge-state gradient of x' (same as the QP labels'
     //    Jacobian pass, gathered per agent), then the chain into the action
-    BwdArgs b;
-    b.d = d;
-    b.out_dim = 1;
-    b.P = cbf_params;
-    b.PT = PT;
-    b.fw = ws + R.fw;
-    b.gw = ws + R.gw;
-    b.out = ws + R.hn;
-    b.d_out = ws + R.dhn;
-    b.roww = nullptr;
-    b.G = nullptr;
-    b.agent = ws + R.xn;
-    b.goal = goal;
-    b.hits = hits;
-    b.row_start = row_start;
-    b.row_deg = row_deg;
-    b.edge_recv = edge_recv;
-    b.edge_src = edge_src;
-    b.counters = rows;
-    b.agent_rows = rows + 1;
-    b.clip_all = 1;
-    b.d_es = ws + R.d_es;
-    b.je = ws + R.je;
-    b.part = nullptr;
-    b.use_tc = use_tensor_cores;
+    const BwdArgs b{d, gr, ws + R.gw, nullptr, use_tensor_cores, 1, cbf_params, PT, ws + R.fw, ws + R.hn, ws + R.dhn,
+                    nullptr, nullptr, 1, ws + R.d_es, ws + R.je, rows + 1};
     for (int it = 0; it < max_iter; ++it) {
         GCBF_DISPATCH_ENV(d->env_kind, {
             refine_next_state_kernel<KIND><<<blocks, 128, 0, st>>>(*d, rows, agent, goal, action, nullptr, ws + R.xn);
         });
         count_launch();
         RC(check_launch("refine_next_state_kernel"));
-        RC(forward(ws + R.xn, 1, rows, rows + 1, ws + R.hn));
+        RC(forward(gr, 1, rows + 1, ws + R.hn));
         refine_value_kernel<<<G, REFINE_VALUE_THREADS, 0, st>>>(N, env_sd(d->env_kind), alpha, d->dt, it, max_iter,
                                                                 ws + R.h, ws + R.hn, ws + R.xn, ws + R.dhn, active,
                                                                 upd, value, iters);
