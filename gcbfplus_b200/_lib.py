@@ -88,6 +88,8 @@ _SIGNATURES = {
     "gcbf_qp_workspace_layout": (C.c_int32, [C.POINTER(EnvDesc), C.POINTER(C.c_int64)]),
     "gcbf_qp_labels": (C.c_int32, [C.POINTER(EnvDesc), C.c_float, C.c_int32, C.c_int32, C.c_float] + [_P] * 13 +
                        [C.c_int64, _P]),
+    "gcbf_qp_filter": (C.c_int32, [C.POINTER(EnvDesc), C.c_float, C.c_int32, C.c_int32, C.c_float] + [_P] * 14 +
+                       [C.c_int64, _P]),
     "gcbf_refine_prepare": (C.c_int32, [C.c_int32, C.c_int32, _P, _P, _P]),
     "gcbf_refine_workspace_floats": (C.c_int64, [C.POINTER(EnvDesc)]),
     "gcbf_refine_actions": (C.c_int32, [C.POINTER(EnvDesc), C.c_float, C.c_float, C.c_int32, C.c_int32] + [_P] * 15 +

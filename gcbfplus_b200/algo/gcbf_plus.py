@@ -19,6 +19,7 @@ from .nets import GnnRunner
 from .params import NetParams
 from .refine import (REFINE_LR, REFINE_MAX_ITER, launch_refine, planes_buffer, prepare_planes, refine_workspace,
                      require_one_layer_refine)
+from .train import QP_MAX_ITER, QP_TOL, qp_labels
 
 
 class GCBFPlus(MultiAgentController):
@@ -142,13 +143,26 @@ class GCBFPlus(MultiAgentController):
         (the device solver has its own iteration cap / tolerance, algo/train.py)."""
         if relax_penalty != 1e3:
             raise NotImplementedError("relax_penalty is compiled in (1e3, gcbf_plus.py:302)")
-        from .train import qp_labels
         u, aux, _ = qp_labels(self, graph, params=cbf_params or self.cbf_params, with_aux=True)
         return u, aux[..., 1]
 
+    def safety_filter(self, graph: SwarmGraph, u_nom: Optional[torch.Tensor] = None, *,
+                      cbf_params: Optional[NetParams] = None, max_iter: int = QP_MAX_ITER, tol: float = QP_TOL,
+                      return_info: bool = False):
+        """The learned CBF as a QP safety filter, for every graph of the batch: the action closest to the nominal
+        u_nom [G, N, nu] (default u_ref: then this is get_qp_action) such that the CBF condition
+        Lf_h + Lg_h u + 0.1 alpha h >= 0 holds, relaxed by r >= 0 at cost 1000 r + 5 r^2 where no action in the u_lim
+        box satisfies it.  cbf_params defaults to the CBF itself (not the target network); alpha is self.alpha.
+        Returns u [G, N, nu]; with return_info also (r [G, N], iters [G]): a graph whose count reaches max_iter stopped
+        at the cap and its action is the capped iterate."""
+        u, aux, iters = qp_labels(self, graph, params=cbf_params or self.cbf_params, with_aux=True,
+                                  max_iter=max_iter, tol=tol, u_nom=u_nom)
+        if return_info:
+            return u, aux[..., 1], iters
+        return u
+
     def get_b_u_qp(self, b_graph: SwarmGraph, params: Optional[NetParams] = None) -> torch.Tensor:
         """gcbf_plus.py:193-196."""
-        from .train import qp_labels
         return qp_labels(self, b_graph, params=params or self.cbf_tgt_params)
 
     def update(self, rollout, step: int) -> dict:

@@ -355,13 +355,16 @@ QP_TOL = 1e-5           # projected dual-gradient residual
 
 
 def qp_labels(algo, graph: SwarmGraph, params=None, with_aux: bool = False, max_iter: int = QP_MAX_ITER,
-              tol: float = QP_TOL, with_iters: bool = False):
+              tol: float = QP_TOL, with_iters: bool = False, u_nom: Optional[torch.Tensor] = None):
     """get_qp_action vmapped over the graphs of `graph` (gcbf_plus.py:193-196, 299-352): u_qp [G, N, nu];
     with_aux also returns (lam, r) [G, N, 2] and the iteration counts [G]; with_iters returns (u_qp, iters).
-    A graph whose count equals max_iter stopped at the cap (its label is the capped iterate)."""
+    A graph whose count equals max_iter stopped at the cap (its label is the capped iterate).
+    u_nom [G, N, nu]: solve the same QP with this nominal action in place of u_ref (gcbf_qp_filter, the safety filter
+    of GCBFPlus.safety_filter)."""
     env = algo._env
     lib = env.lib
-    require_one_layer((params or algo.cbf_tgt_params).n_layers, "the CBF-QP labels")
+    require_one_layer((params or algo.cbf_tgt_params).n_layers,
+                      "the CBF-QP labels" if u_nom is None else "the CBF-QP safety filter")
     G, N = graph.n_graphs, env.num_agents
     d = env.desc(G, 0, edge_cap=graph.edge_recv.numel())
     cache = algo.__dict__.setdefault("_qp_ws", {})
@@ -378,12 +381,17 @@ def qp_labels(algo, graph: SwarmGraph, params=None, with_aux: bool = False, max_
     u_qp = torch.empty(G, N, env.action_dim, dtype=torch.float32, device=env.device)
     aux = torch.empty(G, N, 2, dtype=torch.float32, device=env.device) if with_aux else None
     iters = torch.empty(G, dtype=torch.int32, device=env.device) if (with_aux or with_iters) else None
-    rc = lib.gcbf_qp_labels(C.byref(d), float(algo.alpha), 1 if _lib.USE_TC else 0, int(max_iter), float(tol),
-                            _lib.ptr(p.flat), _lib.ptr(graph.agent), _lib.ptr(graph.goal), _lib.ptr(graph.hits),
-                            _lib.ptr(graph.row_start), _lib.ptr(graph.row_deg), _lib.ptr(graph.edge_recv),
-                            _lib.ptr(graph.edge_src), _lib.ptr(graph.counters), _lib.ptr(u_qp), _lib.ptr(aux),
-                            _lib.ptr(iters), _lib.ptr(ws), ws.numel(), env._stream())
-    _lib.check(rc, "gcbf_qp_labels")
+    head = (C.byref(d), float(algo.alpha), 1 if _lib.USE_TC else 0, int(max_iter), float(tol), _lib.ptr(p.flat),
+            _lib.ptr(graph.agent), _lib.ptr(graph.goal), _lib.ptr(graph.hits), _lib.ptr(graph.row_start),
+            _lib.ptr(graph.row_deg), _lib.ptr(graph.edge_recv), _lib.ptr(graph.edge_src), _lib.ptr(graph.counters))
+    tail = (_lib.ptr(u_qp), _lib.ptr(aux), _lib.ptr(iters), _lib.ptr(ws), ws.numel(), env._stream())
+    if u_nom is None:
+        _lib.check(lib.gcbf_qp_labels(*head, *tail), "gcbf_qp_labels")
+    else:
+        if tuple(u_nom.shape) != tuple(u_qp.shape):
+            raise ValueError(f"u_nom must have shape {tuple(u_qp.shape)}, got {tuple(u_nom.shape)}")
+        u_nom = u_nom.to(device=env.device, dtype=torch.float32).contiguous()
+        _lib.check(lib.gcbf_qp_filter(*head, _lib.ptr(u_nom), *tail), "gcbf_qp_filter")
     if with_aux:
         return u_qp, aux, iters & 0x3FFFFFFF      # bit 30 flags the global-memory fallback of dense graphs
     if with_iters:

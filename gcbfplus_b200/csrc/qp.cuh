@@ -3,6 +3,7 @@
 //
 // Per graph with N agents, x = [u | r]:
 //     min 1/2 |u|^2 - u_ref.u + 5 |r|^2 + 1000 sum r   s.t.  -Lg_h u - r <= Lf_h + 0.1 alpha h,  |u| <= u_lim,  r >= 0
+// The safety filter (gcbf_qp_filter) solves the same QP with a given nominal action u_nom in place of u_ref.
 // The reference hands the dense [N, N nu] problem to JaxProxQP.  Here:
 //   * h(x) is a ONE-layer GNN, so row i of dh/dx is non-zero only at i and at i's agent neighbours: the
 //     Jacobian is one data-only backward pass with upstream 1 (every receiver's gradient stays on its own
@@ -25,15 +26,16 @@ constexpr int QP_MAX_AGENTS = 2048;
 
 // Thread per agent i: row i of the QP.  JE[e][0..ED) = d h_i / d feat_e (feat = es_recv - es_sender), so
 // d h_i / d es_i = +sum_e JE[e] and d h_i / d es_j = -JE[e] for the agent edge j -> i.
-//   QB[i] = Lf_h_i + 0.1 alpha h_i     QS[i][c] = Lg_h[i, i, c]     QE[e][c] = Lg_h[i, j, c]     UR[i] = u_ref_i
+//   QB[i] = Lf_h_i + 0.1 alpha h_i     QS[i][c] = Lg_h[i, i, c]     QE[e][c] = Lg_h[i, j, c]
+//   UR[i] = the nominal action: u_nom_i ([A, NU]) where u_nom is given, u_ref_i otherwise
 //   REV[e] = index of the mirror edge i -> j in row j (or -1)        QSC[i] = row scale 1 / sqrt(|row|^2 + 0.1)
 template <int KIND>
 __global__ void __launch_bounds__(128)
 qp_assemble_kernel(const gcbf_env_desc d, const float alpha, const float* __restrict__ agent,
                    const float* __restrict__ goal, const float* __restrict__ h, const float* __restrict__ JE,
                    const int32_t* __restrict__ row_start, const int32_t* __restrict__ row_deg,
-                   const int32_t* __restrict__ edge_src, float* __restrict__ QB, float* __restrict__ QS,
-                   float* __restrict__ QE, float* __restrict__ UR, float* __restrict__ QSC,
+                   const int32_t* __restrict__ edge_src, const float* __restrict__ u_nom, float* __restrict__ QB,
+                   float* __restrict__ QS, float* __restrict__ QE, float* __restrict__ UR, float* __restrict__ QSC,
                    int32_t* __restrict__ REV) {
     using T = EnvTraits<KIND>;
     constexpr int SD = T::SD, NU = T::NU, ED = T::ED;
@@ -89,7 +91,12 @@ qp_assemble_kernel(const gcbf_env_desc d, const float alpha, const float* __rest
     float lf, lg[NU], ur[NU];
     qp_lie_terms<KIND>(d, xi, ci, &lf, lg);
     lf_sum += lf;
-    u_ref_dev<KIND>(d, xi, gl, ur);
+    if (u_nom) {
+#pragma unroll
+        for (int c = 0; c < NU; ++c) ur[c] = u_nom[(size_t)i * NU + c];
+    } else {
+        u_ref_dev<KIND>(d, xi, gl, ur);
+    }
 #pragma unroll
     for (int c = 0; c < NU; ++c) {
         QS[(size_t)i * 4 + c] = lg[c];

@@ -1221,17 +1221,18 @@ extern "C" __attribute__((visibility("default"))) int32_t gcbf_qp_workspace_layo
     return 0;
 }
 
-extern "C" __attribute__((visibility("default"))) int32_t gcbf_qp_labels(
-    const gcbf_env_desc* desc, float alpha, int32_t use_tensor_cores, int32_t max_iter, float tol,
-    const float* cbf_params, const float* agent, const float* goal, const float* hits, const int32_t* row_start,
-    const int32_t* row_deg, const int32_t* edge_recv, const int32_t* edge_src, const int32_t* counters, float* u_qp,
-    float* aux, int32_t* iters, float* workspace, int64_t workspace_floats, void* stream) {
+// The QP of the labels with the nominal action u_nom in place of u_ref (u_nom == NULL: u_ref, the labels themselves).
+static int32_t qp_solve(const char* name, const gcbf_env_desc* desc, float alpha, int32_t use_tensor_cores,
+                        int32_t max_iter, float tol, const float* cbf_params, const float* agent, const float* goal,
+                        const float* hits, const int32_t* row_start, const int32_t* row_deg, const int32_t* edge_recv,
+                        const int32_t* edge_src, const int32_t* counters, const float* u_nom, float* u_qp, float* aux,
+                        int32_t* iters, float* workspace, int64_t workspace_floats, void* stream) {
     GCBF_REQUIRE(desc && cbf_params && agent && goal && hits && row_start && row_deg && edge_recv && edge_src &&
-                     counters && u_qp && workspace, "gcbf_qp_labels: NULL pointer argument");
-    if (int32_t rc = check_graph_desc(desc, "gcbf_qp_labels")) return rc;
-    GCBF_REQUIRE(desc->n_agents <= QP_MAX_AGENTS, "gcbf_qp_labels: n_agents %d > %d not supported", desc->n_agents,
+                     counters && u_qp && workspace, "%s: NULL pointer argument", name);
+    if (int32_t rc = check_graph_desc(desc, name)) return rc;
+    GCBF_REQUIRE(desc->n_agents <= QP_MAX_AGENTS, "%s: n_agents %d > %d not supported", name, desc->n_agents,
                  QP_MAX_AGENTS);
-    GCBF_REQUIRE(max_iter > 0 && tol >= 0.f, "gcbf_qp_labels: bad solver settings");
+    GCBF_REQUIRE(max_iter > 0 && tol >= 0.f, "%s: bad solver settings", name);
     const QpWs Q = make_qp_ws(desc);
     GCBF_REQUIRE(workspace_floats >= Q.total, "qp workspace too small: %lld < %lld floats", (long long)workspace_floats,
                  (long long)Q.total);
@@ -1257,8 +1258,8 @@ extern "C" __attribute__((visibility("default"))) int32_t gcbf_qp_labels(
     int32_t* rev = reinterpret_cast<int32_t*>(ws + Q.rev);
     GCBF_DISPATCH_ENV(d->env_kind, {
         qp_assemble_kernel<KIND><<<(A + 127) / 128, 128, 0, st>>>(*d, alpha, agent, goal, ws + Q.h, ws + Q.je, row_start,
-                                                                  row_deg, edge_src, ws + Q.qb, ws + Q.qs, ws + Q.qe,
-                                                                  ws + Q.ur, ws + Q.qsc, rev);
+                                                                  row_deg, edge_src, u_nom, ws + Q.qb, ws + Q.qs,
+                                                                  ws + Q.qe, ws + Q.ur, ws + Q.qsc, rev);
     });
     count_launch();
     RC(check_launch("qp_assemble_kernel"));
@@ -1290,6 +1291,27 @@ extern "C" __attribute__((visibility("default"))) int32_t gcbf_qp_labels(
     RC(check_launch("qp_solve_kernel"));
 #undef RC
     return 0;
+}
+
+extern "C" __attribute__((visibility("default"))) int32_t gcbf_qp_labels(
+    const gcbf_env_desc* desc, float alpha, int32_t use_tensor_cores, int32_t max_iter, float tol,
+    const float* cbf_params, const float* agent, const float* goal, const float* hits, const int32_t* row_start,
+    const int32_t* row_deg, const int32_t* edge_recv, const int32_t* edge_src, const int32_t* counters, float* u_qp,
+    float* aux, int32_t* iters, float* workspace, int64_t workspace_floats, void* stream) {
+    return qp_solve("gcbf_qp_labels", desc, alpha, use_tensor_cores, max_iter, tol, cbf_params, agent, goal, hits,
+                    row_start, row_deg, edge_recv, edge_src, counters, nullptr, u_qp, aux, iters, workspace,
+                    workspace_floats, stream);
+}
+
+extern "C" __attribute__((visibility("default"))) int32_t gcbf_qp_filter(
+    const gcbf_env_desc* desc, float alpha, int32_t use_tensor_cores, int32_t max_iter, float tol,
+    const float* cbf_params, const float* agent, const float* goal, const float* hits, const int32_t* row_start,
+    const int32_t* row_deg, const int32_t* edge_recv, const int32_t* edge_src, const int32_t* counters,
+    const float* u_nom, float* u, float* aux, int32_t* iters, float* workspace, int64_t workspace_floats,
+    void* stream) {
+    return qp_solve("gcbf_qp_filter", desc, alpha, use_tensor_cores, max_iter, tol, cbf_params, agent, goal, hits,
+                    row_start, row_deg, edge_recv, edge_src, counters, u_nom, u, aux, iters, workspace,
+                    workspace_floats, stream);
 }
 
 // ------------------------------------------------------------------------------------ online policy refinement

@@ -13,6 +13,10 @@ env.step with the QP action as input, and the graph build of the next state.
 The `actor_refine` policy (GCBF+ with online policy refinement, algo/refine.py) runs on the same path: per step the
 policy forward, the refinement of its action against the CBF (gcbf_refine_actions), env.step with the refined action as
 input, and the graph build of the next state.
+The `actor_qp` and `u_ref_qp` policies (the learned CBF as a QP safety filter, GCBFPlus.safety_filter) run on the same
+path: per step the policy forward and its action 2 pi + u_ref (actor_qp) or u_ref (u_ref_qp) as the nominal, the CBF-QP
+nearest to it (gcbf_qp_filter), env.step with the filtered action as input, and the canonical graph build of the next
+state.
 """
 from __future__ import annotations
 
@@ -25,10 +29,14 @@ import torch
 from .. import _lib
 from ..algo.cbf_qp import BASELINES, iter_stats
 from ..algo.params import NetParams
-from ..algo.refine import (REFINE_LR, REFINE_MAX_ITER, launch_refine, planes_buffer, prepare_planes,
+from ..algo.refine import (CAPPED_BIT, REFINE_LR, REFINE_MAX_ITER, launch_refine, planes_buffer, prepare_planes,
                            refine_workspace, require_one_layer_refine)
+from ..algo.train import QP_MAX_ITER, QP_TOL, require_one_layer
 from ..utils.graph import SwarmGraph
 from .data import Rollout
+
+#: the CBF-QP safety-filter policies: the nominal action of each, filtered by the learned CBF
+QP_FILTER_POLICIES = ("actor_qp", "u_ref_qp")
 
 
 class _Chain:
@@ -62,13 +70,23 @@ class _Chain:
             # refinement workspace and the per-step iteration record of every graph
             self.refine_ws = refine_workspace(env, self.desc)
             self.refine_iters = torch.zeros(eng.T, E, dtype=i32, device=dev)
+        if eng.policy in QP_FILTER_POLICIES:
+            # QP workspace and the per-step record: iterations per graph, nominal actions, (lam, r) per agent
+            n_qp = env.lib.gcbf_qp_workspace_floats(C.byref(self.desc))
+            if n_qp <= 0:
+                raise RuntimeError("gcbf_qp_workspace_floats: bad descriptor")
+            self.qp_ws = torch.empty(int(n_qp), dtype=f32, device=dev)
+            self.qp_iters = torch.zeros(eng.T, E, dtype=i32, device=dev)
+            self.qp_nominal = torch.zeros(eng.T, E, N, nu, dtype=f32, device=dev)
+            self.qp_aux = torch.zeros(eng.T, E, N, 2, dtype=f32, device=dev)
 
 
 class RolloutEngine:
     def __init__(self, env, n_envs: int, T: Optional[int] = None, n_obs: Optional[int] = None,
                  use_cuda_graph: bool = True, policy: str = "actor", persistent: Optional[bool] = None):
         """policy: 'actor' (a = 2 pi + u_ref, algo.step), 'actor_refine' (that action refined against the CBF,
-        GCBFPlus.online_policy_refinement; set_cbf_params() gives the CBF), 'u_ref' (test.py --u-ref), or a CBF-QP
+        GCBFPlus.online_policy_refinement; set_cbf_params() gives the CBF), 'actor_qp' / 'u_ref_qp' (2 pi + u_ref or
+        u_ref filtered by the CBF, GCBFPlus.safety_filter; set_cbf_params() gives the CBF), 'u_ref' (test.py --u-ref), or a CBF-QP
         baseline: a DecShareCBF / CentralizedCBF object, or its name ('dec_share_cbf' / 'centralized_cbf': built with
         alpha = 1)."""
         self.env = env
@@ -81,14 +99,15 @@ class RolloutEngine:
         elif policy in BASELINES:
             self.controller = BASELINES[policy](env, env.node_dim, env.edge_dim, env.state_dim, env.action_dim,
                                                 env.num_agents)
-        elif policy not in ("actor", "actor_refine", "u_ref"):
+        elif policy not in ("actor", "actor_refine", "u_ref") + QP_FILTER_POLICIES:
             raise ValueError(f"unknown rollout policy {policy!r}")
         if self.controller is None and not getattr(env, "enable_stop", True):
             raise ValueError("the actor / u_ref rollouts apply the DubinsCar stop mask; env.enable_stop is False "
                              "(set by DecShareCBF)")
         self.policy = policy
         self.use_cuda_graph = use_cuda_graph
-        # actor_refine: a copy of the CBF, its prepared planes and the refinement settings (set_cbf_params)
+        # actor_refine / actor_qp / u_ref_qp: a copy of the CBF, its prepared planes (actor_refine) and the settings
+        # (set_cbf_params)
         self.cbf_params: Optional[NetParams] = None
         self._refine_planes: Optional[torch.Tensor] = None
         self.refine_alpha, self.refine_lr, self.refine_max_iter = 1.0, REFINE_LR, REFINE_MAX_ITER
@@ -142,6 +161,9 @@ class RolloutEngine:
         if self.persistent:
             n = env.lib.gcbf_rollout_persistent_workspace_floats(C.byref(self._pdesc))
             self._pws = torch.empty(int(n), dtype=f32, device=dev)
+        # bit 3: rows in ticket order.  The safety filter's sums run over the edge lists in row order, so its policies
+        # build canonical graphs: deterministic, and equal to env.get_graph's
+        self._build_flags = 1 if policy in QP_FILTER_POLICIES else 1 | 8
         self._graph: Optional[torch.cuda.CUDAGraph] = None
         self.launches_per_run = 0
         self._obstacle_obj = None
@@ -159,7 +181,7 @@ class RolloutEngine:
                                       env.ray_table.data_ptr(), self.hits[t, ch.e0].data_ptr(),
                                       ch.row_start[t % 2].data_ptr(), ch.row_deg[t % 2].data_ptr(),
                                       ch.edge_recv[t % 2].data_ptr(), ch.edge_src[t % 2].data_ptr(),
-                                      ch.counters[t].data_ptr(), 1 | 8, stream)      # bit 3: rows in ticket order
+                                      ch.counters[t].data_ptr(), self._build_flags, stream)
         _lib.check(rc, "gcbf_graph_build")
 
     def _step(self, ch: _Chain, t: int, stream: int) -> None:
@@ -168,6 +190,9 @@ class RolloutEngine:
         b = t % 2
         if self.policy == "actor_refine":
             self._step_refine(ch, t, stream)
+            return
+        if self.policy in QP_FILTER_POLICIES:
+            self._step_qp_filter(ch, t, stream)
             return
         if self.policy == "actor":      # algo.step + env.step + get_graph(next) in one call
             rc = env.lib.gcbf_rollout_step_l(
@@ -222,6 +247,41 @@ class RolloutEngine:
         _lib.check(rc, "gcbf_env_step")
         self._build(ch, t + 1, stream)
 
+    def _step_qp_filter(self, ch: _Chain, t: int, stream: int) -> None:
+        """nominal action (actor_qp: policy forward and 2 pi + u_ref; u_ref_qp: u_ref) -> the CBF-QP nearest to it
+        (gcbf_qp_filter; iterations, nominal and (lam, r) recorded) -> env.step with the filtered action as input ->
+        graph build of the next state."""
+        env, d = self.env, ch.desc
+        if self.cbf_params is None:
+            raise RuntimeError(f"the {self.policy} policy needs the CBF: call set_cbf_params() before run()")
+        b = t % 2
+        args = (self.agent[t, ch.e0], self.goal[ch.e0], self.hits[t, ch.e0], ch.row_start[b], ch.row_deg[b],
+                ch.edge_recv[b], ch.edge_src[b], ch.counters[t])
+        pi = None
+        if self.policy == "actor_qp":
+            rc = env.lib.gcbf_gnn_infer(C.byref(d), _lib.NET_ACTOR, env.action_dim, self.params_buf.data_ptr(),
+                                        self.infer_blob.data_ptr(), self.use_tc, *[_lib.ptr(x) for x in args], 0,
+                                        ch.pi.data_ptr(), ch.ws.data_ptr(), ch.ws.numel(), stream)
+            _lib.check(rc, "gcbf_gnn_infer")
+            pi = ch.pi.data_ptr()
+        nominal = ch.qp_nominal[t]
+        _lib.check(env.lib.gcbf_act(C.byref(d), _lib.ptr(args[0]), _lib.ptr(args[1]), pi, nominal.data_ptr(), stream),
+                   "gcbf_act")
+        # u_ref_qp solves with u_nom = NULL: the kernel's own u_ref, the labels' QP (recorded above for the statistics)
+        rc = env.lib.gcbf_qp_filter(C.byref(d), self.refine_alpha, self.use_tc, QP_MAX_ITER, QP_TOL,
+                                    self.cbf_params.flat.data_ptr(), *[_lib.ptr(x) for x in args],
+                                    nominal.data_ptr() if self.policy == "actor_qp" else None,
+                                    self.actions[t, ch.e0].data_ptr(), ch.qp_aux[t].data_ptr(),
+                                    ch.qp_iters[t].data_ptr(), ch.qp_ws.data_ptr(), ch.qp_ws.numel(), stream)
+        _lib.check(rc, "gcbf_qp_filter")
+        obs = self.obstacles[ch.e0].data_ptr() if self.O > 0 else None
+        rc = env.lib.gcbf_env_step(C.byref(d), self.agent[t, ch.e0].data_ptr(), self.goal[ch.e0].data_ptr(), obs,
+                                   None, ch.row_start[b].data_ptr(), ch.row_deg[b].data_ptr(), ch.edge_src[b].data_ptr(),
+                                   self.actions[t, ch.e0].data_ptr(), self.agent[t + 1, ch.e0].data_ptr(),
+                                   self.rewards[t, ch.e0:].data_ptr(), self.costs[t, ch.e0:].data_ptr(), 1, stream)
+        _lib.check(rc, "gcbf_env_step")
+        self._build(ch, t + 1, stream)
+
     def _enqueue_persistent(self, n_steps: int, stream: int) -> None:
         env, ch = self.env, self.chains[0]
         rc = env.lib.gcbf_rollout_persistent(
@@ -260,6 +320,8 @@ class RolloutEngine:
         if n_layers > 1 and self.policy == "actor_refine":
             raise NotImplementedError("online policy refinement implements gnn_layers = 1; the actor has %d GNN layers"
                                       % n_layers)
+        if self.policy in QP_FILTER_POLICIES:
+            require_one_layer(n_layers, f"the {self.policy} policy's actor")
         if n_layers > 1 and self._persistent_requested:
             raise ValueError("the persistent rollout implements one GNN layer; this actor has %d" % n_layers)
         if n_layers > 1 and not self.use_tc:
@@ -328,20 +390,28 @@ class RolloutEngine:
     def set_cbf_params(self, params: NetParams, alpha: float = 1.0, lr: float = REFINE_LR,
                        max_iter: int = REFINE_MAX_ITER) -> None:
         """actor_refine: the CBF the actions are refined against and the refinement's alpha / step size / iteration
-        cap.  The parameters are COPIED (like set_params): after they change, call set_cbf_params again."""
-        if self.policy != "actor_refine":
-            raise RuntimeError("set_cbf_params() is for the actor_refine policy")
-        require_one_layer_refine(params, "CBF")
+        cap.  actor_qp / u_ref_qp: the CBF of the safety filter and its alpha (lr and max_iter are the refinement's and
+        unused; the QP runs with the labels' QP_MAX_ITER / QP_TOL).  The parameters are COPIED (like set_params):
+        after they change, call set_cbf_params again."""
+        qp = self.policy in QP_FILTER_POLICIES
+        if self.policy != "actor_refine" and not qp:
+            raise RuntimeError("set_cbf_params() is for the actor_refine, actor_qp and u_ref_qp policies")
+        if qp:
+            require_one_layer(params.n_layers, "the CBF-QP safety filter")
+        else:
+            require_one_layer_refine(params, "CBF")
         if int(max_iter) < 1:
             raise ValueError(f"max_iter must be >= 1, got {max_iter}")
         settings = (float(alpha), float(lr), int(max_iter))
         if self.cbf_params is None:
             self.cbf_params = params.clone()
-            self._refine_planes = planes_buffer(params)
+            if not qp:
+                self._refine_planes = planes_buffer(params)
         else:       # in place: a captured rollout keeps reading the same buffers
             self.cbf_params.flat.copy_(params.flat)
-        prepare_planes(self.cbf_params, self._refine_planes, self.use_tc,
-                       torch.cuda.current_stream(self.env.device).cuda_stream)
+        if not qp:  # the QP filter builds the planes it needs itself, inside its launch sequence
+            prepare_planes(self.cbf_params, self._refine_planes, self.use_tc,
+                           torch.cuda.current_stream(self.env.device).cuda_stream)
         if settings != (self.refine_alpha, self.refine_lr, self.refine_max_iter):
             self._graph = None      # the settings are baked into the captured launches
         self.refine_alpha, self.refine_lr, self.refine_max_iter = settings
@@ -356,11 +426,20 @@ class RolloutEngine:
         return st
 
     def qp_stats(self) -> dict:
-        """CBF-QP baselines: median / max iterations and capped solves over every solve of the last run() (reads the
-        device record once; call after run())."""
+        """CBF-QP baselines and the actor_qp / u_ref_qp safety filters: median / max iterations and capped solves over
+        every solve of the last run() (reads the device record once; call after run()).  The safety filters also report
+        the mean |u - u_nom| over the agent-steps (`mean_correction`) and the fraction of agent-steps whose CBF
+        condition was relaxed (r > 0, `relaxed_frac`); a solve counts as capped when it ran QP_MAX_ITER iterations."""
+        ch = self.chains[0]
+        if self.policy in QP_FILTER_POLICIES:
+            n = ch.qp_iters & (CAPPED_BIT - 1)          # bit 30 of the QP's count marks the dense-graph path, not a cap
+            st = iter_stats(torch.where(n >= QP_MAX_ITER, n | CAPPED_BIT, n))
+            st["mean_correction"] = float(torch.linalg.vector_norm(self.actions - ch.qp_nominal, dim=-1).mean())
+            st["relaxed_frac"] = float((ch.qp_aux[..., 1] > 0).float().mean())
+            return st
         if self.controller is None:
-            raise RuntimeError("qp_stats() needs a CBF-QP baseline policy")
-        return iter_stats(self.chains[0].qp_iters.reshape(-1))
+            raise RuntimeError("qp_stats() needs a CBF-QP baseline or safety-filter policy")
+        return iter_stats(ch.qp_iters.reshape(-1))
 
     def check_overflow(self) -> None:
         c = self.counters.cpu()

@@ -345,6 +345,20 @@ int32_t gcbf_qp_labels(const gcbf_env_desc* desc, float alpha, int32_t use_tenso
                        const int32_t* edge_recv, const int32_t* edge_src, const int32_t* counters,
                        float* u_qp, float* aux, int32_t* iters, float* workspace, int64_t workspace_floats,
                        void* stream);
+/* gcbf_qp_filter: the learned-CBF safety filter.  The QP of gcbf_qp_labels with a nominal action in place of u_ref:
+ *   min_{u,r} 1/2|u|^2 - u_nom.u + 5|r|^2 + 1000 sum(r)   (same constraints)
+ * i.e. the action closest to u_nom that keeps the CBF condition (relaxed by r where no admissible action does).
+ *   u_nom [G, N, nu]: the nominal action (the policy's 2 pi + u_ref, or any other); may lie outside the u_lim box.
+ *     NULL: u_ref, and then every output is bit-identical to gcbf_qp_labels'.
+ *   u [G, N, nu] (out), aux, iters, workspace (gcbf_qp_workspace_floats) and the other arguments as gcbf_qp_labels.
+ * The solve's sums run over the edge lists in row order, so the result depends on the layout: callers that need
+ * deterministic results pass canonical graphs (gcbf_graph_build without flags bit3). */
+int32_t gcbf_qp_filter(const gcbf_env_desc* desc, float alpha, int32_t use_tensor_cores, int32_t max_iter,
+                       float tol, const float* cbf_params, const float* agent, const float* goal,
+                       const float* hits, const int32_t* row_start, const int32_t* row_deg,
+                       const int32_t* edge_recv, const int32_t* edge_src, const int32_t* counters,
+                       const float* u_nom, float* u, float* aux, int32_t* iters, float* workspace,
+                       int64_t workspace_floats, void* stream);
 
 /* ---------------------------------------------------------------- online policy refinement
  * gcbf_refine_actions replaces GCBF.online_policy_refinement (gcbfplus/algo/gcbf.py:161-201, inherited by GCBFPlus)

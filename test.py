@@ -7,7 +7,10 @@ reference needs it to survive n >= 512 with dense graphs (env/base.py:191-259); 
 --algo centralized_cbf | dec_share_cbf without --path runs the CBF-QP baseline controllers (test.py:88-103) with
 alpha = --alpha and writes to ./logs/<env>/<algo>.
 --online-refine (with --path) refines every action of the trained GCBF+ policy against its CBF
-(GCBFPlus.online_policy_refinement, gcbf.py:161-201) and prints the refinement's iteration statistics."""
+(GCBFPlus.online_policy_refinement, gcbf.py:161-201) and prints the refinement's iteration statistics.
+--qp-filter (with --path) passes every action of the trained GCBF+ policy through the learned CBF's QP safety filter
+(GCBFPlus.safety_filter: the action nearest to 2 pi + u_ref that keeps the CBF condition); with --u-ref as well it
+filters u_ref instead (the reference's get_qp_action as a controller).  It prints the QP statistics after the rates."""
 import argparse
 import os
 
@@ -16,6 +19,7 @@ import yaml
 
 from gcbfplus_b200.algo import make_algo
 from gcbfplus_b200.algo.cbf_qp import BASELINES
+from gcbfplus_b200.algo.train import QP_MAX_ITER
 from gcbfplus_b200.env import make_env
 from gcbfplus_b200.trainer.rollout import RolloutEngine
 from gcbfplus_b200.trainer.utils import cbf_contours, test_rates
@@ -25,10 +29,12 @@ def test(args):
     print(f"> Running test.py {args}")
     if args.cpu:
         raise SystemExit("--cpu: gcbfplus_b200 is the sm_90a CUDA path only (no CPU fallback by design)")
+    check_qp_filter_flags(args)
     check_refine_flags(args)
     np.random.seed(args.seed)
     config = None
-    if not args.u_ref and args.path is not None:
+    trained = args.path is not None and (not args.u_ref or args.qp_filter)
+    if trained:
         with open(os.path.join(args.path, "config.yaml"), "r") as f:
             config = yaml.load(f, Loader=yaml.UnsafeLoader)
     num_agents = config.num_agents if args.num_agents is None else args.num_agents
@@ -47,7 +53,7 @@ def test(args):
         policy = algo
         path = os.path.join(f"./logs/{args.env}/{args.algo}")
         os.makedirs(path, exist_ok=True)
-    elif not args.u_ref:
+    elif trained or not args.u_ref:
         assert args.path is not None, "--path or --u-ref required"
         model_path = os.path.join(args.path, "models")
         step = max(int(m) for m in os.listdir(model_path) if m.isdigit()) if args.step is None else args.step
@@ -61,7 +67,10 @@ def test(args):
             loss_safe_coef=config.loss_safe_coef, loss_h_dot_coef=config.loss_h_dot_coef, max_grad_norm=2.0,
             seed=config.seed)
         algo.load(model_path, step)
-        policy = "actor_refine" if args.online_refine else "actor"
+        if args.qp_filter:
+            policy = "u_ref_qp" if args.u_ref else "actor_qp"
+        else:
+            policy = "actor_refine" if args.online_refine else "actor"
         path = args.path
     else:
         assert args.env is not None
@@ -71,7 +80,7 @@ def test(args):
     eng = RolloutEngine(env, n_epi, T=env.max_episode_steps, policy=policy)
     if algo is not None and not baseline:
         eng.set_params(algo.actor_params)
-        if args.online_refine:
+        if args.online_refine or args.qp_filter:
             eng.set_cbf_params(algo.cbf_params, alpha=algo.alpha)
     # test.py:117-119,158: test_keys = split(PRNGKey(seed), 1000)[:epi][offset:]; episode i resets with
     # split(test_keys[i])[0].  All episodes run as one batch here.
@@ -94,12 +103,16 @@ def test(args):
           f"cost: {np.mean(costs):.3f}, min/max cost: {np.min(costs):.3f}/{np.max(costs):.3f}, "
           f"safe_rate: {safe_mean * 100:.3f}%, finish_rate: {finish_mean * 100:.3f}%, "
           f"success_rate: {succ.mean() * 100:.3f}%")
-    if baseline:
+    if baseline or args.qp_filter:
         st = eng.qp_stats()
         print(f"QP iterations: median {st['iters_median']:.0f}, max {st['iters_max']}, "
               f"capped {st['capped']} of {st['solves']} solves")
+        if args.qp_filter:
+            print(f"QP filter: mean |u - u_nom| {st['mean_correction']:.4f}, CBF condition relaxed (r > 0) in "
+                  f"{st['relaxed_frac'] * 100:.3f}% of agent-steps")
         if st["capped"]:
-            print(f"WARNING: {st['capped']} QP solve(s) hit the iteration cap ({algo.max_iter}); their actions are the "
+            cap = QP_MAX_ITER if args.qp_filter else algo.max_iter
+            print(f"WARNING: {st['capped']} QP solve(s) hit the iteration cap ({cap}); their actions are the "
                   "capped iterates, not the exact QP minimisers")
     if args.online_refine:
         st = eng.refine_stats()
@@ -139,6 +152,20 @@ def check_refine_flags(args) -> None:
         raise SystemExit("--online-refine needs a trained GCBF+ run (--path)")
 
 
+def check_qp_filter_flags(args) -> None:
+    """--qp-filter filters through a trained GCBF+ CBF: it needs --path and excludes --online-refine and the
+    baselines (--u-ref selects u_ref as the nominal action)."""
+    if not args.qp_filter:
+        return
+    if args.online_refine:
+        raise SystemExit("--qp-filter and --online-refine both correct the policy's action; give one of them")
+    if args.algo in BASELINES:
+        raise SystemExit(f"--qp-filter filters through a trained GCBF+ CBF; it cannot be combined with the {args.algo} "
+                         "baseline")
+    if args.path is None:
+        raise SystemExit("--qp-filter needs a trained GCBF+ run (--path)")
+
+
 # the reference's command line (test.py:239-266), table-driven like train.py
 FLAGS = [
     (("-n", "--num-agents"), int, None), (("--obs",), int, 0), (("--area-size",), float, "required"),
@@ -147,7 +174,7 @@ FLAGS = [
     (("--cpu",), "flag", False), (("--u-ref",), "flag", False), (("--env",), str, None), (("--algo",), str, None),
     (("--step",), int, None), (("--epi",), int, 5), (("--offset",), int, 0), (("--no-video",), "flag", False),
     (("--nojit-rollout",), "flag", False), (("--log",), "flag", False), (("--dpi",), int, 100),
-    (("--online-refine",), "flag", False),
+    (("--online-refine",), "flag", False), (("--qp-filter",), "flag", False),
 ]
 
 
