@@ -64,6 +64,10 @@ _SIGNATURES = {
     "gcbf_rollout_persistent_supported": (C.c_int32, [C.POINTER(EnvDesc)]),
     "gcbf_rollout_persistent_max_clusters": (C.c_int32, [C.c_int32]),
     "gcbf_rollout_persistent": (C.c_int32, [C.POINTER(EnvDesc), C.c_int32] + [_P] * 12 + [C.c_int64, _P, _P]),
+    "gcbf_rollout_persistent_multi": (C.c_int32, [C.POINTER(EnvDesc), C.c_int32, C.c_int32] + [_P] * 13 +
+                                      [C.c_int64, _P, _P]),
+    "gcbf_rollout_persistent_multi_strides": (C.c_int32, [C.c_int32, C.c_int32, C.POINTER(C.c_int64),
+                                                          C.POINTER(C.c_int64)]),
     "gcbf_env_step": (C.c_int32, [C.POINTER(EnvDesc)] + [_P] * 11 + [C.c_int32, _P]),
     "gcbf_act": (C.c_int32, [C.POINTER(EnvDesc)] + [_P] * 5),
     "gcbf_masks": (C.c_int32, [C.POINTER(EnvDesc)] + [_P] * 9),

@@ -89,6 +89,13 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* m
         "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
         : "memory");
 }
+__device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2) {
+    asm volatile(
+        "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];" ::"r"(
+            smem_u32(smem_dst)),
+        "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
+        : "memory");
+}
 
 // generic-proxy shared-memory writes -> reads by the async proxy (wgmma operands, TMA)
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
@@ -414,6 +421,30 @@ inline int32_t make_map_box(CUtensorMap* map, const float* ptr, int rows, int co
 // row-major [rows, cols] tensor, box = [box_rows, BK cols] with the 128-byte swizzle the MMA descriptors expect
 inline int32_t make_map(CUtensorMap* map, const float* ptr, int rows, int cols, int box_rows) {
     return make_map_box(map, ptr, rows, cols, cols, box_rows, BK, CU_TENSOR_MAP_SWIZZLE_128B);
+}
+// `depth` row-major [rows, cols] tensors `stride` floats apart as one 3-D map (the stack index outermost, a multiple of
+// 4 floats), box = [1, box_rows, BK cols] with make_map's swizzle: a load with third coordinate k lands the same tile
+// of tensor k that make_map's load lands of tensor 0
+inline int32_t make_map_stack(CUtensorMap* map, const float* ptr, int rows, int cols, int box_rows, int depth,
+                              int64_t stride) {
+    EncodeTiledFn fn = encode_fn();
+    if (!fn) {
+        set_error("cuTensorMapEncodeTiled unavailable");
+        return -2;
+    }
+    cuuint64_t dims[3] = {(cuuint64_t)cols, (cuuint64_t)rows, (cuuint64_t)depth};
+    cuuint64_t strides[2] = {(cuuint64_t)cols * 4, (cuuint64_t)stride * 4};
+    cuuint32_t box[3] = {(cuuint32_t)BK, (cuuint32_t)box_rows, 1};
+    cuuint32_t estr[3] = {1, 1, 1};
+    CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(ptr), dims, strides, box, estr,
+                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) {
+        set_error("cuTensorMapEncodeTiled failed (%d) rows=%d cols=%d depth=%d stride=%lld", (int)r, rows, cols, depth,
+                  (long long)stride);
+        return -2;
+    }
+    return 0;
 }
 
 template <int EPI, bool ACC>

@@ -84,6 +84,12 @@ struct PArgs {
     // (arrival counter in global memory) once per step.
     int soft;                                            // 0 / 1 = mode
     unsigned* gbar;                                      // [E] arrival counters of the environment barrier (zeroed by the launcher)
+    // network table (gcbf_rollout_persistent_multi): environment e runs network net_of_env[e] (NULL: network 0), whose
+    // raw parameters / folded weights sit p_stride / i_stride floats after the previous network's; the weight-plane maps
+    // are 3-D with the network outermost.  counters is [T + 1][n_nets][4].
+    const int32_t* net_of_env;
+    int64_t p_stride, i_stride;
+    int n_nets;
 };
 
 __device__ __forceinline__ unsigned long long gtime() {
@@ -171,6 +177,9 @@ rollout_persist_kernel(const __grid_constant__ PArgs P, const __grid_constant__ 
     const int seg_cap = cap / (C / L);                // edge rows of one local group (mode 0: the whole environment)
     const int seg_off = grp * seg_cap;                // ... and where they start inside the environment's lists
     const int ga_lo = min(grp * L * APC, N), ga_hi = min(ga_lo + L * APC, N);   // agents of my local group
+    // this environment's network.  Re-read where it is used (one L1 / L2 hit) rather than kept live across the step
+    // loop: the kernel sits at its 128-register limit
+    auto net = [&]() { return P.net_of_env != nullptr ? P.net_of_env[env] : 0; };
 
     // ---------------------------------------------------------------- one-time setup
     if (tid == 0) {
@@ -186,19 +195,20 @@ rollout_persist_kernel(const __grid_constant__ PArgs P, const __grid_constant__ 
         mbar_init(&bars[B_T2F], CONSUMERS);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    load_l1_table<ED>(sW, P.W1, P.b1, tid, PT);    // message layer 1: W1[:ED] and the per-sender-type bias table
+    const int64_t p_off = net() * P.p_stride, i_off = net() * P.i_stride;   // this network's raw / folded weights
+    load_l1_table<ED>(sW, P.W1 + p_off, P.b1 + p_off, tid, PT);   // message layer 1: W1[:ED] and the per-sender-type bias table
     auto stage = [&](int off, const float* src, int n) {
         for (int i = tid; i < n; i += PT) sk[off + i] = src[i];
     };
-    stage(K_B23, P.b23, 128);
-    stage(K_BIAS_G, P.bias_g, 128);
-    stage(K_AVEC, P.avec, 128);
-    stage(K_BU1, P.b_u1, 256);
-    stage(K_BU1ROW, P.b_u1row, 256);
-    stage(K_BUH, P.buh, 256);
-    stage(K_HO, P.ho, 256 * NU);
-    stage(K_BHO, P.bho, NU);
-    stage(K_CST, P.cst, 1);
+    stage(K_B23, P.b23 + i_off, 128);
+    stage(K_BIAS_G, P.bias_g + p_off, 128);
+    stage(K_AVEC, P.avec + i_off, 128);
+    stage(K_BU1, P.b_u1 + p_off, 256);
+    stage(K_BU1ROW, P.b_u1row + p_off, 256);
+    stage(K_BUH, P.buh + i_off, 256);
+    stage(K_HO, P.ho + i_off, 256 * NU);
+    stage(K_BHO, P.bho + i_off, NU);
+    stage(K_CST, P.cst + i_off, 1);
     // obstacles of this environment (+ derived far-skip fields) and the ray table stay resident for the whole rollout
     if (O > 0) {
         const float* ob = P.obstacles + (d.obs_per_graph ? (size_t)env * O * OBW : 0);
@@ -232,6 +242,7 @@ rollout_persist_kernel(const __grid_constant__ PArgs P, const __grid_constant__ 
             const size_t seg_e0 = env_e0 + seg_off;                      // first slot of the segment
             if (warp == 0) {
                 if (lane == 0) {
+                    const int k = net();
                     uint32_t it_l = it, ne_l = ne;
                     for (int tile = lrank; tile < n_tiles; tile += L, ++ne_l) {
                         if (ne_l > 0) mbar_wait(&bars[B_T2F], (ne_l - 1) & 1);
@@ -240,8 +251,8 @@ rollout_persist_kernel(const __grid_constant__ PArgs P, const __grid_constant__ 
                             mbar_wait(&bars[B_EMPTY + s], ((it_l / 3) & 1) ^ 1);
                             uint8_t* st = smem + s * STG;
                             mbar_expect_tx(&bars[B_FULL + s], 2 * B_BYTES);
-                            tma_load_2d(st + 2 * A_BYTES, &tmW23h, &bars[B_FULL + s], kb * BK, 0);
-                            tma_load_2d(st + 2 * A_BYTES + B_BYTES, &tmW23l, &bars[B_FULL + s], kb * BK, 0);
+                            tma_load_3d(st + 2 * A_BYTES, &tmW23h, &bars[B_FULL + s], kb * BK, 0, k);
+                            tma_load_3d(st + 2 * A_BYTES + B_BYTES, &tmW23l, &bars[B_FULL + s], kb * BK, 0, k);
                         }
                         mbar_wait(&bars[B_MAIN], ne_l & 1);           // main-loop MMAs retired: stage 2 is free
                         for (int kb2 = 0; kb2 < 4; ++kb2) {
@@ -249,8 +260,8 @@ rollout_persist_kernel(const __grid_constant__ PArgs P, const __grid_constant__ 
                             mbar_wait(&bars[B_B2E + slot], (use & 1) ^ 1);
                             uint8_t* sl = smem + 2 * STG + slot * 32768;
                             mbar_expect_tx(&bars[B_B2F + slot], 32768);
-                            tma_load_2d(sl, &tmA1h, &bars[B_B2F + slot], kb2 * BK, 0);
-                            tma_load_2d(sl + 16384, &tmA1l, &bars[B_B2F + slot], kb2 * BK, 0);
+                            tma_load_3d(sl, &tmA1h, &bars[B_B2F + slot], kb2 * BK, 0, k);
+                            tma_load_3d(sl + 16384, &tmA1l, &bars[B_B2F + slot], kb2 * BK, 0, k);
                         }
                     }
                 }
@@ -343,6 +354,7 @@ rollout_persist_kernel(const __grid_constant__ PArgs P, const __grid_constant__ 
                 const CUtensorMap* tmBl = ph2 == 0 ? &tmU1l : &tmUHl;
                 if (warp == 0) {
                     if (lane == 0) {
+                        const int k = net();
                         uint32_t it_l = it;
                         fence_async_global();      // consumer side of the generic-store -> TMA-load hand-over (AG / V1)
                         for (int item = lrank; item < n_items; item += L) {
@@ -353,8 +365,8 @@ rollout_persist_kernel(const __grid_constant__ PArgs P, const __grid_constant__ 
                                 uint8_t* st = smem + s * STG;
                                 mbar_expect_tx(&bars[B_FULL + s], A_BYTES + 2 * B_BYTES);
                                 tma_load_2d(st, tmA, &bars[B_FULL + s], kb * BK, env_a0 + m0);
-                                tma_load_2d(st + 2 * A_BYTES, tmBh, &bars[B_FULL + s], kb * BK, nc0);
-                                tma_load_2d(st + 2 * A_BYTES + B_BYTES, tmBl, &bars[B_FULL + s], kb * BK, nc0);
+                                tma_load_3d(st + 2 * A_BYTES, tmBh, &bars[B_FULL + s], kb * BK, nc0, k);
+                                tma_load_3d(st + 2 * A_BYTES + B_BYTES, tmBl, &bars[B_FULL + s], kb * BK, nc0, k);
                             }
                         }
                     }
@@ -529,7 +541,7 @@ rollout_persist_kernel(const __grid_constant__ PArgs P, const __grid_constant__ 
                 const int rbase = seg_off + base + s_off[slot];       // row offset inside the environment's lists
                 if (over) {
                     if (lane == 0) {
-                        atomicOr(&P.counters[(size_t)tn * 4 + 1], 1);
+                        atomicOr(&P.counters[((size_t)tn * P.n_nets + net()) * 4 + 1], 1);
                         rs_n[a_id] = 0;
                         rd_n[a_id] = 0;
                     }
@@ -541,7 +553,7 @@ rollout_persist_kernel(const __grid_constant__ PArgs P, const __grid_constant__ 
                 }
                 fill_row(er_n + env_e0, es_n + env_e0, rbase, a_id, env_a0, sbits + slot * n_words, n_words, s_hb[slot], lane);
             }
-            if (lrank == 0 && tid == 0) atomicAdd(&P.counters[(size_t)tn * 4 + 0], min(env_total, seg_cap));
+            if (lrank == 0 && tid == 0) atomicAdd(&P.counters[((size_t)tn * P.n_nets + net()) * 4 + 0], min(env_total, seg_cap));
             M_cur = min(env_total, seg_cap);
             SYNC_LOCAL();
             if (stamp) pr[7] = gtime();
@@ -650,14 +662,33 @@ extern "C" __attribute__((visibility("default"))) int32_t gcbf_rollout_persisten
     return n;
 }
 
-extern "C" __attribute__((visibility("default"))) int32_t gcbf_rollout_persistent(
-    const gcbf_env_desc* desc, int32_t n_steps, const float* actor_params, const float* infer_blob, const float* goal,
-    const float* obstacles, const float* ray_table, float* agent_rec, float* hits_rec, float* actions_rec, float* rewards,
-    float* costs, int32_t* counters, float* workspace, int64_t workspace_floats, uint64_t* phase_stamps, void* stream) {
+// Per-network strides of the stacked arrays of gcbf_rollout_persistent_multi: the raw-parameter and folded-weight counts
+// rounded up to 4 floats (16 bytes: the stride of a TMA map and the alignment every network's block keeps).
+static int64_t net_stride(int64_t count) { return (count + 3) & ~(int64_t)3; }
+
+extern "C" __attribute__((visibility("default"))) int32_t gcbf_rollout_persistent_multi_strides(
+    int32_t edge_dim, int32_t out_dim, int64_t* param_stride, int64_t* infer_stride) {
+    GCBF_REQUIRE(param_stride && infer_stride, "gcbf_rollout_persistent_multi_strides: NULL pointer argument");
+    const int32_t pc = gcbf_param_count_l(edge_dim, out_dim, 1), ic = gcbf_infer_count(edge_dim, out_dim);
+    GCBF_REQUIRE(pc > 0 && ic > 0, "gcbf_rollout_persistent_multi_strides: bad argument (edge_dim %d, out_dim %d)",
+                 edge_dim, out_dim);
+    *param_stride = net_stride(pc);
+    *infer_stride = net_stride(ic);
+    return 0;
+}
+
+// The launch behind gcbf_rollout_persistent (n_nets = 1, net_of_env NULL) and gcbf_rollout_persistent_multi.  `rounds`
+// (the multi entry point) also launches when the environments' clusters are not all co-resident and pair mode does not
+// fit: in mode 0 no cluster ever waits on another, so the clusters beyond the resident ones run in later rounds.
+static int32_t persist_launch(const char* who, bool rounds, const gcbf_env_desc* desc, int32_t n_steps, int32_t n_nets,
+                              const float* actor_params, const float* infer_blob, const int32_t* net_of_env,
+                              const float* goal, const float* obstacles, const float* ray_table, float* agent_rec,
+                              float* hits_rec, float* actions_rec, float* rewards, float* costs, int32_t* counters,
+                              float* workspace, int64_t workspace_floats, uint64_t* phase_stamps, void* stream) {
     GCBF_REQUIRE(desc && actor_params && infer_blob && goal && ray_table && agent_rec && hits_rec && actions_rec && rewards &&
-                     costs && counters && workspace, "gcbf_rollout_persistent: NULL pointer argument");
-    GCBF_REQUIRE(gcbf_rollout_persistent_supported(desc) > 0, "gcbf_rollout_persistent: unsupported configuration (2-D envs, "
-                 "n_agents <= 512, n_obs <= 32, edge_cap >= n_graphs * n_agents)");
+                     costs && counters && workspace, "%s: NULL pointer argument", who);
+    GCBF_REQUIRE(gcbf_rollout_persistent_supported(desc) > 0, "%s: unsupported configuration (2-D envs, "
+                 "n_agents <= 512, n_obs <= 32, edge_cap >= n_graphs * n_agents)", who);
     GCBF_REQUIRE(desc->n_obs == 0 || obstacles, "obstacles is NULL but n_obs > 0");
     GCBF_REQUIRE(n_steps >= 0, "n_steps must be >= 0");
     const int E = desc->n_graphs, N = desc->n_agents;
@@ -676,13 +707,19 @@ extern "C" __attribute__((visibility("default"))) int32_t gcbf_rollout_persisten
     P.T = n_steps;
     P.cap_env = cap_env;
     P.C = rp::cluster_size(N, cap_env);
+    P.net_of_env = net_of_env;
+    P.n_nets = n_nets;
+    P.p_stride = net_stride(gcbf_param_count_l(ed, nu, 1));
+    P.i_stride = net_stride(gcbf_infer_count(ed, nu));
     const int max_cl = gcbf_rollout_persistent_max_clusters(P.C);
     // mode 0: one hardware cluster per environment when all of them are resident at once; otherwise mode 1: clusters of 2 + one software barrier per step, when the grid fits on the
     // device (1 CTA / SM).  GCBF_PERSIST_SOFT=1 forces mode 1 (tests).
     static const int force_soft = [] { const char* e = getenv("GCBF_PERSIST_SOFT"); return e ? atoi(e) : -1; }();
-    P.soft = (force_soft >= 0) ? (force_soft != 0) : ((E <= max_cl) ? 0 : 1);
-    GCBF_REQUIRE(!P.soft || (P.C >= 2 && E * P.C <= sm_count()), "pair mode needs n_graphs * %d <= %d CTAs", P.C, sm_count());
-    GCBF_REQUIRE(P.soft || E <= max_cl || force_soft == 0, "more environments (%d) than resident clusters (%d)", E, max_cl);
+    const bool pairs_fit = P.C >= 2 && E * P.C <= sm_count();
+    P.soft = (force_soft >= 0) ? (force_soft != 0) : ((E <= max_cl || (rounds && !pairs_fit)) ? 0 : 1);
+    GCBF_REQUIRE(!P.soft || pairs_fit, "pair mode needs n_graphs * %d <= %d CTAs", P.C, sm_count());
+    GCBF_REQUIRE(P.soft || E <= max_cl || force_soft == 0 || rounds, "more environments (%d) than resident clusters (%d)", E,
+                 max_cl);
     P.gbar = reinterpret_cast<unsigned*>(workspace + W.gbar);
     P.W1 = actor_params + L.w[L_MSG0];
     P.b1 = actor_params + L.b[L_MSG0];
@@ -716,15 +753,17 @@ extern "C" __attribute__((visibility("default"))) int32_t gcbf_rollout_persisten
     P.edge_src = reinterpret_cast<int32_t*>(workspace + W.edge_src);
     CUtensorMap tW23h, tW23l, tA1h, tA1l, tU1h, tU1l, tUHh, tUHl, tAG, tV1;
     int32_t rc;
+    const int K = n_nets;
+    const int64_t S = P.i_stride;
 #define RC(x) do { if ((rc = (x))) return rc; } while (0)
-    RC(tc::make_map(&tW23h, infer_blob + I.t_w23, 128, 256, 128));
-    RC(tc::make_map(&tW23l, infer_blob + I.t_w23 + 256 * 128, 128, 256, 128));
-    RC(tc::make_map(&tA1h, infer_blob + I.t_a1, 128, 128, 128));
-    RC(tc::make_map(&tA1l, infer_blob + I.t_a1 + 128 * 128, 128, 128, 128));
-    RC(tc::make_map(&tU1h, infer_blob + I.t_u1, 256, 128, 128));
-    RC(tc::make_map(&tU1l, infer_blob + I.t_u1 + 256 * 128, 256, 128, 128));
-    RC(tc::make_map(&tUHh, infer_blob + I.t_uh, 256, 256, 128));
-    RC(tc::make_map(&tUHl, infer_blob + I.t_uh + 256 * 256, 256, 256, 128));
+    RC(tc::make_map_stack(&tW23h, infer_blob + I.t_w23, 128, 256, 128, K, S));
+    RC(tc::make_map_stack(&tW23l, infer_blob + I.t_w23 + 256 * 128, 128, 256, 128, K, S));
+    RC(tc::make_map_stack(&tA1h, infer_blob + I.t_a1, 128, 128, 128, K, S));
+    RC(tc::make_map_stack(&tA1l, infer_blob + I.t_a1 + 128 * 128, 128, 128, 128, K, S));
+    RC(tc::make_map_stack(&tU1h, infer_blob + I.t_u1, 256, 128, 128, K, S));
+    RC(tc::make_map_stack(&tU1l, infer_blob + I.t_u1 + 256 * 128, 256, 128, 128, K, S));
+    RC(tc::make_map_stack(&tUHh, infer_blob + I.t_uh, 256, 256, 128, K, S));
+    RC(tc::make_map_stack(&tUHl, infer_blob + I.t_uh + 256 * 256, 256, 256, 128, K, S));
     RC(tc::make_map(&tAG, P.ag, E * N + 128, 128, 128));
     RC(tc::make_map(&tV1, P.v1, E * N + 128, 256, 128));
 #undef RC
@@ -762,7 +801,7 @@ extern "C" __attribute__((visibility("default"))) int32_t gcbf_rollout_persisten
         GCBF_RP_CASE(GCBF_ENV_DOUBLE_INTEGRATOR)
         GCBF_RP_CASE(GCBF_ENV_DUBINS_CAR)
 #undef GCBF_RP_CASE
-        default: set_error("gcbf_rollout_persistent: bad env_kind"); return -1;
+        default: set_error("%s: bad env_kind", who); return -1;
     }
     if (e != cudaSuccess) {
         set_error("rollout_persist_kernel launch: %s", cudaGetErrorString(e));
@@ -770,4 +809,28 @@ extern "C" __attribute__((visibility("default"))) int32_t gcbf_rollout_persisten
     }
     count_launch();
     return check_launch("rollout_persist_kernel");
+}
+
+extern "C" __attribute__((visibility("default"))) int32_t gcbf_rollout_persistent(
+    const gcbf_env_desc* desc, int32_t n_steps, const float* actor_params, const float* infer_blob, const float* goal,
+    const float* obstacles, const float* ray_table, float* agent_rec, float* hits_rec, float* actions_rec, float* rewards,
+    float* costs, int32_t* counters, float* workspace, int64_t workspace_floats, uint64_t* phase_stamps, void* stream) {
+    return persist_launch("gcbf_rollout_persistent", false, desc, n_steps, 1, actor_params, infer_blob, nullptr, goal,
+                          obstacles, ray_table, agent_rec, hits_rec, actions_rec, rewards, costs, counters, workspace,
+                          workspace_floats, phase_stamps, stream);
+}
+
+extern "C" __attribute__((visibility("default"))) int32_t gcbf_rollout_persistent_multi(
+    const gcbf_env_desc* desc, int32_t n_steps, int32_t n_nets, const float* actor_params, const float* infer_blob,
+    const int32_t* net_of_env, const float* goal, const float* obstacles, const float* ray_table, float* agent_rec,
+    float* hits_rec, float* actions_rec, float* rewards, float* costs, int32_t* counters, float* workspace,
+    int64_t workspace_floats, uint64_t* phase_stamps, void* stream) {
+    GCBF_REQUIRE(n_nets >= 1, "gcbf_rollout_persistent_multi: n_nets must be >= 1, got %d", n_nets);
+    GCBF_REQUIRE(net_of_env != nullptr, "gcbf_rollout_persistent_multi: net_of_env is NULL");
+    GCBF_REQUIRE(((uintptr_t)actor_params & 15) == 0 && ((uintptr_t)infer_blob & 15) == 0 && ((uintptr_t)net_of_env & 3) == 0,
+                 "gcbf_rollout_persistent_multi: the stacked actor_params / infer_blob must be 16-byte aligned, "
+                 "net_of_env 4-byte aligned");
+    return persist_launch("gcbf_rollout_persistent_multi", true, desc, n_steps, n_nets, actor_params, infer_blob,
+                          net_of_env, goal, obstacles, ray_table, agent_rec, hits_rec, actions_rec, rewards, costs,
+                          counters, workspace, workspace_floats, phase_stamps, stream);
 }

@@ -17,6 +17,11 @@ The `actor_qp` and `u_ref_qp` policies (the learned CBF as a QP safety filter, G
 path: per step the policy forward and its action 2 pi + u_ref (actor_qp) or u_ref (u_ref_qp) as the nominal, the CBF-QP
 nearest to it (gcbf_qp_filter), env.step with the filtered action as input, and the canonical graph build of the next
 state.
+Several actor networks (n_nets > 1; set_params() takes a list): environment g runs network net_of_env[g], by default
+g // (n_envs // n_nets).  Where the persistent kernel applies, ONE gcbf_rollout_persistent_multi launch rolls out every
+network, each cluster reading its own network's weights, so every network's environments get the bits a solo persistent
+rollout of that network gives them.  Otherwise (LinearDrone, n > 512, deeper actors, persistent=False or not chosen by
+default) the engine runs one solo engine per network, one after another, and gathers their records.
 """
 from __future__ import annotations
 
@@ -81,10 +86,40 @@ class _Chain:
             self.qp_aux = torch.zeros(eng.T, E, N, 2, dtype=f32, device=dev)
 
 
+def check_net_table(net_of_env, n_nets: int, n_envs: int) -> list:
+    """Host check of a network table before any launch: one entry per environment, each in [0, n_nets), and every
+    network runs at least one environment.  Returns the table as a list of ints."""
+    table = [int(k) for k in net_of_env]
+    if len(table) != n_envs:
+        raise ValueError(f"net_of_env has {len(table)} entries for {n_envs} environments")
+    bad = [k for k in table if not 0 <= k < n_nets]
+    if bad:
+        raise ValueError(f"net_of_env entry {bad[0]} is out of range for {n_nets} networks")
+    idle = sorted(set(range(n_nets)) - set(table))
+    if idle:
+        raise ValueError(f"network {idle[0]} runs no environment in net_of_env")
+    return table
+
+
+def check_nets(nets, n_nets: int) -> list:
+    """The networks of one multi-network rollout: n_nets actors of one edge dim, action dim and depth."""
+    nets = [nets] if isinstance(nets, NetParams) else list(nets)
+    if len(nets) != n_nets:
+        raise ValueError(f"set_params: the engine runs {n_nets} networks, got {len(nets)}")
+    for key in ("edge_dim", "out_dim", "n_layers"):
+        vals = [getattr(p, key) for p in nets]
+        if len(set(vals)) > 1:
+            raise ValueError(f"set_params: the networks differ in {key} ({vals})")
+    return nets
+
+
 class RolloutEngine:
     def __init__(self, env, n_envs: int, T: Optional[int] = None, n_obs: Optional[int] = None,
-                 use_cuda_graph: bool = True, policy: str = "actor", persistent: Optional[bool] = None):
-        """policy: 'actor' (a = 2 pi + u_ref, algo.step), 'actor_refine' (that action refined against the CBF,
+                 use_cuda_graph: bool = True, policy: str = "actor", persistent: Optional[bool] = None,
+                 n_nets: int = 1, net_of_env=None):
+        """n_nets: number of actor networks (policy 'actor' only).  Environment g runs network net_of_env[g]; the
+        default table gives each network n_envs // n_nets consecutive environments (n_envs % n_nets == 0).
+        policy: 'actor' (a = 2 pi + u_ref, algo.step), 'actor_refine' (that action refined against the CBF,
         GCBFPlus.online_policy_refinement; set_cbf_params() gives the CBF), 'actor_qp' / 'u_ref_qp' (2 pi + u_ref or
         u_ref filtered by the CBF, GCBFPlus.safety_filter; set_cbf_params() gives the CBF), 'u_ref' (test.py --u-ref), or a CBF-QP
         baseline: a DecShareCBF / CentralizedCBF object, or its name ('dec_share_cbf' / 'centralized_cbf': built with
@@ -106,6 +141,18 @@ class RolloutEngine:
                              "(set by DecShareCBF)")
         self.policy = policy
         self.use_cuda_graph = use_cuda_graph
+        self.n_nets = int(n_nets)
+        if self.n_nets < 1:
+            raise ValueError(f"n_nets must be >= 1, got {n_nets}")
+        if self.n_nets > 1 and policy != "actor":
+            raise ValueError(f"n_nets > 1 rolls out actor networks (policy 'actor'), not {policy!r}")
+        if net_of_env is None:
+            if n_envs % self.n_nets:
+                raise ValueError(f"n_envs ({n_envs}) must be a multiple of n_nets ({self.n_nets})")
+            net_of_env = [g // (n_envs // self.n_nets) for g in range(n_envs)]
+        #: the network of every environment (host list) and each network's environments
+        self.net_table = check_net_table(net_of_env, self.n_nets, n_envs)
+        self.net_envs = [[g for g, k in enumerate(self.net_table) if k == j] for j in range(self.n_nets)]
         # actor_refine / actor_qp / u_ref_qp: a copy of the CBF, its prepared planes (actor_refine) and the settings
         # (set_cbf_params)
         self.cbf_params: Optional[NetParams] = None
@@ -139,6 +186,7 @@ class RolloutEngine:
             if (policy == "actor" and self.use_tc) else 0
         ok = level > 0
         self._persistent_requested = persistent is True   # an explicit request, not the default choice below
+        self._persistent_arg = persistent                 # what each per-network engine of a sequential path gets
         if persistent is None:
             # default only where every environment's cluster is resident at once (level 2): otherwise the environments
             # beyond the resident clusters run in a second round
@@ -147,7 +195,10 @@ class RolloutEngine:
             # (step 0); from the first step with v != 0 a few policy outputs differ by 1-2 ulp (1.8e-7) -- the
             # (v cos th, v sin th) edge features are evaluated in two translation units -- which the closed loop
             # amplifies to 1.6e-5 after 24 steps.  Env-sharded runs must not mix two numeric paths.
-            persistent = (level == 2 and env.ENV_ID != "DubinsCar" and os.environ.get("GCBF_PERSISTENT", "1") != "0")
+            # Several networks take the persistent kernel at level 1 as well: gcbf_rollout_persistent_multi then runs the
+            # clusters beyond the resident ones in later rounds, which is still one launch instead of one per network.
+            persistent = (level >= (2 if self.n_nets == 1 else 1) and env.ENV_ID != "DubinsCar"
+                          and os.environ.get("GCBF_PERSISTENT", "1") != "0")
         if persistent and not ok:
             raise ValueError("persistent rollout unsupported for this configuration (2-D env, n <= 512, tensor-core path, "
                              "actor policy)")
@@ -167,11 +218,32 @@ class RolloutEngine:
         self._graph: Optional[torch.cuda.CUDAGraph] = None
         self.launches_per_run = 0
         self._obstacle_obj = None
+        if self.n_nets > 1:
+            # the network table on the device, the per-network step counters, and -- on the persistent path -- the
+            # stacked weights of gcbf_rollout_persistent_multi ([n_nets, stride] each; strides from the library)
+            self._net_of_env = torch.tensor(self.net_table, dtype=i32, device=dev)
+            self._net_counters = torch.zeros(T + 1, self.n_nets, 4, dtype=i32, device=dev)
+            ps, ist = C.c_int64(), C.c_int64()
+            _lib.check(env.lib.gcbf_rollout_persistent_multi_strides(env.edge_dim, nu, C.byref(ps), C.byref(ist)),
+                       "gcbf_rollout_persistent_multi_strides")
+            self._strides = (int(ps.value), int(ist.value))
+            self._multi_persistent = self.persistent    # the path one-layer actors take
+            self._subs: Optional[list] = None            # the per-network engines of the sequential path
+            if self.persistent:
+                self.params_buf = torch.zeros(self.n_nets, self._strides[0], dtype=f32, device=dev)
+                self.infer_blob = torch.zeros(self.n_nets, self._strides[1], dtype=f32, device=dev)
 
     @property
     def counters(self) -> torch.Tensor:
         """[T+1, 4] int32 record: per step total edge count (col 0) and overflow flag (col 1)."""
+        if self.n_nets > 1:
+            c = self._net_counters
+            return torch.cat([c[:, :, :1].sum(dim=1, dtype=torch.int32), c[:, :, 1:].amax(dim=1)], dim=1)
         return self.chains[0].counters
+
+    def net_counters(self, k: int) -> torch.Tensor:
+        """[T+1, 4] int32 record of network k's environments (the engine's counters when n_nets = 1)."""
+        return self._net_counters[:, k] if self.n_nets > 1 else self.chains[0].counters
 
     # ------------------------------------------------------------------ one env step (enqueue only)
     def _build(self, ch: _Chain, t: int, stream: int) -> None:
@@ -284,6 +356,15 @@ class RolloutEngine:
 
     def _enqueue_persistent(self, n_steps: int, stream: int) -> None:
         env, ch = self.env, self.chains[0]
+        if self.n_nets > 1:
+            rc = env.lib.gcbf_rollout_persistent_multi(
+                C.byref(self._pdesc), int(n_steps), self.n_nets, self.params_buf.data_ptr(), self.infer_blob.data_ptr(),
+                self._net_of_env.data_ptr(), self.goal.data_ptr(), self.obstacles.data_ptr() if self.O > 0 else None,
+                env.ray_table.data_ptr(), self.agent.data_ptr(), self.hits.data_ptr(), self.actions.data_ptr(),
+                self.rewards.data_ptr(), self.costs.data_ptr(), self._net_counters.data_ptr(), self._pws.data_ptr(),
+                self._pws.numel(), self.phase_stamps.data_ptr() if self.phase_stamps is not None else None, stream)
+            _lib.check(rc, "gcbf_rollout_persistent_multi")
+            return
         rc = env.lib.gcbf_rollout_persistent(
             C.byref(self._pdesc), int(n_steps), self.params_buf.data_ptr(), self.infer_blob.data_ptr(), self.goal.data_ptr(),
             self.obstacles.data_ptr() if self.O > 0 else None, env.ray_table.data_ptr(), self.agent.data_ptr(),
@@ -343,7 +424,14 @@ class RolloutEngine:
         ch.ws = torch.empty(int(env.lib.gcbf_rollout_workspace_floats_l(C.byref(ch.desc), n_layers)),
                             dtype=torch.float32, device=dev)
 
-    def set_params(self, params: NetParams) -> None:
+    def set_params(self, params) -> None:
+        """The actor: one NetParams, or a list of n_nets of them (network k runs the environments net_envs[k]).  The
+        parameters are COPIED: after they change, call set_params again."""
+        if self.n_nets > 1:
+            self._set_nets(check_nets(params, self.n_nets))
+            return
+        if not isinstance(params, NetParams):
+            params = check_nets(params, 1)[0]
         if params.n_layers != self.n_layers:
             self._set_depth(params.n_layers)
         self.params_buf.copy_(params.flat, non_blocking=True)
@@ -356,11 +444,55 @@ class RolloutEngine:
         _lib.check(env.lib.gcbf_prepare_infer(env.edge_dim, env.action_dim, _lib.ptr(self.params_buf),
                                               _lib.ptr(self.infer_blob), env._stream()), "gcbf_prepare_infer")
 
+    def _set_nets(self, nets: list) -> None:
+        env = self.env
+        depth = nets[0].n_layers
+        if depth > 1 and self._persistent_requested:
+            raise ValueError("the persistent rollout implements one GNN layer; these actors have %d" % depth)
+        self.n_layers = depth
+        self.persistent = self._multi_persistent and depth == 1
+        if not self.persistent:        # one solo engine per network, run one after another
+            if self._subs is None:
+                self._subs = [RolloutEngine(env, len(idx), T=self.T, n_obs=self.O, use_cuda_graph=self.use_cuda_graph,
+                                            policy=self.policy, persistent=self._persistent_arg)
+                              for idx in self.net_envs]
+            for sub, p in zip(self._subs, nets):
+                sub.set_params(p)
+            return
+        # stacked flat parameters and one gcbf_prepare_infer per network into the stacked blob
+        st = env._stream()
+        for k, p in enumerate(nets):
+            self.params_buf[k, :p.count].copy_(p.flat, non_blocking=True)
+            _lib.check(env.lib.gcbf_prepare_infer(env.edge_dim, env.action_dim, _lib.ptr(self.params_buf[k]),
+                                                  _lib.ptr(self.infer_blob[k]), st), "gcbf_prepare_infer")
+
+    def _run_subs(self, check: bool) -> None:
+        """Sequential path of several networks: network k's solo engine from its environments' initial conditions, then
+        its record gathered into this engine's."""
+        n = 0
+        for k, (sub, idx) in enumerate(zip(self._subs, self.net_envs)):
+            ix = torch.tensor(idx, dtype=torch.long, device=self.env.device)
+            sub.set_initial(self.agent[0, ix], self.goal[ix], self.obstacles[ix] if self.O > 0 else None)
+            sub.run(check=False)
+            n += sub.launches_per_run
+            for name in ("agent", "hits", "actions", "rewards", "costs"):
+                getattr(self, name).index_copy_(1, ix, getattr(sub, name))
+            self._net_counters[:, k].copy_(sub.counters)
+        self.launches_per_run = n
+        if check:
+            self.check_overflow()
+
     def run(self, check: bool = True) -> None:
         """Run the T-step rollout from the current initial conditions (async)."""
+        if self.n_nets > 1 and not self.persistent:
+            if self._subs is None:
+                raise RuntimeError("call set_params() before run()")
+            self._run_subs(check)
+            return
         dev = self.env.device
         ch = self.chains[0]
-        ch.counters.zero_()
+        counters = self._net_counters if self.n_nets > 1 else ch.counters
+        counters.zero_()
         lib = self.env.lib
         if self.use_cuda_graph:
             if self._graph is None:
@@ -368,7 +500,7 @@ class RolloutEngine:
                 st = torch.cuda.current_stream(dev).cuda_stream
                 if self.persistent:
                     self._enqueue_persistent(min(self.T, 1), st)
-                    ch.counters.zero_()
+                    counters.zero_()
                 else:
                     self._build(ch, 0, st)
                     self._step(ch, 0, st)
@@ -456,3 +588,16 @@ class RolloutEngine:
                        obstacle=self._obstacle_obj, actions=self.actions.transpose(0, 1),
                        rewards=self.rewards.transpose(0, 1), costs=self.costs.transpose(0, 1), dones=dones,
                        log_pis=None, n_edges=self.counters[:, 0])
+
+    def net_result(self, k: int) -> Rollout:
+        """result() restricted to network k's environments (net_envs[k], in environment order)."""
+        if self.n_nets == 1:
+            return self.result()
+        ix = torch.tensor(self.net_envs[k], dtype=torch.long, device=self.env.device)
+        ro = self.result()
+        obs = self._obstacle_obj
+        if obs is not None:
+            obs = obs.select(ix.cpu().numpy()) if hasattr(obs, "select") else obs[ix]
+        return Rollout(agent=ro.agent[ix], goal=ro.goal[ix], hits=ro.hits[ix], obstacle=obs, actions=ro.actions[ix],
+                       rewards=ro.rewards[ix], costs=ro.costs[ix], dones=ro.dones[ix], log_pis=None,
+                       n_edges=self._net_counters[:, k, 0])

@@ -262,6 +262,34 @@ int32_t gcbf_rollout_persistent(const gcbf_env_desc* desc, int32_t n_steps, cons
                                 const float* ray_table, float* agent_rec, float* hits_rec, float* actions_rec,
                                 float* rewards, float* costs, int32_t* counters, float* workspace,
                                 int64_t workspace_floats, uint64_t* phase_stamps, void* stream);
+/* The persistent rollout of several one-layer actors in ONE launch: environment g runs network net_of_env[g].  Each
+ * cluster reads its network once, at its start, and runs the operations of gcbf_rollout_persistent in the same order, so
+ * every network's environments get the bits a gcbf_rollout_persistent launch of that network alone gives them (the
+ * environments never read one another's data).
+ *   actor_params [n_nets, param_stride]: network k's flat parameters (gcbf_param_count_l(ed, nu, 1) floats) at
+ *   k * param_stride;  infer_blob [n_nets, infer_stride]: network k's gcbf_prepare_infer output (gcbf_infer_count(ed, nu)
+ *   floats) at k * infer_stride.  The strides are those counts rounded up to a multiple of 4 floats (16 bytes: the
+ *   stride of the 3-D weight tensor maps, network outermost); gcbf_rollout_persistent_multi_strides returns them.  Both
+ *   arrays 16-byte aligned.
+ *   net_of_env [G] int32 (device): every entry in [0, n_nets).  The library does not read it on the host; an entry out
+ *   of range is the caller's bug (undefined reads).
+ *   counters [n_steps+1, n_nets, 4] (zeroed by the caller): [t][k][0] += edges of the graphs of state t of network k's
+ *   environments, [t][k][1] |= their overflow.  Every other argument as gcbf_rollout_persistent (desc->n_graphs = G
+ *   counts the environments of all networks; workspace: gcbf_rollout_persistent_workspace_floats(desc)).
+ * Unlike gcbf_rollout_persistent it also launches when gcbf_rollout_persistent_supported(desc) is 1 and the pair mode
+ * does not fit the device: the clusters beyond the resident ones then run in later rounds (none waits on another).
+ * Rejected before anything is enqueued: n_nets < 1, a NULL net_of_env, misaligned stacked arrays, and whatever
+ * gcbf_rollout_persistent rejects. */
+int32_t gcbf_rollout_persistent_multi(const gcbf_env_desc* desc, int32_t n_steps, int32_t n_nets,
+                                      const float* actor_params, const float* infer_blob, const int32_t* net_of_env,
+                                      const float* goal, const float* obstacles, const float* ray_table,
+                                      float* agent_rec, float* hits_rec, float* actions_rec, float* rewards,
+                                      float* costs, int32_t* counters, float* workspace, int64_t workspace_floats,
+                                      uint64_t* phase_stamps, void* stream);
+/* Per-network strides (floats) of gcbf_rollout_persistent_multi's stacked actor_params / infer_blob for edge_dim /
+ * out_dim (one GNN layer).  0, or -1 for bad dimensions. */
+int32_t gcbf_rollout_persistent_multi_strides(int32_t edge_dim, int32_t out_dim, int64_t* param_stride,
+                                              int64_t* infer_stride);
 
 /* ---------------------------------------------------------------- labels / masks (a9)
  * Replaces env.unsafe_mask / collision_mask / finish_mask / safe_mask
