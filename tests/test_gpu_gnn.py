@@ -12,7 +12,10 @@ pytestmark = pytest.mark.gpu
 
 # strict-fp32 SIMT path: 1e-5 (SURVEY 8c).  wgmma 3xTF32 path: 3e-5 -- each of its GEMMs is within 2e-6 of |A||B| of
 # float64 (tests/test_gpu_train.py), the bar here leaves room for the rounding of 3*K/8 accumulated partial products per
-# output; the network-level error vs float64 is not measured.  Far inside the 2e-3 SURVEY 8c grants a tensor-core path.
+# output; tests/test_gpu_gnn_f64.py measures the network-level error vs float64 in units of fp32 rounding
+# (tests/gnn_f64.py): measured on an H100, <= 15 units on the SIMT path and up to 260 on the tensor-core path,
+# whose wgmma fp32 accumulation truncates (tests/gnn_f64.py::tc_dense reproduces it; each of its GEMMs stays within
+# GEMM_BAR units of its own inputs).  Far inside the 2e-3 SURVEY 8c grants a tensor-core path.
 TOL = {"simt": 1e-5, "tc": 3e-5}
 CASES = [("SingleIntegrator", 8, 3, 2.0, 4), ("DoubleIntegrator", 8, 4, 2.0, 8), ("DoubleIntegrator", 48, 2, 3.0, 8),
          ("DubinsCar", 12, 3, 2.5, 6), ("LinearDrone", 10, 2, 1.5, 4)]
