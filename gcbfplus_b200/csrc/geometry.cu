@@ -37,9 +37,9 @@ graph_build_kernel(const gcbf_env_desc d, const float* __restrict__ agent, const
     float* sobs = spos + N * PD;                // [O, OBS2]
     float* stab = sobs + O * OBS2;              // [n_rays, PD]
     float* salpha = stab + d.n_rays * PD;       // 3-D only: [GB_WARPS, n_rays]
-    const int n_words = (N + 31) / 32;
-    unsigned* sbits = reinterpret_cast<unsigned*>(salpha + (PD == 3 ? GB_WARPS * d.n_rays : 0));  // [GB_WARPS, n_words]
-    int* stk = reinterpret_cast<int*>(sbits + GB_WARPS * n_words);                                 // 3-D only: [GB_WARPS, 96] top-k scratch
+    const int n_words = (N + 31) / 32, bstride = n_words | 1;
+    unsigned* sbits = reinterpret_cast<unsigned*>(salpha + (PD == 3 ? GB_WARPS * d.n_rays : 0));  // [GB_WARPS, bstride]
+    int* stk = reinterpret_cast<int*>(sbits + GB_WARPS * bstride);                                 // 3-D only: [GB_WARPS, 96] top-k scratch
     __shared__ int s_off[GB_WARPS + 1];
     __shared__ int s_base;
 
@@ -114,7 +114,8 @@ graph_build_kernel(const gcbf_env_desc d, const float* __restrict__ agent, const
     // A CTA serves `rounds` groups of GB_WARPS agents: at ~60 registers per thread one 1024-thread CTA fills an SM, so
     // the grid is sized to one wave (graph_build_impl) instead of paying the prologue (and the fused tail) per wave.
     for (int round = 0; round < rounds; ++round) {
-    const int i = (blockIdx.x * rounds + round) * GB_WARPS + warp;
+    const int i0 = (blockIdx.x * rounds + round) * GB_WARPS;   // first agent of the round
+    const int i = i0 + warp;
     const bool valid = i < N;
     const int ii = valid ? i : 0;
     float p[PD];
@@ -123,10 +124,16 @@ graph_build_kernel(const gcbf_env_desc d, const float* __restrict__ agent, const
     const size_t a_glob = (size_t)g * N + ii;
     float* my_hits = hits + a_glob * R * PD;
 
+    // ---------------- neighbour words of the round's agents (thread per (word, agent)); independent of the LiDAR, so
+    // the two overlap across warps.  The words stay in shared memory for the count and the fill pass.
+    neighbour_words<PD, PD>(d, spos, i0, max(0, min(GB_WARPS, N - i0)), sbits, bstride, tid, blockDim.x);
+
     // ---------------- LiDAR (env/utils.py:49-131)
+    float h[PD];   // hit `lane` of this agent (lanes < R)
+    const bool in_regs = PD == 2 && do_cast;
     if (do_cast && valid) {
         if (PD == 2) {
-            lidar2d_warp(p, stab, sobs, O, d.n_rays, R, lane, my_hits);
+            lidar2d_warp(p, stab, sobs, O, d.n_rays, R, lane, my_hits, h[0], h[1]);
         } else {
             const bool is_in = (O > 0) ? inside_any<PD>(sobs, O, p, 0.f) : false;
             const float keep = 1.f - (is_in ? 1.f : 0.f);
@@ -241,11 +248,14 @@ graph_build_kernel(const gcbf_env_desc d, const float* __restrict__ agent, const
     }
     __syncwarp();
 
-    // ---------------- active hit nodes and neighbours; the ballots are kept in shared memory for the fill pass
-    const unsigned hit_bits = active_hit_bits<PD>(d, p, my_hits, lane, valid);
-    int cnt = 0;
-    unsigned* my_bits = sbits + warp * n_words;
-    if (valid) cnt = neighbour_bits<PD, PD>(d, p, i, spos, lane, my_bits);
+    // ---------------- active hit nodes (2-D cast: the hits are still in registers; otherwise read back) and degrees
+    if (!in_regs && valid && lane < R)
+#pragma unroll
+        for (int c = 0; c < PD; ++c) h[c] = my_hits[lane * PD + c];
+    const unsigned hit_bits = active_hit_bits<PD>(d, p, h, lane, valid);
+    __syncthreads();   // the round's neighbour words are complete
+    unsigned* my_bits = sbits + warp * bstride;
+    const int cnt = valid ? word_count(my_bits, n_words, lane) : 0;
     const int deg = valid ? (1 + cnt + __popc(hit_bits)) : 0;
     if (lane == 0) s_off[warp + 1] = deg;
     __syncthreads();
@@ -591,7 +601,8 @@ int32_t gcbf::graph_build_impl(const gcbf_env_desc* desc, const float* agent, co
     const int obw = pd == 2 ? 16 : 4;
     const size_t smem = sizeof(float) * ((size_t)desc->n_agents * pd + (size_t)desc->n_obs * (pd == 2 ? 24 : 4) +
                                          (size_t)desc->n_rays * pd + (pd == 3 ? (size_t)GB_WARPS * desc->n_rays : 0) +
-                                         (size_t)GB_WARPS * ((desc->n_agents + 31) / 32) + (pd == 3 ? (size_t)GB_WARPS * 96 : 0));
+                                         (size_t)GB_WARPS * (((desc->n_agents + 31) / 32) | 1) +
+                                         (pd == 3 ? (size_t)GB_WARPS * 96 : 0));
     GCBF_REQUIRE(smem <= 200 * 1024, "graph_build needs %zu B shared memory (> 200 KB): too many agents/obstacles", smem);
     if (!(flags & 4)) {   // bit 2: the caller's previous kernel already cleared counters[0]
         cudaError_t e = cudaMemsetAsync(counters, 0, sizeof(int32_t), st);

@@ -88,14 +88,15 @@ __device__ __forceinline__ float sphere_raytrace(const float* ob, float x1, floa
     return valid1 * alphas + (1.f - valid1) * NO_HIT;
 }
 
-// inside_obstacles (env/utils.py:82-107) for one point against the graph's obstacle set.
-template <int PD>
+// inside_obstacles (env/utils.py:82-107) for one point against the graph's obstacle set; obstacle o at sobs + OSTRIDE o
+// (packed rows by default; OBS2D for the shared-memory rows of the graph build).
+template <int PD, int OSTRIDE = (PD == 2 ? 16 : 4)>
 __device__ __forceinline__ bool inside_any(const float* sobs, int O, const float* p, float r) {
     bool in = false;
     if (PD == 2) {
-        for (int o = 0; o < O; ++o) in = in || rect_inside(sobs + 16 * o, p[0], p[1], r);
+        for (int o = 0; o < O; ++o) in = in || rect_inside(sobs + OSTRIDE * o, p[0], p[1], r);
     } else {
-        for (int o = 0; o < O; ++o) in = in || sphere_inside(sobs + 4 * o, p[0], p[1], p[2], r);
+        for (int o = 0; o < O; ++o) in = in || sphere_inside(sobs + OSTRIDE * o, p[0], p[1], p[2], r);
     }
     return in;
 }
@@ -328,9 +329,10 @@ __device__ __forceinline__ void derive_far_fields(float* sobs, int O, float comm
 }
 
 // 2-D LiDAR (env/utils.py:49-131) of the agent at p, one ray per lane: the R closest returns in stable argsort order
-// -> my_hits[R][2].  sobs: O obstacle rows of OBS2D floats (derive_far_fields), stab: [n_rays][2] ray offsets.
+// -> my_hits[R][2], and lane r < R also returns hit r in (hx, hy), so that the active-hit test need not read the
+// global store back.  sobs: O obstacle rows of OBS2D floats (derive_far_fields), stab: [n_rays][2] ray offsets.
 __device__ __forceinline__ void lidar2d_warp(const float* p, const float* stab, const float* sobs, int O, int n_rays,
-                                             int R, int lane, float* my_hits) {
+                                             int R, int lane, float* my_hits, float& hx_out, float& hy_out) {
     const bool ray_ok = lane < n_rays;
     const int rl = ray_ok ? lane : 0;
     const float x1 = p[0], y1 = p[1];
@@ -380,18 +382,21 @@ __device__ __forceinline__ void lidar2d_warp(const float* p, const float* stab, 
         my_hits[lane * 2 + 0] = shx;
         my_hits[lane * 2 + 1] = shy;
     }
+    hx_out = shx;
+    hy_out = shy;
 }
 
-// active hit nodes: ||p - hit|| < comm_radius - 0.1 (double_integrator.py:254-257); bit r = hit r (ballot, lane r)
+// active hit nodes: ||p - hit|| < comm_radius - 0.1 (double_integrator.py:254-257); bit r = hit r (ballot, lane r).
+// h: hit `lane` (read only on lanes < n_hits).
 template <int PD>
-__device__ __forceinline__ unsigned active_hit_bits(const gcbf_env_desc& d, const float* p, const float* my_hits, int lane,
+__device__ __forceinline__ unsigned active_hit_bits(const gcbf_env_desc& d, const float* p, const float* h, int lane,
                                                     bool valid) {
     bool act = false;
     if (valid && lane < d.n_hits) {
         float acc = 0.f;
 #pragma unroll
         for (int c = 0; c < PD; ++c) {
-            const float dlt = p[c] - my_hits[lane * PD + c];
+            const float dlt = p[c] - h[c];
             acc = (c == 0) ? dlt * dlt : acc + dlt * dlt;
         }
         act = acc < d.lidar_sq_thr;   // == (sqrtf(acc) < lidar_radius), threshold precomputed exactly on the host
@@ -399,55 +404,67 @@ __device__ __forceinline__ unsigned active_hit_bits(const gcbf_env_desc& d, cons
     return __ballot_sync(0xffffffffu, act);
 }
 
-// neighbours of agent i: ||p_i - p_j|| < comm_radius, j != i (double_integrator.py:227-232), j's position at
-// pos + j * STRIDE.  sqrtf(acc) < Rc  <=>  acc < d.comm_sq_thr (smallest fp32 whose correctly rounded sqrt is >= Rc;
-// host-computed), so the scan needs no sqrt.  Writes one ballot word per 32 candidates to my_bits (lane 0) and
-// returns the neighbour count.  Full words run without the per-lane range / self tests (the self bit is cleared after
-// the ballot), unrolled x4: this scan was 40 % of graph_build_kernel's instructions.
+// Neighbour words of the n agents i0 .. i0 + n - 1 of a graph: ||p_i - p_j|| < comm_radius, j != i
+// (double_integrator.py:227-232), agent j's position at pos + j * STRIDE.  Word w of agent i0 + s goes to
+// bits[s * bstride + w], bit b = candidate 32 w + b.  sqrtf(acc) < Rc  <=>  acc < d.comm_sq_thr (smallest fp32 whose
+// correctly rounded sqrt is >= Rc; host-computed), so the scan needs no sqrt.
+// One thread per (word, agent), tasks tid, tid + nthreads, ...: consecutive threads take consecutive agents of the same
+// word, so each candidate load is a shared-memory broadcast, and every thread runs an independent 32-candidate chain
+// (no ballot, no warp-wide dependence).  An odd bstride keeps the word stores of 32 consecutive agents conflict-free.
 template <int PD, int STRIDE>
-__device__ __forceinline__ int neighbour_bits(const gcbf_env_desc& d, const float* p, int i, const float* pos, int lane,
-                                              unsigned* my_bits) {
-    const int N = d.n_agents;
-    int cnt = 0;
-    const int n_full = N >> 5;
-#pragma unroll 4
-    for (int w = 0; w < n_full; ++w) {
-        const int j = (w << 5) + lane;
-        float acc;
-        if (PD == 2) {
-            const float2 q = *reinterpret_cast<const float2*>(pos + j * STRIDE);
-            const float dx = p[0] - q.x, dy = p[1] - q.y;
-            acc = dx * dx;
-            acc = acc + dy * dy;
+__device__ __forceinline__ void neighbour_words(const gcbf_env_desc& d, const float* pos, int i0, int n, unsigned* bits,
+                                                int bstride, int tid, int nthreads) {
+    const int N = d.n_agents, n_words = (N + 31) >> 5;
+    const float thr = d.comm_sq_thr;
+    for (int task = tid; task < n * n_words; task += nthreads) {
+        const int w = task / n, s = task - w * n;
+        const int i = i0 + s;
+        float p[PD];
+#pragma unroll
+        for (int c = 0; c < PD; ++c) p[c] = pos[i * STRIDE + c];
+        const float* q = pos + (w << 5) * STRIDE;
+        unsigned word = 0u;
+        if ((w << 5) + 32 <= N) {
+#pragma unroll
+            for (int b = 0; b < 32; ++b) {
+                float acc;
+                if (PD == 2) {
+                    const float2 qq = *reinterpret_cast<const float2*>(q + b * STRIDE);
+                    const float dx = p[0] - qq.x, dy = p[1] - qq.y;
+                    acc = dx * dx;
+                    acc = acc + dy * dy;
+                } else {
+#pragma unroll
+                    for (int c = 0; c < PD; ++c) {
+                        const float dlt = p[c] - q[b * STRIDE + c];
+                        acc = (c == 0) ? dlt * dlt : acc + dlt * dlt;
+                    }
+                }
+                word |= (acc < thr ? 1u : 0u) << b;
+            }
         } else {
-            acc = 0.f;
+            const int nb = N - (w << 5);
+            for (int b = 0; b < nb; ++b) {
+                float acc;
 #pragma unroll
-            for (int c = 0; c < PD; ++c) {
-                const float dlt = p[c] - pos[j * STRIDE + c];
-                acc = (c == 0) ? dlt * dlt : acc + dlt * dlt;
+                for (int c = 0; c < PD; ++c) {
+                    const float dlt = p[c] - q[b * STRIDE + c];
+                    acc = (c == 0) ? dlt * dlt : acc + dlt * dlt;
+                }
+                word |= (acc < thr ? 1u : 0u) << b;
             }
         }
-        unsigned bits = __ballot_sync(0xffffffffu, acc < d.comm_sq_thr);
-        if (w == (i >> 5)) bits &= ~(1u << (i & 31));
-        if (lane == 0) my_bits[w] = bits;
-        cnt += __popc(bits);
+        if (w == (i >> 5)) word &= ~(1u << (i & 31));
+        bits[s * bstride + w] = word;
     }
-    if (N & 31) {
-        const int j = (n_full << 5) + lane;
-        bool ok = false;
-        if (j < N && j != i) {
-            float acc = 0.f;
+}
+
+// neighbour count of one agent from its words (warp-wide; every lane returns it)
+__device__ __forceinline__ int word_count(const unsigned* my_bits, int n_words, int lane) {
+    int cnt = 0;
+    for (int w = lane; w < n_words; w += 32) cnt += __popc(my_bits[w]);
 #pragma unroll
-            for (int c = 0; c < PD; ++c) {
-                const float dlt = p[c] - pos[j * STRIDE + c];
-                acc = (c == 0) ? dlt * dlt : acc + dlt * dlt;
-            }
-            ok = acc < d.comm_sq_thr;
-        }
-        const unsigned bits = __ballot_sync(0xffffffffu, ok);
-        if (lane == 0) my_bits[n_full] = bits;
-        cnt += __popc(bits);
-    }
+    for (int o = 16; o > 0; o >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
     return cnt;
 }
 

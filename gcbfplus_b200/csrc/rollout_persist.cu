@@ -13,13 +13,14 @@
 //   A   warp per receiver: segment softmax + weighted aggregate                                             [gnn.cuh aggregate_logits]
 //   U1  (agent tile, column half) items: update layer 128->256, bias + one-hot row, ReLU                   [gemm_tc.cuh EPI_BIAS_RELU]
 //   U2  same items: folded update/head layer 256->256, ReLU, output-layer partial sums                      [gemm_tc.cuh EPI_RELU_DOTN]
-//   G   policy tail (tanh, a = 2 pi + u_ref, clip, Euler; record action / next state / reward / cost) + LiDAR +
-//       stable top-k + radius neighbour lists of the next state, rows laid out in agent order through a
+//   G   policy tail (tanh, a = 2 pi + u_ref, clip, Euler; record action / next state / reward / cost terms of the
+//       CTA's own agents) + LiDAR + stable top-k + radius neighbour lists of the next state, rows laid out in agent order through a
 //       CTA-local prefix sum and a cluster-wide exchange of the CTA totals over distributed shared memory    [geometry_dev.cuh]
 // The phases call the device functions the 5-launch kernels call (GEMM main loops and epilogues; aggregate; policy
 // tail, LiDAR, neighbour scan and row fill), so the two paths give the same bits (tests/test_gpu_rollout.py).  What
 // differs stays here: the edge-row limit of a local group, the row base from the prefix over the cluster, and that
-// only the environment's first CTA records.  This translation unit is
+// each CTA records its own agents (the environment's first CTA reduces their reward / cost terms one step later, after
+// the environment barrier).  This translation unit is
 // compiled with -fmad=false like geometry.cu (the LiDAR / dynamics code must keep one rounding per operation); the
 // GEMM-side code uses explicit fmaf wherever the other translation units rely on contraction.
 //
@@ -74,6 +75,7 @@ struct PArgs {
     // per-environment scratch (L2)
     int32_t *row_start, *row_deg, *edge_recv, *edge_src; // [2][...] double-buffered lists
     float *msg, *logit, *ag, *v1, *z;
+    float* terms;                                        // [2][A][4] per-agent reward / cost terms, by step parity
     unsigned long long* prof;                            // optional [T + 1][8] %globaltimer stamps of cluster 0 / CTA 0 (ns)
     // mode 0: one hardware cluster of C CTAs per environment (every barrier is barrier.cluster).
     // mode 1 ("pairs"): when fewer clusters of C CTAs than environments are resident (BASELINE's config has 16
@@ -141,8 +143,8 @@ rollout_persist_kernel(const __grid_constant__ PArgs P, const __grid_constant__ 
     float* sst = sW + 7 * 256;                                             // [N][SD] states of all agents of the environment
     float* sobs = sst + MAX_N * 4;                                         // [O][24]
     float* stab = sobs + MAX_OBS * OBS2;                                   // [32][2]
-    unsigned* sbits = reinterpret_cast<unsigned*>(stab + 64);              // [APC][n_words]
-    int* s_off = reinterpret_cast<int*>(sbits + 64 * 16);                  // [APC + 1]
+    unsigned* sbits = reinterpret_cast<unsigned*>(stab + 64);              // [APC][n_words | 1] neighbour words
+    int* s_off = reinterpret_cast<int*>(sbits + 64 * 17);                  // [APC + 1]
     unsigned* s_hb = reinterpret_cast<unsigned*>(s_off + 72);              // [APC]
     float* s_red = reinterpret_cast<float*>(s_hb + 64);                    // [3][PW]
     float* sk = s_red + 3 * PW;                                            // [K_FLOATS] rollout constants
@@ -433,12 +435,28 @@ rollout_persist_kernel(const __grid_constant__ PArgs P, const __grid_constant__ 
                 }
             } else {
                 // fused policy tail (geometry.cu graph_build_kernel): every CTA recomputes the next state of all N
-                // agents into its position table; the cluster's first CTA records and reduces reward / cost
-                const bool rec = rank == 0;
+                // agents into its position table and records its own agents [a_lo, a_hi): action, next state and the
+                // per-agent reward / cost terms (terms, by step parity).  The environment's first CTA reduces the terms
+                // of step t - 1 in the same loop, with reduce_reward_cost's thread -> agent mapping.
+                // Ordering: the owners wrote those terms, and the next states agent_t that collides_prev reads, in
+                // phase G of step t - 1 (t = 0: agent_t is the initial state).  The environment barrier at the end of
+                // this step's U2 (barrier.cluster release / acquire in mode 0; gpu-scope fences around the arrival
+                // counter in pair mode) makes them visible here.  Terms of step t go to the other parity half.  The
+                // half read here is rewritten in phase G of step t + 1, after that step's environment barrier, which
+                // the first CTA reaches only after this reduce.
+                const bool red = rank == 0 && t > 0;
                 float acc[3] = {0.f, 0.f, 0.f};
                 float* act_t = P.actions + (size_t)t * A_tot * NU;
+                float* terms_t = P.terms + (size_t)(t & 1) * A_tot * 4;
                 for (int i = tid; i < N; i += PT) {
                     const size_t a = (size_t)env_a0 + i;
+                    if (red) {
+                        const float4 v = *reinterpret_cast<const float4*>(P.terms + ((size_t)((t - 1) & 1) * A_tot + a) * 4);
+                        acc[0] += v.x;
+                        acc[1] += v.y;
+                        acc[2] += v.z;
+                    }
+                    const bool own = i >= a_lo && i < a_hi;
                     float zz[4] = {0.f, 0.f, 0.f, 0.f};
                     const float* z_t = P.z + (size_t)(t & 1) * 2 * A_tot * 4;
                     for (int p = 0; p < 2; ++p) {
@@ -452,58 +470,55 @@ rollout_persist_kernel(const __grid_constant__ PArgs P, const __grid_constant__ 
                         gl[c] = P.goal[a * SD + c];
                     }
                     policy_action<KIND>(d, x, gl, zz, sk + K_BHO, ur, act);
-                    if (rec)
+                    if (own)
 #pragma unroll
                         for (int c = 0; c < NU; ++c) act_t[a * NU + c] = act[c];
                     const float sq = step_agent<KIND>(d, x, gl, act, ur, true, xn);
 #pragma unroll
                     for (int c = 0; c < SD; ++c) sst[i * SD + c] = xn[c];
-                    if (rec) {
+                    if (own) {
 #pragma unroll
                         for (int c = 0; c < SD; ++c) agent_n[a * SD + c] = xn[c];
                         const float nr = sqrtf(sq);
+                        // the agent's own row of the graph of state t was filled by this CTA (phase G of step t - 1)
                         const bool col = collides_prev<PD, SD>(x, rs_t[a], rd_t[a], es_t + env_e0, agent_t, d.two_r);
-                        bool in_obs = false;
-                        if (O > 0) {
-                            const float* ob = P.obstacles + (d.obs_per_graph ? (size_t)env * O * OBW : 0);
-                            in_obs = inside_any<PD>(ob, O, x, d.radius);
-                        }
-                        acc[0] += nr * nr;
-                        acc[1] += col ? 1.f : 0.f;
-                        acc[2] += in_obs ? 1.f : 0.f;
+                        const bool in_obs = O > 0 && inside_any<PD, OBS2>(sobs, O, x, d.radius);
+                        *reinterpret_cast<float4*>(terms_t + a * 4) =
+                            make_float4(nr * nr, col ? 1.f : 0.f, in_obs ? 1.f : 0.f, 0.f);
                     }
                 }
-                if (rec) reduce_reward_cost<PW>(acc, s_red, N, P.rewards + (size_t)t * E + env, P.costs + (size_t)t * E + env);
+                if (red)
+                    reduce_reward_cost<PW>(acc, s_red, N, P.rewards + (size_t)(t - 1) * E + env,
+                                           P.costs + (size_t)(t - 1) * E + env);
             }
             __syncthreads();
             if (stamp) pr[5] = gtime();
 
-            // ---- LiDAR + neighbour bits for this CTA's agents (warp per agent, PW agents per round)
+            // ---- neighbour words (thread per (word, agent)) and LiDAR + active hit bits (warp per agent) of this
+            // CTA's agents.  The words do not depend on the LiDAR, so the two overlap across warps.
             const int n_slots = a_hi - a_lo;
-            for (int slot0 = 0; slot0 < APC; slot0 += PW) {
-                const int slot = slot0 + warp;
+            const int bstride = n_words | 1;
+            neighbour_words<PD, SD>(d, sst, a_lo, n_slots, sbits, bstride, tid, PT);
+            for (int slot = warp; slot < n_slots; slot += PW) {
                 const int i = a_lo + slot;
-                const bool valid = slot < n_slots;
-                const int ii = valid ? i : 0;
-                float p[PD];
+                float p[PD], h[PD];
 #pragma unroll
-                for (int c = 0; c < PD; ++c) p[c] = sst[ii * SD + c];
-                const size_t a_glob = (size_t)env_a0 + ii;
-                float* my_hits = hits_n + a_glob * R * PD;
-                if (valid) lidar2d_warp(p, stab, sobs, O, d.n_rays, R, lane, my_hits);
-                __syncwarp();
-                const unsigned hit_bits = active_hit_bits<PD>(d, p, my_hits, lane, valid);
-                int cnt = 0;
-                if (valid) cnt = neighbour_bits<PD, SD>(d, p, i, sst, lane, sbits + slot * n_words);
-                if (lane == 0 && slot < APC) {
-                    s_off[slot + 1] = valid ? (1 + cnt + __popc(hit_bits)) : 0;
-                    s_hb[slot] = hit_bits;
-                }
+                for (int c = 0; c < PD; ++c) p[c] = sst[i * SD + c];
+                float* my_hits = hits_n + ((size_t)env_a0 + i) * R * PD;
+                lidar2d_warp(p, stab, sobs, O, d.n_rays, R, lane, my_hits, h[0], h[1]);
+                const unsigned hit_bits = active_hit_bits<PD>(d, p, h, lane, true);
+                if (lane == 0) s_hb[slot] = hit_bits;
             }
             __syncthreads();
-            if (warp == 0) {                     // exclusive prefix of the (<= 64) row degrees, agent order
-                int v0 = (lane < APC) ? s_off[lane + 1] : 0;
-                int v1 = (lane + 32 < APC) ? s_off[lane + 33] : 0;
+            if (warp == 0) {                     // row degrees 1 + neighbours + active hits, their exclusive prefix (<= 64 rows)
+                auto degree = [&](int slot) {
+                    if (slot >= n_slots) return 0;
+                    int c = 1 + __popc(s_hb[slot]);
+                    for (int w = 0; w < n_words; ++w) c += __popc(sbits[slot * bstride + w]);
+                    return c;
+                };
+                int v0 = degree(lane);
+                int v1 = degree(lane + 32);
                 int inc0 = v0, inc1 = v1;
 #pragma unroll
                 for (int o = 1; o < 32; o <<= 1) {
@@ -551,12 +566,27 @@ rollout_persist_kernel(const __grid_constant__ PArgs P, const __grid_constant__ 
                     rs_n[a_id] = rbase;
                     rd_n[a_id] = deg;
                 }
-                fill_row(er_n + env_e0, es_n + env_e0, rbase, a_id, env_a0, sbits + slot * n_words, n_words, s_hb[slot], lane);
+                fill_row(er_n + env_e0, es_n + env_e0, rbase, a_id, env_a0, sbits + slot * bstride, n_words, s_hb[slot], lane);
             }
             if (lrank == 0 && tid == 0) atomicAdd(&P.counters[((size_t)tn * P.n_nets + net()) * 4 + 0], min(env_total, seg_cap));
             M_cur = min(env_total, seg_cap);
             SYNC_LOCAL();
             if (stamp) pr[7] = gtime();
+        }
+    }
+    // reward / cost of the last step: its owners wrote the terms in the last phase G
+    if (P.T > 0) {
+        SYNC_ENV((unsigned)P.T + 1u);
+        if (rank == 0) {
+            const int t = P.T - 1;
+            float acc[3] = {0.f, 0.f, 0.f};
+            for (int i = tid; i < N; i += PT) {
+                const float4 v = *reinterpret_cast<const float4*>(P.terms + ((size_t)(t & 1) * A_tot + env_a0 + i) * 4);
+                acc[0] += v.x;
+                acc[1] += v.y;
+                acc[2] += v.z;
+            }
+            reduce_reward_cost<PW>(acc, s_red, N, P.rewards + (size_t)t * E + env, P.costs + (size_t)t * E + env);
         }
     }
 #undef SYNC_LOCAL
@@ -565,7 +595,7 @@ rollout_persist_kernel(const __grid_constant__ PArgs P, const __grid_constant__ 
 }
 
 struct WsLayout {
-    int64_t msg, logit, ag, v1, z, row_start, row_deg, edge_recv, edge_src, gbar, total;
+    int64_t msg, logit, ag, v1, z, terms, row_start, row_deg, edge_recv, edge_src, gbar, total;
 };
 static WsLayout make_ws_layout(int E, int N, int cap_env) {   // (+ 16 (T + 1) floats of phase stamps appended by the caller)
     WsLayout W;
@@ -577,6 +607,7 @@ static WsLayout make_ws_layout(int E, int N, int cap_env) {   // (+ 16 (T + 1) f
     W.ag = take(A * 128 + 128 * 128);      // + one tile of slack: the last environment's row tile may overhang
     W.v1 = take(A * 256 + 128 * 256);
     W.z = take(2 * 2 * A * 4);             // [step parity][column half][A][4]
+    W.terms = take(2 * A * 4);             // [step parity][A][||u - u_ref||^2, collides, inside an obstacle, 0]
     W.row_start = take(2 * A);
     W.row_deg = take(2 * A);
     W.edge_recv = take(2 * EC);
@@ -630,7 +661,7 @@ extern "C" __attribute__((visibility("default"))) int32_t gcbf_rollout_persisten
 }
 
 static int persist_smem_bytes() {
-    return 3 * rp::STG + 512 + 7 * 256 * 4 + rp::MAX_N * 4 * 4 + rp::MAX_OBS * 24 * 4 + 64 * 4 + 64 * 16 * 4 + 72 * 4 + 64 * 4 +
+    return 3 * rp::STG + 512 + 7 * 256 * 4 + rp::MAX_N * 4 * 4 + rp::MAX_OBS * 24 * 4 + 64 * 4 + 64 * 17 * 4 + 72 * 4 + 64 * 4 +
            3 * rp::PW * 4 + rp::K_FLOATS * 4 + 1024;
 }
 
@@ -747,6 +778,7 @@ static int32_t persist_launch(const char* who, bool rounds, const gcbf_env_desc*
     P.ag = workspace + W.ag;
     P.v1 = workspace + W.v1;
     P.z = workspace + W.z;
+    P.terms = workspace + W.terms;
     P.row_start = reinterpret_cast<int32_t*>(workspace + W.row_start);
     P.row_deg = reinterpret_cast<int32_t*>(workspace + W.row_deg);
     P.edge_recv = reinterpret_cast<int32_t*>(workspace + W.edge_recv);
