@@ -278,7 +278,11 @@ graph_build_kernel(const gcbf_env_desc d, const float* __restrict__ agent, const
             row_start[a_id] = base;
             row_deg[a_id] = deg;
         }
-        fill_row(edge_recv, edge_src, base, a_id, g * N, my_bits, n_words, hit_bits, lane);
+        const int rb[1] = {base}, ai[1] = {a_id};
+        const bool ok[1] = {true};
+        const unsigned* const mb[1] = {my_bits};
+        const unsigned hb[1] = {hit_bits};
+        fill_row<1>(edge_recv, edge_src, rb, ai, ok, g * N, mb, n_words, hb, lane);
     }
     __syncthreads();   // s_off / s_base / the per-warp scratch are reused by the next round
     }

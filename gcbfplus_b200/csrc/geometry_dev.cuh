@@ -284,6 +284,16 @@ __device__ __forceinline__ bool collides_prev(const float* x, int rs, int rd, co
     return col;
 }
 
+// Smallest fp32 a whose correctly rounded sqrtf is >= r, so that (sqrtf(x) < r) == (x < a) and (r > sqrtf(x)) ==
+// (x < a) for every fp32 x (NaN: both false).  The device twin of _lib.sqrt_threshold, which the host uses for
+// comm_sq_thr / lidar_sq_thr; r <= 0 gives 0, which no x is below.
+__device__ __forceinline__ float sqrt_threshold(float r) {
+    float a = r * r;
+    while (a > 0.f && sqrtf(a) >= r) a = nextafterf(a, 0.f);
+    while (sqrtf(a) < r) a = nextafterf(a, INFINITY);
+    return a;
+}
+
 // Reward and cost of one graph from per-thread sums acc = [sum ||u - u_ref||^2, #colliding, #inside an obstacle]:
 // warp sums, then thread 0 adds the NW warp sums in warp order.  Warps without agents add +0, so CTAs of different
 // widths give the same bits.  Every thread of the CTA calls it.
@@ -309,7 +319,8 @@ __device__ __forceinline__ void reduce_reward_cost(const float* acc, float* s_re
 }
 
 // ------------------------------------------------------------------------------------
-// graph build of one agent per warp (graph_build_kernel and the persistent rollout kernel)
+// graph build of one agent per warp (graph_build_kernel and the persistent rollout kernel; the persistent kernel fills
+// FILL_NA rows per warp at once)
 // ------------------------------------------------------------------------------------
 // 2-D obstacle rows in shared memory are 24 floats: the packed rectangle, then the derived fields of the far-obstacle
 // skip at [14] reach^2, [15..18] edge dx, [19..22] edge dy.
@@ -411,9 +422,13 @@ __device__ __forceinline__ unsigned active_hit_bits(const gcbf_env_desc& d, cons
 // One thread per (word, agent), tasks tid, tid + nthreads, ...: consecutive threads take consecutive agents of the same
 // word, so each candidate load is a shared-memory broadcast, and every thread runs an independent 32-candidate chain
 // (no ballot, no warp-wide dependence).  An odd bstride keeps the word stores of 32 consecutive agents conflict-free.
-template <int PD, int STRIDE>
+// COL: also set col[s] = 1 when some other agent j has acc < col_thr (= two_r_sq_thr: 2r > ||p_i - p_j||; the caller
+// zeroes col).  Only the candidates already in the word are tested, which finds them all when col_thr <= comm_sq_thr:
+// the caller's condition for using the flag.
+template <int PD, int STRIDE, bool COL = false>
 __device__ __forceinline__ void neighbour_words(const gcbf_env_desc& d, const float* pos, int i0, int n, unsigned* bits,
-                                                int bstride, int tid, int nthreads) {
+                                                int bstride, int tid, int nthreads, float col_thr = 0.f,
+                                                uint8_t* col = nullptr) {
     const int N = d.n_agents, n_words = (N + 31) >> 5;
     const float thr = d.comm_sq_thr;
     for (int task = tid; task < n * n_words; task += nthreads) {
@@ -456,6 +471,20 @@ __device__ __forceinline__ void neighbour_words(const gcbf_env_desc& d, const fl
         }
         if (w == (i >> 5)) word &= ~(1u << (i & 31));
         bits[s * bstride + w] = word;
+        if (COL && word != 0u) {   // the same acc expression as above, for the few neighbours
+            bool c = false;
+            for (unsigned m = word; m != 0u; m &= m - 1u) {
+                const int b = __ffs(m) - 1;
+                float acc;
+#pragma unroll
+                for (int c2 = 0; c2 < PD; ++c2) {
+                    const float dlt = p[c2] - q[b * STRIDE + c2];
+                    acc = (c2 == 0) ? dlt * dlt : acc + dlt * dlt;
+                }
+                c = c || (acc < col_thr);
+            }
+            if (c) col[s] = 1;
+        }
     }
 }
 
@@ -468,30 +497,51 @@ __device__ __forceinline__ int word_count(const unsigned* my_bits, int n_words, 
     return cnt;
 }
 
-// Edge row of receiver a_id at rbase: [goal | agents ascending | active hits ascending] (edge codes: gcbf_b200.h).
-// Agent j of the graph is sender sender0 + j.
-__device__ __forceinline__ void fill_row(int32_t* er, int32_t* es, int rbase, int a_id, int sender0,
-                                         const unsigned* my_bits, int n_words, unsigned hit_bits, int lane) {
-    if (lane == 0) {
-        er[rbase] = a_id;
-        es[rbase] = -1;
-    }
-    int pos = rbase + 1;
+// Edge rows of NA receivers a_id[a] at rbase[a]: [goal | agents ascending | active hits ascending] (edge codes:
+// gcbf_b200.h); rows with ok[a] false are not written.  Agent j of the graph is sender sender0 + j.
+// Lane w holds word w of every row (32 words per round), so the word loads of all NA rows issue at once and the row
+// walks only the non-empty words (most words of a sparse neighbourhood are empty).
+template <int NA>
+__device__ __forceinline__ void fill_row(int32_t* er, int32_t* es, const int (&rbase)[NA], const int (&a_id)[NA],
+                                         const bool (&ok)[NA], int sender0, const unsigned* const (&my_bits)[NA],
+                                         int n_words, const unsigned (&hit_bits)[NA], int lane) {
     const unsigned lt = (1u << lane) - 1u;
-    for (int w = 0; w < n_words; ++w) {
-        const unsigned bits = my_bits[w];
-        if (bits == 0u) continue;            // warp-uniform: most words of a sparse neighbourhood are empty
-        if ((bits >> lane) & 1u) {
-            const int e = pos + __popc(bits & lt);
-            er[e] = a_id;
-            es[e] = sender0 + (w << 5) + lane;
+    int pos[NA];
+#pragma unroll
+    for (int a = 0; a < NA; ++a) {
+        if (ok[a] && lane == 0) {
+            er[rbase[a]] = a_id[a];
+            es[rbase[a]] = -1;
         }
-        pos += __popc(bits);
+        pos[a] = rbase[a] + 1;
     }
-    if ((hit_bits >> lane) & 1u) {
-        const int e = pos + __popc(hit_bits & lt);
-        er[e] = a_id;
-        es[e] = -2 - lane;
+    for (int w0 = 0; w0 < n_words; w0 += 32) {
+        unsigned words[NA], nz[NA];
+#pragma unroll
+        for (int a = 0; a < NA; ++a) words[a] = (ok[a] && w0 + lane < n_words) ? my_bits[a][w0 + lane] : 0u;
+#pragma unroll
+        for (int a = 0; a < NA; ++a) nz[a] = __ballot_sync(0xffffffffu, words[a] != 0u);
+#pragma unroll
+        for (int a = 0; a < NA; ++a) {
+            for (unsigned m = nz[a]; m != 0u; m &= m - 1u) {      // warp-uniform
+                const int wl = __ffs(m) - 1;
+                const unsigned bits = __shfl_sync(0xffffffffu, words[a], wl);
+                if ((bits >> lane) & 1u) {
+                    const int e = pos[a] + __popc(bits & lt);
+                    er[e] = a_id[a];
+                    es[e] = sender0 + ((w0 + wl) << 5) + lane;
+                }
+                pos[a] += __popc(bits);
+            }
+        }
+    }
+#pragma unroll
+    for (int a = 0; a < NA; ++a) {
+        if (ok[a] && ((hit_bits[a] >> lane) & 1u)) {
+            const int e = pos[a] + __popc(hit_bits[a] & lt);
+            er[e] = a_id[a];
+            es[e] = -2 - lane;
+        }
     }
 }
 

@@ -42,6 +42,8 @@ constexpr int PW = PT / 32;         // warps per CTA
 constexpr int STG = 65536;          // one pipeline stage: A hi | A lo | B hi | B lo, 16 KB each (BN = 128)
 constexpr int MAX_N = 512;
 constexpr int MAX_OBS = 32;
+constexpr int MAX_APC = 64;         // agents per CTA (MAX_N / 8 CTAs)
+constexpr int FILL_NA = 2;          // rows per warp in one pass of the row fill (4 at 128 registers spills in SI)
 
 // barrier indices
 // B_MAIN: both consumer warpgroups' main-loop MMAs of an edge tile retired; B_T2F: its chained gate GEMM retired
@@ -61,7 +63,8 @@ enum {
     K_HO = 1152,        // [256][NU] folded output layer
     K_BHO = K_HO + 256 * PNU,   // [NU] output bias
     K_CST = K_BHO + PNU,        // [1] folded gate constant
-    K_FLOATS = K_CST + 1
+    K_COL_THR = K_CST + 1,      // [1] two_r_sq_thr = sqrt_threshold(two_r)
+    K_FLOATS = K_COL_THR + 1
 };
 
 struct PArgs {
@@ -77,6 +80,9 @@ struct PArgs {
     float *msg, *logit, *ag, *v1, *z;
     float* terms;                                        // [2][A][4] per-agent reward / cost terms, by step parity
     unsigned long long* prof;                            // optional [T + 1][8] %globaltimer stamps of cluster 0 / CTA 0 (ns)
+    // 1 when 2r < comm_radius: every agent closer than 2r is in the row, so the cost's collision term comes from the
+    // neighbour scan of the graph build (s_col) instead of collides_prev's walk of the previous row
+    int col_scan;
     // mode 0: one hardware cluster of C CTAs per environment (every barrier is barrier.cluster).
     // mode 1 ("pairs"): when fewer clusters of C CTAs than environments are resident (BASELINE's config has 16
     // environments of 8 CTAs), the C CTAs of an environment are C/2 hardware clusters of 2.  A pair owns 2 APC consecutive agents, their edge
@@ -148,6 +154,7 @@ rollout_persist_kernel(const __grid_constant__ PArgs P, const __grid_constant__ 
     unsigned* s_hb = reinterpret_cast<unsigned*>(s_off + 72);              // [APC]
     float* s_red = reinterpret_cast<float*>(s_hb + 64);                    // [3][PW]
     float* sk = s_red + 3 * PW;                                            // [K_FLOATS] rollout constants
+    uint8_t* s_col = reinterpret_cast<uint8_t*>(sk + K_FLOATS);            // [APC] collision flags of the graph built last
 
     const gcbf_env_desc& d = P.d;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -217,6 +224,8 @@ rollout_persist_kernel(const __grid_constant__ PArgs P, const __grid_constant__ 
         for (int i = tid; i < O * OBW; i += PT) sobs[(i / OBW) * OBS2 + (i % OBW)] = ob[i];
     }
     for (int i = tid; i < d.n_rays * PD; i += PT) stab[i] = P.ray_table[i];
+    for (int i = tid; i < MAX_APC; i += PT) s_col[i] = 0;
+    if (tid == 0) sk[K_COL_THR] = sqrt_threshold(d.two_r);
     __syncthreads();
     derive_far_fields(sobs, O, d.comm_radius, tid, PT);
     uint32_t it = 0;      // k-blocks pushed through the 3-stage ring so far (all roles advance it identically)
@@ -480,8 +489,11 @@ rollout_persist_kernel(const __grid_constant__ PArgs P, const __grid_constant__ 
 #pragma unroll
                         for (int c = 0; c < SD; ++c) agent_n[a * SD + c] = xn[c];
                         const float nr = sqrtf(sq);
-                        // the agent's own row of the graph of state t was filled by this CTA (phase G of step t - 1)
-                        const bool col = collides_prev<PD, SD>(x, rs_t[a], rd_t[a], es_t + env_e0, agent_t, d.two_r);
+                        // the agent's own row of the graph of state t was filled by this CTA (phase G of step t - 1),
+                        // and so was its collision flag, which is cleared here for the next graph
+                        const bool col = P.col_scan ? s_col[i - a_lo] != 0
+                                                    : collides_prev<PD, SD>(x, rs_t[a], rd_t[a], es_t + env_e0, agent_t, d.two_r);
+                        s_col[i - a_lo] = 0;
                         const bool in_obs = O > 0 && inside_any<PD, OBS2>(sobs, O, x, d.radius);
                         *reinterpret_cast<float4*>(terms_t + a * 4) =
                             make_float4(nr * nr, col ? 1.f : 0.f, in_obs ? 1.f : 0.f, 0.f);
@@ -494,11 +506,11 @@ rollout_persist_kernel(const __grid_constant__ PArgs P, const __grid_constant__ 
             __syncthreads();
             if (stamp) pr[5] = gtime();
 
-            // ---- neighbour words (thread per (word, agent)) and LiDAR + active hit bits (warp per agent) of this
-            // CTA's agents.  The words do not depend on the LiDAR, so the two overlap across warps.
+            // ---- neighbour words (thread per (word, agent)) with the collision flags, and LiDAR + active hit bits (warp
+            // per agent) of this CTA's agents.  The words do not depend on the LiDAR, so the two overlap across warps.
             const int n_slots = a_hi - a_lo;
             const int bstride = n_words | 1;
-            neighbour_words<PD, SD>(d, sst, a_lo, n_slots, sbits, bstride, tid, PT);
+            neighbour_words<PD, SD, true>(d, sst, a_lo, n_slots, sbits, bstride, tid, PT, sk[K_COL_THR], s_col);
             for (int slot = warp; slot < n_slots; slot += PW) {
                 const int i = a_lo + slot;
                 float p[PD], h[PD];
@@ -547,26 +559,36 @@ rollout_persist_kernel(const __grid_constant__ PArgs P, const __grid_constant__ 
                 base += (r2 < lrank) ? v : 0;
                 env_total += v;
             }
-            // ---- fill pass: rows [goal | agents ascending | active hits ascending], agent order inside the environment
-            for (int slot = warp; slot < n_slots; slot += PW) {
-                const int i = a_lo + slot;
-                const int a_id = env_a0 + i;
-                const int deg = s_off[slot + 1] - s_off[slot];
-                const bool over = base + s_off[slot] + deg > seg_cap;
-                const int rbase = seg_off + base + s_off[slot];       // row offset inside the environment's lists
-                if (over) {
-                    if (lane == 0) {
-                        atomicOr(&P.counters[((size_t)tn * P.n_nets + net()) * 4 + 1], 1);
-                        rs_n[a_id] = 0;
-                        rd_n[a_id] = 0;
+            // ---- fill pass: rows [goal | agents ascending | active hits ascending], agent order inside the environment,
+            // FILL_NA agents per warp (slots s0 + PW a; slots past n_slots repeat s0 and write nothing).  An overflowed
+            // row is dropped (row degree 0), and so is its collision flag: collides_prev finds no sender in it
+            for (int s0 = warp; s0 < n_slots; s0 += PW * FILL_NA) {
+                int rbase[FILL_NA], a_id[FILL_NA];
+                bool ok[FILL_NA];
+                const unsigned* my_bits[FILL_NA];
+                unsigned hit_bits[FILL_NA];
+#pragma unroll
+                for (int a = 0; a < FILL_NA; ++a) {
+                    const int slot = s0 + PW * a;
+                    const bool in = slot < n_slots;
+                    const int sl = in ? slot : s0;
+                    a_id[a] = env_a0 + a_lo + sl;
+                    const int deg = s_off[sl + 1] - s_off[sl];
+                    const bool over = base + s_off[sl] + deg > seg_cap;
+                    rbase[a] = seg_off + base + s_off[sl];       // row offset inside the environment's lists
+                    ok[a] = in && !over;
+                    my_bits[a] = sbits + sl * bstride;
+                    hit_bits[a] = s_hb[sl];
+                    if (in && lane == 0) {
+                        if (over) {
+                            atomicOr(&P.counters[((size_t)tn * P.n_nets + net()) * 4 + 1], 1);
+                            s_col[sl] = 0;
+                        }
+                        rs_n[a_id[a]] = over ? 0 : rbase[a];
+                        rd_n[a_id[a]] = over ? 0 : deg;
                     }
-                    continue;
                 }
-                if (lane == 0) {
-                    rs_n[a_id] = rbase;
-                    rd_n[a_id] = deg;
-                }
-                fill_row(er_n + env_e0, es_n + env_e0, rbase, a_id, env_a0, sbits + slot * bstride, n_words, s_hb[slot], lane);
+                fill_row<FILL_NA>(er_n + env_e0, es_n + env_e0, rbase, a_id, ok, env_a0, my_bits, n_words, hit_bits, lane);
             }
             if (lrank == 0 && tid == 0) atomicAdd(&P.counters[((size_t)tn * P.n_nets + net()) * 4 + 0], min(env_total, seg_cap));
             M_cur = min(env_total, seg_cap);
@@ -662,7 +684,7 @@ extern "C" __attribute__((visibility("default"))) int32_t gcbf_rollout_persisten
 
 static int persist_smem_bytes() {
     return 3 * rp::STG + 512 + 7 * 256 * 4 + rp::MAX_N * 4 * 4 + rp::MAX_OBS * 24 * 4 + 64 * 4 + 64 * 17 * 4 + 72 * 4 + 64 * 4 +
-           3 * rp::PW * 4 + rp::K_FLOATS * 4 + 1024;
+           3 * rp::PW * 4 + rp::K_FLOATS * 4 + rp::MAX_APC + 1024;
 }
 
 /* Co-resident clusters of `cluster_size` CTAs of the persistent rollout kernel on the current device
@@ -738,6 +760,7 @@ static int32_t persist_launch(const char* who, bool rounds, const gcbf_env_desc*
     P.T = n_steps;
     P.cap_env = cap_env;
     P.C = rp::cluster_size(N, cap_env);
+    P.col_scan = desc->two_r < desc->comm_radius ? 1 : 0;
     P.net_of_env = net_of_env;
     P.n_nets = n_nets;
     P.p_stride = net_stride(gcbf_param_count_l(ed, nu, 1));
