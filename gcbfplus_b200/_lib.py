@@ -98,6 +98,9 @@ _SIGNATURES = {
     "gcbf_refine_workspace_floats": (C.c_int64, [C.POINTER(EnvDesc)]),
     "gcbf_refine_actions": (C.c_int32, [C.POINTER(EnvDesc), C.c_float, C.c_float, C.c_int32, C.c_int32] + [_P] * 15 +
                             [C.c_int64, _P]),
+    "gcbf_cbf_condition_prepare": (C.c_int32, [C.c_int32, C.c_int32, C.c_int32, _P, _P, C.c_int64, _P]),
+    "gcbf_cbf_condition_workspace_floats": (C.c_int64, [C.POINTER(EnvDesc)]),
+    "gcbf_cbf_condition": (C.c_int32, [C.POINTER(EnvDesc), C.c_float, C.c_int32] + [_P] * 17 + [C.c_int64, _P]),
     "gcbf_cbf_pairwise": (C.c_int32, [C.POINTER(EnvDesc)] + [_P] * 9),
     "gcbf_cbfqp_workspace_floats": (C.c_int64, [C.POINTER(EnvDesc)]),
     "gcbf_cbfqp_dec_share": (C.c_int32, [C.POINTER(EnvDesc), C.c_float, C.c_int32, C.c_float] + [_P] * 7 +

@@ -15,6 +15,8 @@ from .. import _lib
 from ..env.base import MultiAgentEnv
 from ..utils.graph import SwarmGraph
 from .base import MultiAgentController
+from .falsify import FALSIFY_LR, CbfCondition
+from .falsify import falsify as _falsify
 from .nets import GnnRunner
 from .params import NetParams
 from .refine import (REFINE_LR, REFINE_MAX_ITER, launch_refine, planes_buffer, prepare_planes, refine_workspace,
@@ -131,6 +133,21 @@ class GCBFPlus(MultiAgentController):
         if return_info:
             return action, value, iters
         return action
+
+    def cbf_condition(self, graph: SwarmGraph, with_grad: bool = False):
+        """The CBF condition under the policy for every graph of the batch (DESIGN 4.10): with a = 2 pi + u_ref and
+        g' = forward_graph(g, a), term_i = -(h_i(g') - h_i(g)) / dt - alpha h_i(g); the worst agent maximises term over
+        the agents with h >= 0 and a finite term (-1: none).  Returns (h [G, N], term [G, N], worst [G] int32) and,
+        with with_grad, the gradient [G, N, sd] of the worst term wrt the agent states (topology and LiDAR hits held
+        fixed).  One-layer networks only."""
+        return CbfCondition(self)(graph, with_grad)
+
+    def falsify(self, agent: torch.Tensor, goal: torch.Tensor, obstacle, n_iter: int, lr: float = FALSIFY_LR) -> dict:
+        """Search for states where the CBF condition fails: n_iter iterations of normalised gradient ascent on the
+        worst term of each graph from the states agent [G, N, sd] (goals and obstacles fixed).  Returns per graph the
+        start J0, the best J with its agent, iteration, states, h and term, and the false-safe counts (unsafe agents
+        with h >= 0) at the start and at the best states (algo/falsify.py)."""
+        return _falsify(self, agent, goal, obstacle, n_iter, lr)
 
     def get_cbf(self, graph: SwarmGraph, params: Optional[NetParams] = None) -> torch.Tensor:
         """gcbf.py:209-212 -> [G, N, 1]."""

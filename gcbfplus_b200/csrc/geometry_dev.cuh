@@ -1,6 +1,7 @@
 // geometry_dev.cuh -- device functions shared by geometry.cu, rollout_persist.cu and train.cu: obstacle primitives
 // (Rectangle / Sphere inside + ray cast), the stable 32-key warp sort of the LiDAR returns, u_ref, the Euler step,
-// the policy tail and reward / cost terms of an env step, and the per-warp pieces of the graph build (2-D LiDAR,
+// their state Jacobians (the CBF-condition gradient of falsify.cuh), the policy tail and reward / cost terms of an env
+// step, and the per-warp pieces of the graph build (2-D LiDAR,
 // active hits, neighbour scan, edge-row fill).  The 5-launch rollout step and the persistent rollout kernel run these
 // same functions, which is what keeps the two paths bit-identical.
 // Every including unit is compiled with -fmad=false: every arithmetic step keeps the reference's
@@ -192,6 +193,99 @@ __device__ __forceinline__ void u_ref_dev(const gcbf_env_desc& d, const float* x
     }
 }
 
+// dx += du . d u_ref / dx (the state Jacobian of u_ref_dev, applied to du).  Kinks as torch autograd differentiates the
+// reference's formulas: a clip passes no gradient outside its limits (strictly inside: gradient 1), the branch
+// conditions of the DubinsCar law and the python-style mod of theta are piecewise constant.
+template <int KIND>
+__device__ __forceinline__ void u_ref_vjp_dev(const gcbf_env_desc& d, const float* x, const float* gl, const float* du,
+                                              float* dx) {
+    using T = EnvTraits<KIND>;
+    constexpr int SD = T::SD, NU = T::NU;
+    if (KIND == GCBF_ENV_DUBINS_CAR) {
+        const float PI_F = 3.14159265358979323846f;
+        const float TWO_PI = 6.283185307179586f;
+        const float pdx = x[0] - gl[0], pdy = x[1] - gl[1];
+        const float dist = sqrtf(pdx * pdx + pdy * pdy);
+        float theta_t = atan2f(-pdy, -pdx);
+        theta_t = theta_t - floorf(theta_t / TWO_PI) * TWO_PI;
+        const float theta = x[2] - floorf(x[2] / TWO_PI) * TWO_PI;
+        const float theta_diff = theta_t - theta;
+        const float cth = cosf(theta), sth = sinf(theta);
+        const float dot = (-pdx) * cth + (-pdy) * sth;
+        const float D = dist + 0.0001f;
+        const float q = dot / D;
+        // omega = s tb (s = +-1 by the branch conditions, 0 never: one of the four cases always holds)
+        const bool c1 = (theta_diff < PI_F) && (theta_diff >= 0.f);
+        const bool c2 = (theta_diff > -PI_F) && (theta_diff <= 0.f);
+        const float s = (theta <= PI_F) ? (c1 ? 1.f : -1.f) : (c2 ? -1.f : 1.f);
+        const float tb = acosf(fminf(fmaxf(q, -1.f), 1.f));
+        const float om = s * tb;
+        const float dom = (om > -5.f && om < 5.f) ? du[0] : 0.f;
+        const float dq = (q > -1.f && q < 1.f) ? dom * s * (-1.f / sqrtf(1.f - q * q)) : 0.f;
+        // q = dot / (dist + 1e-4)
+        const float dD = -dq * dot / (D * D);
+        float gx = dq * (-cth) / D + dD * pdx / dist;
+        float gy = dq * (-sth) / D + dD * pdy / dist;
+        const float gth = dq * (pdx * sth - pdy * cth) / D;
+        // u[1] = -2.5 v + 2.3 |coef pd|, coef = rc / nrm where nrm = sqrt(1e-6 + |pd|^2) > rc
+        const float nrm = sqrtf(1e-6f + (pdx * pdx + pdy * pdy));
+        const bool clip = nrm > d.comm_radius;
+        const float coef = clip ? d.comm_radius / fmaxf(nrm, d.comm_radius) : 1.f;
+        const float qx = coef * pdx, qy = coef * pdy;
+        const float r = sqrtf(qx * qx + qy * qy);
+        const float dr = 2.3f * du[1];
+        const float dqx = dr * qx / r, dqy = dr * qy / r;
+        gx += coef * dqx;
+        gy += coef * dqy;
+        if (clip) {
+            const float dn = (dqx * pdx + dqy * pdy) * (-d.comm_radius / (nrm * nrm));
+            gx += dn * pdx / nrm;
+            gy += dn * pdy / nrm;
+        }
+        dx[0] += gx;
+        dx[1] += gy;
+        dx[2] += gth;
+        dx[3] += -2.5f * du[1];
+        return;
+    }
+    // e = clip(err, -|err| rc / |err|, |err| rc / |err|) componentwise with err = goal - x: a clipped component is
+    // err_c rc / |err|;  u = clip(K e, -u_lim, u_lim)
+    float err[SD], e[SD];
+    float acc = 0.f;
+#pragma unroll
+    for (int c = 0; c < SD; ++c) {
+        err[c] = gl[c] - x[c];
+        acc = (c == 0) ? err[c] * err[c] : acc + err[c] * err[c];
+    }
+    const float nrm = sqrtf(acc);
+    bool clipped[SD];
+#pragma unroll
+    for (int c = 0; c < SD; ++c) {
+        const float emax = fabsf(err[c] / nrm * d.comm_radius);
+        clipped[c] = err[c] > emax || err[c] < -emax;
+        e[c] = fminf(fmaxf(err[c], -emax), emax);
+    }
+    float de[SD];
+#pragma unroll
+    for (int c = 0; c < SD; ++c) de[c] = 0.f;
+#pragma unroll
+    for (int a = 0; a < NU; ++a) {
+        float s = 0.f;
+#pragma unroll
+        for (int c = 0; c < SD; ++c) s = (c == 0) ? e[c] * d.K[a * SD + c] : s + e[c] * d.K[a * SD + c];
+        const float ds = (s > -d.u_lim && s < d.u_lim) ? du[a] : 0.f;
+#pragma unroll
+        for (int c = 0; c < SD; ++c) de[c] += ds * d.K[a * SD + c];
+    }
+    const float k = d.comm_radius / nrm;
+    float dot = 0.f;   // sum over the clipped components of de_c err_c
+#pragma unroll
+    for (int c = 0; c < SD; ++c) dot += clipped[c] ? de[c] * err[c] : 0.f;
+    const float w = k * dot / (nrm * nrm);
+#pragma unroll
+    for (int c = 0; c < SD; ++c) dx[c] -= (clipped[c] ? k * de[c] : de[c]) - w * err[c];   // d err / dx = -1
+}
+
 // agent_step_euler (double_integrator.py:128-143; SI :104-109; Dubins :104-122; LD :123-134)
 // stop = false: the DubinsCar stop mask is off (env.enable_stop = False, dubins_car.py:138-142)
 template <int KIND>
@@ -235,6 +329,50 @@ __device__ __forceinline__ void euler_dev(const gcbf_env_desc& d, const float* x
                              (KIND == GCBF_ENV_LINEAR_DRONE && c >= 3);
         if (limited) v = isnan(v) ? v : fminf(fmaxf(v, -d.v_lim), d.v_lim);
         xn[c] = v;
+    }
+}
+
+// The transposed Jacobians of euler_dev (stop mask on) at (x, u): dx = dxn . dx'/dx and du = dxn . dx'/du, where dxn
+// is the gradient wrt x' after the velocity clip (the caller zeroes the clipped components).  The DubinsCar stop
+// mask is piecewise constant in x.
+template <int KIND>
+__device__ __forceinline__ void euler_vjp_dev(const gcbf_env_desc& d, const float* x, const float* gl, const float* dxn,
+                                              float* dx, float* du) {
+    using T = EnvTraits<KIND>;
+    constexpr int SD = T::SD, NU = T::NU;
+#pragma unroll
+    for (int c = 0; c < SD; ++c) dx[c] = dxn[c];
+    if (KIND == GCBF_ENV_SINGLE_INTEGRATOR) {
+        du[0] = dxn[0] * d.dt;
+        du[1] = dxn[1] * d.dt;
+    } else if (KIND == GCBF_ENV_DOUBLE_INTEGRATOR) {
+        dx[2] += dxn[0] * d.dt;
+        dx[3] += dxn[1] * d.dt;
+        du[0] = dxn[2] * d.dt / d.mass;
+        du[1] = dxn[3] * d.dt / d.mass;
+    } else if (KIND == GCBF_ENV_DUBINS_CAR) {
+        const float ddx = x[0] - gl[0], ddy = x[1] - gl[1];
+        const float keep = (sqrtf(ddx * ddx + ddy * ddy) < d.half_r) ? 0.f : 1.f;
+        const float c = cosf(x[2]), s = sinf(x[2]), kt = keep * d.dt;
+        dx[2] += (dxn[0] * (-s * x[3]) + dxn[1] * (c * x[3])) * kt;
+        dx[3] += (dxn[0] * c + dxn[1] * s) * kt;
+        du[0] = dxn[2] * 20.f * kt;
+        du[1] = dxn[3] * kt;
+    } else {
+#pragma unroll
+        for (int c = 0; c < SD; ++c) {
+            float s = 0.f;
+#pragma unroll
+            for (int r = 0; r < SD; ++r) s += dxn[r] * d.A[r * SD + c];
+            dx[c] += s * d.dt;
+        }
+#pragma unroll
+        for (int c = 0; c < NU; ++c) {
+            float s = 0.f;
+#pragma unroll
+            for (int r = 0; r < SD; ++r) s += dxn[r] * d.B[r * NU + c];
+            du[c] = s * d.dt;
+        }
     }
 }
 

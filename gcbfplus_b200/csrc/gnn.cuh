@@ -84,6 +84,22 @@ __device__ __forceinline__ void edge_state_dev(const float* s, float* es) {
     }
 }
 
+// ds = des (d edge_state / d s): the DubinsCar (x, y, v cos th, v sin th) Jacobian, the identity otherwise
+template <int KIND>
+__device__ __forceinline__ void edge_state_vjp_dev(const float* s, const float* des, float* ds) {
+    constexpr int SD = EnvTraits<KIND>::SD;
+    if (KIND == GCBF_ENV_DUBINS_CAR) {
+        const float c = cosf(s[2]), sn = sinf(s[2]);
+        ds[0] = des[0];
+        ds[1] = des[1];
+        ds[2] = des[2] * (-s[3] * sn) + des[3] * (s[3] * c);
+        ds[3] = des[2] * c + des[3] * sn;
+    } else {
+#pragma unroll
+        for (int c = 0; c < SD; ++c) ds[c] = des[c];
+    }
+}
+
 // Sender edge-state for an edge code (see gcbf_b200.h): agent / goal / hit node.
 template <int KIND>
 __device__ __forceinline__ void sender_state_dev(int code, int a, int R, const float* agent, const float* goal,

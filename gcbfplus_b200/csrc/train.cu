@@ -5,7 +5,9 @@
 // workspace, then partial_sum_kernel; per-edge input gradients gathered per agent), so the step is bit-identical from
 // run to run for the same inputs on the same GPU model.  On the tensor-core path the step runs on the folded
 // network (gnn_backward_folded / unfold_jobs below: 4 GEMMs per pass and direction instead of
-// 9-10, same gradient); the strict-fp32 SIMT path runs the layer-by-layer step.
+// 9-10, same gradient); the strict-fp32 SIMT path runs the layer-by-layer step.  The same pieces serve the online
+// policy refinement (refine.cuh) and the CBF condition with its gradient wrt the agent states (falsify.cuh), both
+// included at the end of this unit.
 //
 // Replaces gcbfplus/algo/gcbf_plus.py:354-447 (update_inner / get_loss / value_and_grad),
 // trainer/utils.py:62-75 (compute_norm_and_clip), optax.adamw + optax.apply_if_finite
@@ -944,6 +946,7 @@ __global__ void polyak_kernel(float* __restrict__ tgt, const float* __restrict__
 }  // namespace gcbf
 #include "qp.cuh"
 #include "refine.cuh"
+#include "falsify.cuh"
 namespace gcbf {
 
 // ------------------------------------------------------------------------------------ QP label workspace layout
@@ -1408,6 +1411,100 @@ extern "C" __attribute__((visibility("default"))) int32_t gcbf_refine_actions(
         count_launch();
         RC(check_launch("refine_update_kernel"));
     }
+#undef RC
+    return 0;
+}
+
+// ------------------------------------------------------------------------------------ CBF condition + state gradient
+extern "C" __attribute__((visibility("default"))) int32_t gcbf_cbf_condition_prepare(int32_t edge_dim, int32_t out_dim,
+                                                                                     int32_t use_tensor_cores,
+                                                                                     const float* params,
+                                                                                     float* prepared,
+                                                                                     int64_t prepared_floats,
+                                                                                     void* stream) {
+    GCBF_REQUIRE(params && prepared && (edge_dim == 2 || edge_dim == 4 || edge_dim == 6) && out_dim >= 1 && out_dim <= 3,
+                 "gcbf_cbf_condition_prepare: bad argument");
+    GCBF_REQUIRE((((uintptr_t)params | (uintptr_t)prepared) & 15) == 0, "buffers must be 16-byte aligned");
+    const ParamLayout L = make_layout(edge_dim, out_dim);
+    const int64_t need = use_tensor_cores ? make_plane_layout(make_deep_layout(edge_dim, out_dim, 1), edge_dim).total
+                                          : make_trans_layout(L).total;
+    GCBF_REQUIRE(prepared_floats >= need, "gcbf_cbf_condition_prepare: buffer too small: %lld < %lld floats",
+                 (long long)prepared_floats, (long long)need);
+    return prepare_bwd_operands(edge_dim, out_dim, use_tensor_cores, params, prepared, (cudaStream_t)stream);
+}
+
+extern "C" __attribute__((visibility("default"))) int64_t gcbf_cbf_condition_workspace_floats(const gcbf_env_desc* desc) {
+    return graph_desc_ok(desc) ? make_falsify_ws(desc).total : -1;
+}
+
+extern "C" __attribute__((visibility("default"))) int32_t gcbf_cbf_condition(
+    const gcbf_env_desc* desc, float alpha, int32_t use_tensor_cores, const float* cbf_params, const float* cbf_planes,
+    const float* actor_params, const float* actor_planes, const float* agent, const float* goal, const float* hits,
+    const int32_t* row_start, const int32_t* row_deg, const int32_t* edge_recv, const int32_t* edge_src,
+    const int32_t* counters, float* h, float* term, int32_t* worst, float* grad_x, float* workspace,
+    int64_t workspace_floats, void* stream) {
+    GCBF_REQUIRE(desc && cbf_params && cbf_planes && actor_params && actor_planes && agent && goal && hits &&
+                     row_start && row_deg && edge_recv && edge_src && counters && h && term && worst && workspace,
+                 "gcbf_cbf_condition: NULL pointer argument");
+    if (int32_t rc = check_graph_desc(desc, "gcbf_cbf_condition")) return rc;
+    GCBF_REQUIRE(desc->dt > 0.f && isfinite(alpha), "gcbf_cbf_condition: bad settings (dt %g, alpha %g)",
+                 (double)desc->dt, (double)alpha);
+    const FalsifyWs F = make_falsify_ws(desc);
+    GCBF_REQUIRE(workspace_floats >= F.total, "cbf condition workspace too small: %lld < %lld floats",
+                 (long long)workspace_floats, (long long)F.total);
+    GCBF_REQUIRE((((uintptr_t)workspace | (uintptr_t)cbf_params | (uintptr_t)cbf_planes | (uintptr_t)actor_params |
+                   (uintptr_t)actor_planes) & 15) == 0, "buffers must be 16-byte aligned");
+    cudaStream_t st = (cudaStream_t)stream;
+    const gcbf_env_desc* d = desc;
+    const int nu = env_nu(d->env_kind);
+    const int G = d->n_graphs, N = d->n_agents, A = G * N;
+    const int blocks = (A + 127) / 128;
+    float* ws = workspace;
+    int32_t rc;
+#define RC(x) do { if ((rc = (x))) return rc; } while (0)
+    // g: the graph; gn: its edges over the next states x' (forward_graph: every feature norm-clipped)
+    const GraphRefs g{agent, goal, hits, row_start, row_deg, edge_recv, edge_src, counters};
+    const GraphRefs gn = g.with_agent(ws + F.xn);
+    auto forward = [&](int out_dim, const float* P, const float* PT, const GraphRefs& on, int clip_all, float* out,
+                       float* fws) -> int32_t {
+        return gnn_forward(d, out_dim, 1, P, use_tensor_cores ? PT : nullptr, on, clip_all, out, nullptr, fws, st);
+    };
+    // 1. forwards: h = cbf(g), pi = actor(g), a = 2 pi + u_ref and x' (act_dyn_kernel), h' = cbf(g')
+    RC(forward(1, cbf_params, cbf_planes, g, 0, h, ws + F.fw_h));
+    RC(forward(nu, actor_params, actor_planes, g, 0, ws + F.pi, ws + F.fw_pi));
+    GCBF_DISPATCH_ENV(d->env_kind, {
+        act_dyn_kernel<KIND><<<blocks, 128, 0, st>>>(*d, agent, goal, ws + F.pi, ws + F.act, ws + F.xn);
+    });
+    count_launch();
+    RC(check_launch("act_dyn_kernel"));
+    RC(forward(1, cbf_params, cbf_planes, gn, 1, ws + F.hn, ws + F.fw_hn));
+    // 2. terms, worst agent per graph, upstream gradients of J wrt h and h'
+    falsify_select_kernel<<<G, FALSIFY_SELECT_THREADS, 0, st>>>(N, env_sd(d->env_kind), alpha, d->dt, h, ws + F.hn,
+                                                                ws + F.xn, term, worst, ws + F.dh, ws + F.dhn);
+    count_launch();
+    RC(check_launch("falsify_select_kernel"));
+    if (!grad_x) return 0;
+    // 3. data-only backward of cbf(g') -> d_es'
+    RC(gnn_backward_impl({d, gn, ws + F.gw, nullptr, use_tensor_cores, 1, cbf_params, cbf_planes, ws + F.fw_hn,
+                          ws + F.hn, ws + F.dhn, nullptr, nullptr, 1, ws + F.des_n, ws + F.je}, st));
+    // 4. through x' = Euler(x, clip_action(2 pi + u_ref(x))): dpi and the direct / u_ref parts of d J / dx
+    GCBF_DISPATCH_ENV(d->env_kind, {
+        falsify_dyn_kernel<KIND><<<blocks, 128, 0, st>>>(*d, agent, goal, ws + F.act, ws + F.xn, ws + F.des_n,
+                                                         ws + F.dpi, ws + F.gx);
+    });
+    count_launch();
+    RC(check_launch("falsify_dyn_kernel"));
+    // 5. data-only backwards on g: the actor with upstream dpi, the CBF with upstream dh
+    RC(gnn_backward_impl({d, g, ws + F.gw, nullptr, use_tensor_cores, nu, actor_params, actor_planes, ws + F.fw_pi,
+                          ws + F.pi, ws + F.dpi, nullptr, nullptr, 0, ws + F.des_a, ws + F.je}, st));
+    RC(gnn_backward_impl({d, g, ws + F.gw, nullptr, use_tensor_cores, 1, cbf_params, cbf_planes, ws + F.fw_h, h,
+                          ws + F.dh, nullptr, nullptr, 0, ws + F.des_c, ws + F.je}, st));
+    // 6. edge-state gradients -> states, plus the Euler / u_ref part
+    GCBF_DISPATCH_ENV(d->env_kind, {
+        falsify_grad_kernel<KIND><<<blocks, 128, 0, st>>>(*d, agent, ws + F.des_a, ws + F.des_c, ws + F.gx, grad_x);
+    });
+    count_launch();
+    RC(check_launch("falsify_grad_kernel"));
 #undef RC
     return 0;
 }

@@ -418,6 +418,34 @@ int32_t gcbf_refine_actions(const gcbf_env_desc* desc, float alpha, float lr, in
                             const int32_t* edge_src, const int32_t* counters, float* action, float* value,
                             int32_t* iters, float* workspace, int64_t workspace_floats, void* stream);
 
+/* ---------------------------------------------------------------- CBF condition of the closed loop (falsification)
+ * gcbf_cbf_condition evaluates the learned CBF's condition under the GCBF+ policy for a batch of G graphs and,
+ * optionally, its gradient with respect to the agent states (GCBFPlus.falsify climbs it to find counterexamples):
+ *   a = 2 pi(g) + u_ref(x);  x' = agent_step_euler(x, clip_action(a)) (DubinsCar stop mask on);  g' = forward_graph(g, a)
+ *   term_i = -(h_i(g') - h_i(g)) / dt - alpha h_i(g)
+ *   J = max term_i over the agents of the graph with h_i(g) >= 0 and a finite term; worst = the agent attaining it
+ *       (ties: the lowest index), -1 where no agent qualifies (J = -inf, gradient 0)
+ *   grad_x = d J / d x with the topology and the LiDAR hit points held fixed: through h(g), pi(g), u_ref, the Euler
+ *       step with its velocity clip, clip_action and h(g').  relu'(0) = 0 and a clip passes no gradient outside its
+ *       limits; an agent whose u_ref is NaN (exactly at its goal) has a NaN term and a NaN gradient row.
+ *   cbf_params / actor_params: one-layer networks;  cbf_planes / actor_planes: gcbf_cbf_condition_prepare of them with
+ *     the same use_tensor_cores (rebuild them whenever the parameters change), out_dim 1 and nu,
+ *     gcbf_params_t_count_l(edge_dim, out_dim, 1) floats each
+ *   graph arrays as gcbf_qp_labels takes them;  h [A], term [A], worst [G] int32 (out)
+ *   grad_x [A, sd] (out) or NULL: forwards and selection only
+ *   workspace: gcbf_cbf_condition_workspace_floats(desc) floats.
+ * The launch sequence is fixed (no host sync, capturable).  No float atomics: the same inputs on the same GPU model
+ * give bit-identical outputs. */
+int32_t gcbf_cbf_condition_prepare(int32_t edge_dim, int32_t out_dim, int32_t use_tensor_cores, const float* params,
+                                   float* prepared, int64_t prepared_floats, void* stream);
+int64_t gcbf_cbf_condition_workspace_floats(const gcbf_env_desc* desc);
+int32_t gcbf_cbf_condition(const gcbf_env_desc* desc, float alpha, int32_t use_tensor_cores, const float* cbf_params,
+                           const float* cbf_planes, const float* actor_params, const float* actor_planes,
+                           const float* agent, const float* goal, const float* hits, const int32_t* row_start,
+                           const int32_t* row_deg, const int32_t* edge_recv, const int32_t* edge_src,
+                           const int32_t* counters, float* h, float* term, int32_t* worst, float* grad_x,
+                           float* workspace, int64_t workspace_floats, void* stream);
+
 /* ---------------------------------------------------------------- CBF-QP baseline controllers
  * Replace the reference's hand-written baselines for a batch of G graphs: the pairwise CBFs
  * (gcbfplus/algo/utils.py:44-349, get_pwise_cbf_fn :413-439, k = 3), DecShareCBF.get_qp_action

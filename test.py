@@ -15,7 +15,10 @@ filters u_ref instead (the reference's get_qp_action as a controller).  It print
 several runs of one configuration, --paths with --all-steps every checkpoint of each.  All the networks roll out
 together (RolloutEngine with n_nets networks: one persistent launch where it applies), each on exactly the episodes
 `--path RUN --step S` would give it; one summary line per network, prefixed run=<dir> step=<S>, then the best network
-by success rate.  --log appends one row per network (step first, then test_log.csv's columns) to <run>/test_sweep.csv."""
+by success rate.  --log appends one row per network (step first, then test_log.csv's columns) to <run>/test_sweep.csv.
+--falsify ITERS (with --path) searches for states where the trained CBF's condition fails under the policy
+(GCBFPlus.falsify: ITERS normalised gradient-ascent iterations) from every recorded step of the evaluation episodes,
+prints one summary line and writes <path>/falsify/step<S>.npz."""
 import argparse
 import os
 
@@ -34,6 +37,7 @@ def test(args):
     print(f"> Running test.py {args}")
     if args.cpu:
         raise SystemExit("--cpu: gcbfplus_b200 is the sm_90a CUDA path only (no CPU fallback by design)")
+    check_falsify_flags(args)
     if check_sweep_flags(args):
         test_sweep(args)
         return
@@ -125,6 +129,8 @@ def test(args):
     if args.log:
         with open(os.path.join(path, "test_log.csv"), "a") as f:
             f.write(log_row(env, args, summary) + "\n")
+    if getattr(args, "falsify", None) is not None:
+        run_falsify(args, env, algo, eng, g0, path, step)
     if args.cbf is not None:
         assert algo is not None, "--cbf needs a trained CBF (--path)"
         out_dir = os.path.join(path, "cbf_contours")
@@ -271,6 +277,52 @@ def test_sweep(args):
         print("video rendering is out of scope of the CUDA hot path (SURVEY.md section 2, row 17); skipped")
 
 
+def check_falsify_flags(args) -> None:
+    """--falsify ITERS searches a trained GCBF+ run's CBF (--path) for counterexamples from the states its actor visits:
+    it excludes every other controller and the sweeps."""
+    if getattr(args, "falsify", None) is None:
+        return
+    if args.falsify < 1:
+        raise SystemExit(f"--falsify takes the number of search iterations (>= 1), got {args.falsify}")
+    for flag, given in (("--u-ref", args.u_ref), ("--online-refine", args.online_refine),
+                        ("--qp-filter", args.qp_filter), ("--paths", getattr(args, "paths", None) is not None),
+                        ("--all-steps", getattr(args, "all_steps", False))):
+        if given:
+            raise SystemExit(f"--falsify searches the CBF of one trained GCBF+ actor; it cannot be combined with {flag}")
+    if args.algo in BASELINES:
+        raise SystemExit(f"--falsify searches a trained GCBF+ CBF; it cannot be combined with the {args.algo} baseline")
+    if args.path is None:
+        raise SystemExit("--falsify needs a trained GCBF+ run (--path)")
+
+
+def run_falsify(args, env, algo, eng, g0, path: str, step: int) -> None:
+    """--falsify: the search from every recorded state of the episodes (each with its own goals and obstacles), one
+    summary line, and the per-graph results in <path>/falsify/step<S>.npz (graph g = t * n_epi + e)."""
+    import torch
+    states = eng.agent                                          # [T + 1, E, N, sd]
+    T1, E = states.shape[0], states.shape[1]
+    agent = states.reshape(T1 * E, *states.shape[2:]).contiguous()
+    goal = g0.goal.repeat(T1, 1, 1).contiguous()
+    obstacle = g0.obstacle.repeat(T1) if g0.obstacle is not None else None
+    r = algo.falsify(agent, goal, obstacle, args.falsify)
+    torch.cuda.synchronize()
+    n = agent.shape[0]
+    n_agents = n * env.num_agents
+    viol0 = float((r["J0"] > 0).float().mean()) * 100
+    viol = float((r["J"] > 0).float().mean()) * 100
+    print(f"falsify: {n} graphs searched ({args.falsify} iterations), CBF condition violated in {viol0:.3f}% at the "
+          f"start and {viol:.3f}% after the search, largest term {float(r['J'].max()):.4f}, false-safe "
+          f"{r['false_safe0'] / n_agents * 100:.3f}% at the start and {r['false_safe'] / n_agents * 100:.3f}% at the "
+          f"found states")
+    out_dir = os.path.join(path, "falsify")
+    os.makedirs(out_dir, exist_ok=True)
+    f_out = os.path.join(out_dir, f"step{step}.npz")
+    np.savez_compressed(f_out, **{k: v.cpu().numpy() for k, v in r.items() if torch.is_tensor(v)},
+                        goal=goal.cpu().numpy(), false_safe0=r["false_safe0"], false_safe=r["false_safe"],
+                        n_iter=args.falsify)
+    print(f"falsify results: {f_out}")
+
+
 def check_refine_flags(args) -> None:
     """--online-refine refines a trained GCBF+ policy: it needs --path and excludes --u-ref and the baselines."""
     if not args.online_refine:
@@ -306,7 +358,7 @@ FLAGS = [
     (("--cpu",), "flag", False), (("--u-ref",), "flag", False), (("--env",), str, None), (("--algo",), str, None),
     (("--step",), int, None), (("--epi",), int, 5), (("--offset",), int, 0), (("--no-video",), "flag", False),
     (("--nojit-rollout",), "flag", False), (("--log",), "flag", False), (("--dpi",), int, 100),
-    (("--online-refine",), "flag", False), (("--qp-filter",), "flag", False),
+    (("--online-refine",), "flag", False), (("--qp-filter",), "flag", False), (("--falsify",), int, None),
 ]
 
 
