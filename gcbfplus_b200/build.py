@@ -24,8 +24,12 @@ COMMON = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "-Xcompiler",
 UNITS = {  # translation unit -> extra flags
     "api.cu": [],
     "cbfqp.cu": ["-fmad=false"],
+    "dense.cu": ["-fmad=false"],
+    "falsify.cu": ["-fmad=false"],
     "geometry.cu": ["-fmad=false"],
     "gnn.cu": ["-fmad=false"],
+    "qp.cu": ["-fmad=false"],
+    "refine.cu": ["-fmad=false"],
     "rollout_persist.cu": ["-fmad=false"],
     "train.cu": ["-fmad=false"],
 }

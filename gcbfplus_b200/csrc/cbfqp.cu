@@ -18,7 +18,7 @@
 //
 // Both controllers solve   min 1/2 |u|^2 - u_ref.u + 5 |r|^2 + 1000 sum r   s.t.  -Lg u - r <= b,  |u| <= u_lim,
 // r >= 0 (H = diag(1.., 10..), H > 0: the minimiser is unique).  The reference hands it to JaxProxQP with
-// max_iter = 100; here it is solved exactly on the dual, as qp.cuh does for the GCBF+ labels: with multipliers
+// max_iter = 100; here it is solved exactly on the dual, as qp.cu does for the GCBF+ labels: with multipliers
 // lam >= 0 the inner minimisers are closed-form, u(lam) = clip(u_ref + Lg^T lam), r(lam) = max(0, (lam - 1000) / 10),
 // and an accelerated projected-gradient ascent with gradient restart runs on the row-scaled dual in fp64.
 //   DecShareCBF: one 3-row problem per agent (own Lg block only), b = resp (Lf_h + alpha h), resp = 1 for an

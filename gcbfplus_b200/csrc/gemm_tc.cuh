@@ -15,6 +15,8 @@
 // step j + 1 overlaps the MMAs of step j -- and runs the epilogue straight from the accumulator registers.
 // Persistent tile loop; M may come from a device counter (edge count) so the launch is CUDA-graph friendly.
 // gemm_tn_tc_kernel (weight gradient) is described at its definition.
+// This header holds the device code the kernels share with the persistent rollout kernel and the tensor-map helpers;
+// the kernels and their launchers are in dense.cu.
 #pragma once
 #include <cuda.h>
 
@@ -237,16 +239,6 @@ __device__ __forceinline__ void frag_relu_dot(const float (&d)[64], const float*
         }
 }
 
-// Weights are split once per parameter update (gcbf_prepare_params_l); activations are split in shared memory.
-static __global__ void split_tf32_kernel(const float* __restrict__ in, float* __restrict__ hi, float* __restrict__ lo, int n) {
-    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-        const float x = in[i];
-        const float h = rn_tf32(x);
-        hi[i] = h;
-        lo[i] = rn_tf32(x - h);
-    }
-}
-
 // Main loop of one 128 x 128 tile whose A arrives by TMA (stage layout A | (unused) | B hi | B lo, A as plain fp32):
 // each consumer thread loads its A fragment of a k8 step from the fp32 tile -- for one k8 step the 8 rows of a quad
 // column sit in 8 distinct 16-byte chunks of the swizzled rows, so the loads are free of bank conflicts -- splits it
@@ -282,102 +274,6 @@ __device__ __forceinline__ void tma_a_mainloop(float (&d)[64], uint8_t* smem, ui
     }
     wg_wait<0>();
     mbar_arrive(&empty[(it - 1) % STAGES]);
-}
-
-template <int EPI, bool ACCUM>
-__global__ void __launch_bounds__(THREADS_NN, 1)
-gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmBh,
-               const __grid_constant__ CUtensorMap tmBl, const float* __restrict__ bias,
-               const float* __restrict__ bias2, float* __restrict__ C, const float* __restrict__ aux,
-               const int32_t* __restrict__ m_ptr, const int m_fixed, const int m_cap, const int K, const int N,
-               const int ndot) {
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = smem_align1024(smem_raw);
-    uint64_t* full = reinterpret_cast<uint64_t*>(smem + STAGES * STG);   // [STAGES] TMA bytes landed
-    uint64_t* empty = full + STAGES;                                      // [STAGES] MMAs of the stage retired
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int tiles_n = N / BN;                // 1, or 2 for a 256-wide layer
-    const int nkb = K / BK;
-
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < STAGES; ++s) {
-            mbar_init(&full[s], 1);
-            mbar_init(&empty[s], CONSUMERS);
-        }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncthreads();
-    int M = m_ptr ? *m_ptr : m_fixed;
-    M = min(M, m_cap);
-    const int n_tiles = ((M + BM - 1) / BM) * tiles_n;
-
-    if (warp == 8) {
-        // ================= TMA producer =================
-        if (lane == 0) {
-            uint32_t it = 0;
-            for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-                const int m0 = (tile / tiles_n) * BM, n0 = (tile % tiles_n) * BN;
-                for (int kb = 0; kb < nkb; ++kb, ++it) {
-                    const int s = it % STAGES;
-                    mbar_wait(&empty[s], ((it / STAGES) & 1) ^ 1);
-                    uint8_t* st = smem + s * STG;
-                    mbar_expect_tx(&full[s], 3 * PLANE);
-                    tma_load_2d(st, &tmA, &full[s], kb * BK, m0);
-                    tma_load_2d(st + 2 * PLANE, &tmBh, &full[s], kb * BK, n0);
-                    tma_load_2d(st + 3 * PLANE, &tmBl, &full[s], kb * BK, n0);
-                }
-            }
-        }
-        return;
-    }
-    // ================= consumers: A split, MMAs, epilogue =================
-    const int g = warp >> 2, wt = threadIdx.x & 127;
-    uint32_t it = 0;
-    for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-        const int m0 = (tile / tiles_n) * BM, n0 = (tile % tiles_n) * BN;
-        float d[64];
-        tma_a_mainloop(d, smem, full, empty, it, nkb, g, wt);
-
-        const int r0 = m0 + 64 * g + frag_row0(wt);
-        if (EPI == EPI_RELU_DOTN) {   // output-layer partial sums over this column tile
-            float q[2][4];
-            frag_relu_dot<4>(d, bias + n0, aux + (size_t)n0 * ndot, ndot, ndot, wt, q);
-            if ((lane & 3) == 0)
-#pragma unroll
-                for (int h = 0; h < 2; ++h)
-                    if (r0 + 8 * h < M)
-                        *reinterpret_cast<float4*>(C + ((size_t)(n0 / BN) * m_cap + r0 + 8 * h) * 4) =
-                            make_float4(q[h][0], q[h][1], q[h][2], q[h][3]);
-            continue;
-        }
-#pragma unroll
-        for (int i = 0; i < 64; i += 2) {
-            const int m = r0 + 8 * ((i >> 1) & 1);
-            if (m >= M) continue;
-            const int n = n0 + frag_col(wt, i);
-            float2 o = make_float2(d[i], d[i + 1]);
-            if (EPI == EPI_BIAS || EPI == EPI_BIAS_RELU) {
-                const float2 bb = *reinterpret_cast<const float2*>(bias + n);
-                o.x += bb.x; o.y += bb.y;
-                if (bias2) {
-                    const float2 b2 = *reinterpret_cast<const float2*>(bias2 + n);
-                    o.x += b2.x; o.y += b2.y;
-                }
-                if (EPI == EPI_BIAS_RELU) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); }
-            } else if (EPI == EPI_RELU_MASK) {
-                const float2 mk = *reinterpret_cast<const float2*>(aux + (size_t)m * N + n);
-                o.x = mk.x > 0.f ? o.x : 0.f;
-                o.y = mk.y > 0.f ? o.y : 0.f;
-            }
-            float2* cp = reinterpret_cast<float2*>(C + (size_t)m * N + n);
-            if (ACCUM) {
-                const float2 old = *cp;
-                o.x += old.x; o.y += old.y;
-            }
-            *cp = o;
-        }
-    }
 }
 
 // ---- host side ----------------------------------------------------------------------------------
@@ -445,293 +341,6 @@ inline int32_t make_map_stack(CUtensorMap* map, const float* ptr, int rows, int 
         return -2;
     }
     return 0;
-}
-
-template <int EPI, bool ACC>
-inline void launch_nn_inst(int grid, cudaStream_t st, const CUtensorMap& tmA, const CUtensorMap& tmB,
-                           const CUtensorMap& tmBl, const float* bias, const float* bias2, float* C, const float* aux,
-                           RowCount rc, int K, int N, int ndot) {
-    constexpr int smem = STAGES * STG + 1024 + 256;
-    auto kern = gemm_tc_kernel<EPI, ACC>;
-    static bool attr_done = false;
-    if (!attr_done) {
-        cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-        attr_done = true;
-    }
-    kern<<<grid, THREADS_NN, smem, st>>>(tmA, tmB, tmBl, bias, bias2, C, aux, rc.ptr, rc.fixed, rc.cap, K, N, ndot);
-}
-
-// C[M,N] = epi(A[M,K] @ Bt[N,K]^T) with Bt given as its tf32 split (Bt_hi + Bt_lo, split_tf32_kernel).
-// A must be backed by at least rc.cap rows.  A 256-wide layer runs as two 128-wide column tiles; EPI_RELU_DOTN writes
-// one partial sum per column tile (*parts_out = N / BN).
-inline int32_t launch_gemm_tc(int epi, bool accum, const float* A, const float* Bt_hi, const float* Bt_lo,
-                              const float* bias, const float* bias2, float* C, const float* aux, RowCount rc, int K,
-                              int N, cudaStream_t st, int ndot = 0, int* parts_out = nullptr) {
-    if (K % BK != 0 || (N != 128 && N != 256) || ndot > 4) {
-        set_error("gemm_tc: K=%d N=%d epi=%d unsupported", K, N, epi);
-        return -1;
-    }
-    if (parts_out) *parts_out = N / BN;
-    const int rows = rc.ptr ? rc.cap : min(rc.fixed, rc.cap);
-    if (rows <= 0) return 0;
-    const int tiles_m = (rows + BM - 1) / BM;
-    CUtensorMap tmA, tmB, tmBl;
-    if (int32_t r = make_map(&tmA, A, rc.cap, K, BM)) return r;
-    if (int32_t r = make_map(&tmB, Bt_hi, N, K, BN)) return r;
-    if (int32_t r = make_map(&tmBl, Bt_lo, N, K, BN)) return r;
-    const int grid = min(tiles_m * (N / BN), sm_count());
-#define GCBF_TC_CASE(E, ACC) launch_nn_inst<E, ACC>(grid, st, tmA, tmB, tmBl, bias, bias2, C, aux, rc, K, N, ndot)
-    if (!accum) {
-        switch (epi) {
-            case EPI_BIAS: GCBF_TC_CASE(EPI_BIAS, false); break;
-            case EPI_BIAS_RELU: GCBF_TC_CASE(EPI_BIAS_RELU, false); break;
-            case EPI_NONE: GCBF_TC_CASE(EPI_NONE, false); break;
-            case EPI_RELU_MASK: GCBF_TC_CASE(EPI_RELU_MASK, false); break;
-            case EPI_RELU_DOTN: GCBF_TC_CASE(EPI_RELU_DOTN, false); break;
-            default: set_error("bad epilogue"); return -1;
-        }
-    } else {
-        switch (epi) {
-            case EPI_NONE: GCBF_TC_CASE(EPI_NONE, true); break;
-            case EPI_RELU_MASK: GCBF_TC_CASE(EPI_RELU_MASK, true); break;
-            default: set_error("bad accumulate epilogue"); return -1;
-        }
-    }
-#undef GCBF_TC_CASE
-    count_launch();
-    return check_launch("gemm_tc_kernel");
-}
-
-
-// =====================================================================================================
-// backward-weight on tensor cores:  C[K1, N] += sum_m w(m) X[m, k1] dY[m, n]
-// D[128 k1-rows, BN n-columns] += A B^T with A = X^T and B = dY^T: the MMA-K index is the row index m of X / dY.
-// tf32 wgmma reads both operands K-major only, so TMA lands plain [32 m x 32] boxes of X and dY (a "raw" ring of
-// 2 stages) and the consumers transpose them while splitting into K-major SWIZZLE_128B hi / lo planes ([128 k1][32 m]
-// and [BN n][32 m]; double-buffered for BN = 128, single for BN = 256).  Rows m >= M are selected to zero (they may
-// hold stale data, possibly NaN), dY is scaled by the row weight, and the column sums sum_m w(m) dY[m, n] are taken
-// from the very values converted.  Split over M: CTA (tile, split) walks 32-row chunks {split, split + S, ...}.  With
-// more than one split each CTA stores its tile (and its column sums) to a workspace and partial_sum_kernel adds the
-// splits to C in split order: no float atomics, the same bits on every run.
-// =====================================================================================================
-constexpr int TN_RAWS = 2;
-
-template <int BNT>
-struct TnCfg {
-    static constexpr int NH = BNT / 128;                     // 128-wide accumulators per warpgroup
-    static constexpr int PB = (BNT == 256) ? 1 : 2;          // plane buffers
-    static constexpr int RAW = (4 + BNT / 32) * 4096;        // 4 boxes of X, BNT / 32 boxes of dY
-    static constexpr int PLANES = 2 * PLANE + 2 * BNT * 128; // A hi | A lo | B hi | B lo
-    static constexpr int SMEM = TN_RAWS * RAW + PB * PLANES + 1024 + 256;
-};
-
-// `cs1` / `cs2` (optional): column sums sum_m w(m) dY[m, n] -- the bias gradient of the same layer (and the agent
-// one-hot row of the update layer) -- accumulated by the converting threads, so no separate pass over dY is needed.
-// Only the CTAs of k1-tile 0 contribute.
-// `part` (splits > 1): CTA (tile, split) stores its tile to part[split][K1][N] and its column sums to
-// part[split][K1 * N + n] (stride K1 * N + N); otherwise (one split) it adds them to C / cs1 / cs2 itself.
-template <int BNT>
-__global__ void __launch_bounds__(THREADS_NN, 1)
-gemm_tn_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmY,
-                  float* __restrict__ C, const float* __restrict__ roww, const int32_t* __restrict__ row2agent,
-                  const int32_t* __restrict__ m_ptr, const int m_fixed, const int m_cap, const int N, const int splits,
-                  const int n_agents_total, float* __restrict__ cs1, float* __restrict__ cs2, const int K1,
-                  float* __restrict__ part) {
-    using CF = TnCfg<BNT>;
-    constexpr int MR = 32 * BNT / 256;                       // m rows of dY converted per thread
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = smem_align1024(smem_raw);
-    uint8_t* planes = smem + TN_RAWS * CF::RAW;
-    uint64_t* full = reinterpret_cast<uint64_t*>(planes + CF::PB * CF::PLANES);
-    uint64_t* empty = full + TN_RAWS;
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    int M = m_ptr ? *m_ptr : m_fixed;
-    M = min(M, m_cap);
-    const int tile = blockIdx.x / splits, split = blockIdx.x % splits;
-    const int k1_0 = tile * 128;
-    const int n_chunks = (M + 31) / 32;
-    const int n_my = (split < n_chunks) ? (n_chunks - split + splits - 1) / splits : 0;
-
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < TN_RAWS; ++s) {
-            mbar_init(&full[s], 1);
-            mbar_init(&empty[s], CONSUMERS);
-        }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncthreads();
-
-    if (warp == 8) {
-        if (lane == 0) {
-            for (int it = 0; it < n_my; ++it) {
-                const int s = it % TN_RAWS;
-                const int m0 = (split + it * splits) * 32;
-                mbar_wait(&empty[s], ((it / TN_RAWS) & 1) ^ 1);
-                uint8_t* st = smem + s * CF::RAW;
-                mbar_expect_tx(&full[s], CF::RAW);
-#pragma unroll
-                for (int i = 0; i < 4; ++i) tma_load_2d(st + i * 4096, &tmX, &full[s], k1_0 + 32 * i, m0);
-#pragma unroll
-                for (int j = 0; j < BNT / 32; ++j) tma_load_2d(st + (4 + j) * 4096, &tmY, &full[s], 32 * j, m0);
-            }
-        }
-        return;
-    }
-    const int t = threadIdx.x;                 // 0..255
-    const int g = warp >> 2, wt = t & 127;
-    const int xk = t & 127, xm = (t >> 7) * 16;          // X: column k1 = xk, rows xm .. xm + 15
-    const int yn = t % BNT, ym = (t / BNT) * MR;         // dY: column n = yn, rows ym .. ym + MR - 1
-    const bool do_cs = (cs1 != nullptr) && tile == 0;
-    float csum = 0.f;
-    float d[CF::NH][64];
-#pragma unroll
-    for (int h = 0; h < CF::NH; ++h)
-#pragma unroll
-        for (int i = 0; i < 64; ++i) d[h][i] = 0.f;
-    for (int it = 0; it < n_my; ++it) {
-        const int s = it % TN_RAWS;
-        const int m0 = (split + it * splits) * 32;
-        uint8_t* raw = smem + s * CF::RAW;
-        uint8_t* pl = planes + (it % CF::PB) * CF::PLANES;
-        mbar_wait(&full[s], (it / TN_RAWS) & 1);
-        bar_consumers();                       // the MMAs that last read this plane buffer have retired in both warpgroups
-        {   // X -> A planes [k1][m]
-            const float* xs = reinterpret_cast<const float*>(raw + (xk >> 5) * 4096) + (xk & 31);
-#pragma unroll
-            for (int c = 0; c < 4; ++c) {
-                float v[4];
-#pragma unroll
-                for (int j = 0; j < 4; ++j) {
-                    const int m = xm + 4 * c + j;
-                    v[j] = (m0 + m < M) ? xs[m * 32] : 0.f;
-                }
-                float4 h, l;
-                split_tf32(make_float4(v[0], v[1], v[2], v[3]), h, l);
-                const int off = swz(xk, (xm >> 2) + c);
-                *reinterpret_cast<float4*>(pl + off) = h;
-                *reinterpret_cast<float4*>(pl + PLANE + off) = l;
-            }
-        }
-        {   // dY (scaled by the row weight) -> B planes [n][m]
-            const float* ys = reinterpret_cast<const float*>(raw + (4 + (yn >> 5)) * 4096) + (yn & 31);
-            uint8_t* bh = pl + 2 * PLANE;
-            uint8_t* bl = bh + BNT * 128;
-#pragma unroll
-            for (int c = 0; c < MR / 4; ++c) {
-                float v[4];
-#pragma unroll
-                for (int j = 0; j < 4; ++j) {
-                    const int m = ym + 4 * c + j;
-                    const int gm = m0 + m;
-                    float y = 0.f;
-                    if (gm < M) {
-                        float w = 1.f;
-                        if (roww) {
-                            int ag = row2agent ? row2agent[gm] : gm;
-                            ag = min(max(ag, 0), n_agents_total - 1);
-                            w = roww[ag];
-                        }
-                        y = ys[m * 32] * w;
-                    }
-                    csum += y;
-                    v[j] = y;
-                }
-                float4 h, l;
-                split_tf32(make_float4(v[0], v[1], v[2], v[3]), h, l);
-                const int off = swz(yn, (ym >> 2) + c);
-                *reinterpret_cast<float4*>(bh + off) = h;
-                *reinterpret_cast<float4*>(bl + off) = l;
-            }
-        }
-        fence_async_smem();
-        bar_consumers();
-        mbar_arrive(&empty[s]);                // raw stage consumed
-        wg_fence();
-        const uint32_t a_hi = smem_u32(pl) + g * WG_ROWS_BYTES;
-        const uint32_t b_hi = smem_u32(pl) + 2 * PLANE;
-#pragma unroll
-        for (int h = 0; h < CF::NH; ++h)
-            mma_kblock(d[h], a_hi, a_hi + PLANE, b_hi + h * 128 * 128, b_hi + BNT * 128 + h * 128 * 128, it == 0);
-        wg_commit();
-        wg_wait<CF::PB - 1>();
-    }
-    wg_wait<0>();
-    if (n_my == 0) return;
-    if (do_cs) {
-        bar_consumers();                       // every MMA has retired: the plane buffers are free
-        float* s_cs = reinterpret_cast<float*>(planes);
-        s_cs[t] = csum;                        // [t / BNT][n]
-        bar_consumers();
-        if (t < BNT) {
-            float v = s_cs[t];
-            if (BNT == 128) v += s_cs[t + 128];
-            if (part) {
-                part[(size_t)split * ((size_t)K1 * N + N) + (size_t)K1 * N + t] = v;
-            } else {
-                cs1[t] += v;
-                if (cs2) cs2[t] += v;
-            }
-        }
-    }
-    float* dst = part ? part + (size_t)split * ((size_t)K1 * N + N) : C;
-    const int r0 = 64 * g + frag_row0(wt);
-#pragma unroll
-    for (int h = 0; h < CF::NH; ++h)
-#pragma unroll
-        for (int i = 0; i < 64; i += 2) {
-            float2* p = reinterpret_cast<float2*>(dst + (size_t)(k1_0 + r0 + 8 * ((i >> 1) & 1)) * N + h * 128 + frag_col(wt, i));
-            float2 v = make_float2(d[h][i], d[h][i + 1]);
-            if (!part) {
-                const float2 o = *p;
-                v.x += o.x;
-                v.y += o.y;
-            }
-            *p = v;
-        }
-}
-
-// C[K1, N] += sum_m w(m) X[m, :K1] dY[m, :N]; X row stride ldx (>= K1, multiple of 4), K1 % 128 == 0, N in {128, 256}.
-// cs1 / cs2 (optional): += sum_m w(m) dY[m, :N] (bias gradient fused into the same pass over dY).
-// `part` (optional, PART_FLOATS): split-M over up to DW_MAX_CTAS_TC CTAs with an ordered reduction of the splits;
-// without it one CTA per 128-row tile of C walks all rows.
-inline int32_t launch_gemm_tn_tc(const float* X, int ldx, const float* dY, float* C, const float* roww,
-                                 const int32_t* row2agent, RowCount rc, int K1, int N, int n_agents_total,
-                                 cudaStream_t st, float* cs1 = nullptr, float* cs2 = nullptr, float* part = nullptr) {
-    if (K1 % 128 != 0 || (N != 128 && N != 256) || ldx % 4 != 0) {
-        set_error("gemm_tn_tc: K1=%d N=%d ldx=%d unsupported", K1, N, ldx);
-        return -1;
-    }
-    const int rows = rc.ptr ? rc.cap : min(rc.fixed, rc.cap);
-    if (rows <= 0) return 0;
-    CUtensorMap tmX, tmY;
-    if (int32_t r = make_map_box(&tmX, X, rc.cap, K1, ldx, 32, 32, CU_TENSOR_MAP_SWIZZLE_NONE)) return r;
-    if (int32_t r = make_map_box(&tmY, dY, rc.cap, N, N, 32, 32, CU_TENSOR_MAP_SWIZZLE_NONE)) return r;
-    const int tiles = K1 / 128;
-    const int chunks = (rows + 31) / 32;
-    int splits = max(1, sm_count() / tiles);
-    splits = min(splits, max(1, chunks * 32 / 128));       // >= 128 rows per CTA
-    splits = part ? min(splits, max(1, DW_MAX_CTAS_TC / tiles)) : 1;
-    float* kpart = splits > 1 ? part : nullptr;
-    const int grid = tiles * splits;
-#define GCBF_TN_CASE(BN_)                                                                                             \
-    do {                                                                                                              \
-        constexpr int smem = TnCfg<BN_>::SMEM;                                                                        \
-        static bool done = false;                                                                                     \
-        if (!done) { cudaFuncSetAttribute(gemm_tn_tc_kernel<BN_>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem); done = true; } \
-        gemm_tn_tc_kernel<BN_><<<grid, THREADS_NN, smem, st>>>(tmX, tmY, C, roww, row2agent, rc.ptr, rc.fixed, rc.cap, N, \
-                                                               splits, n_agents_total, cs1, cs2, K1, kpart);          \
-    } while (0)
-    if (N == 256) GCBF_TN_CASE(256);
-    else GCBF_TN_CASE(128);
-#undef GCBF_TN_CASE
-    count_launch();
-    if (int32_t r = check_launch("gemm_tn_tc_kernel")) return r;
-    if (splits == 1) return 0;
-    PartSegs segs;
-    segs.add(C, K1 * N);
-    if (cs1) segs.add(cs1, N, cs2);
-    return launch_partial_sum(part, (int64_t)K1 * N + N, splits, segs, st, rc.ptr, rc.cap, 32);
 }
 
 }  // namespace tc

@@ -6,10 +6,10 @@
 //
 // Each consumer thread computes the elements of its own register A fragment (two edge rows, 4 columns per k8 step),
 // splits them into tf32 hi / lo and feeds them to the register-A form of wgmma; B (weights, pre-split) arrives by TMA.
+// The device functions here are shared by edge_chain_kernel (gnn.cu) and the persistent rollout kernel.
 #pragma once
 #include "gemm_tc.cuh"
 #include "gnn.cuh"
-#include "internal.cuh"
 
 namespace gcbf {
 namespace tc {
@@ -159,152 +159,6 @@ __device__ __forceinline__ void edge_tile_mainloop(float (&d)[64], uint8_t* smem
     }
     wg_wait<0>();
     mbar_arrive(&empty[(it - 1) % STAGES]);
-}
-
-// edge message GEMM + chained gate GEMM (see ChainArgs).  Barriers: full / empty = the 3-stage ring of W23 planes;
-// main_done = both warpgroups' main-loop MMAs retired (stage 2 free for the gate weights); b2_full / b2_empty = the two
-// gate-weight slots; t2f = the chained GEMM retired (the stages may be refilled for the next tile).
-template <int KIND>
-__global__ void __launch_bounds__(THREADS_NN, 1)
-edge_chain_kernel(const __grid_constant__ CUtensorMap tmBh, const __grid_constant__ CUtensorMap tmBl,
-                  const __grid_constant__ CUtensorMap tmB2h, const __grid_constant__ CUtensorMap tmB2l,
-                  const __grid_constant__ ProdArgs pa, const float* __restrict__ bias, float* __restrict__ C,
-                  const int32_t* __restrict__ m_ptr, const int m_cap, const ChainArgs ch) {
-    constexpr int ED = EnvTraits<KIND>::ED;
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = smem_align1024(smem_raw);
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * STG);
-    uint64_t* full = bars;                 // [3]
-    uint64_t* empty = bars + 3;            // [3]
-    uint64_t* b2_full = bars + 6;          // [2]
-    uint64_t* b2_empty = bars + 8;         // [2]
-    uint64_t* main_done = bars + 10;
-    uint64_t* t2f = bars + 11;
-    float* sW = reinterpret_cast<float*>(smem + STAGES * STG + 256);
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < 3; ++s) {
-            mbar_init(&full[s], 1);
-            mbar_init(&empty[s], CONSUMERS);
-        }
-        for (int i = 0; i < 2; ++i) {
-            mbar_init(&b2_full[i], 1);
-            mbar_init(&b2_empty[i], CONSUMERS);
-        }
-        mbar_init(main_done, CONSUMERS);
-        mbar_init(t2f, CONSUMERS);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    load_l1_table<ED>(sW, pa.W1, pa.b1, threadIdx.x, blockDim.x);
-    __syncthreads();
-    const int M = min(*m_ptr, m_cap);
-    const int n_tiles = (M + BM - 1) / BM;
-
-    if (warp == 8) {
-        if (lane == 0) {
-            uint32_t it = 0, tc_ = 0;
-            for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++tc_) {
-                if (tc_ > 0) mbar_wait(t2f, (tc_ - 1) & 1);       // the previous tile's chained GEMM still reads the stages
-                for (int kb = 0; kb < 8; ++kb, ++it) {
-                    const int s = it % STAGES;
-                    mbar_wait(&empty[s], ((it / STAGES) & 1) ^ 1);
-                    uint8_t* st = smem + s * STG;
-                    mbar_expect_tx(&full[s], 2 * PLANE);
-                    tma_load_2d(st + 2 * PLANE, &tmBh, &full[s], kb * BK, 0);
-                    tma_load_2d(st + 3 * PLANE, &tmBl, &full[s], kb * BK, 0);
-                }
-                mbar_wait(main_done, tc_ & 1);                    // main-loop MMAs retired: stage 2 is free
-                for (int kb2 = 0; kb2 < 4; ++kb2) {
-                    const uint32_t j2 = tc_ * 4 + kb2, slot = j2 & 1, use = j2 >> 1;
-                    mbar_wait(&b2_empty[slot], (use & 1) ^ 1);
-                    uint8_t* sl = smem + 2 * STG + slot * 32768;
-                    mbar_expect_tx(&b2_full[slot], 32768);
-                    tma_load_2d(sl, &tmB2h, &b2_full[slot], kb2 * BK, 0);
-                    tma_load_2d(sl + 16384, &tmB2l, &b2_full[slot], kb2 * BK, 0);
-                }
-            }
-        }
-        return;
-    }
-    const int g = warp >> 2, wt = threadIdx.x & 127;
-    const int r = 64 * g + frag_row0(wt);      // the thread's fragment rows r, r + 8 of the tile
-    const int rs = r + 8 * setup_row(lane);    // ... and the one it sets up
-    uint32_t it = 0, tc_ = 0;
-    for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++tc_) {
-        const int m0 = tile * BM;
-        float fs[ED], f[2][ED];
-        int ss, stype[2];
-        edge_row_setup<KIND>(pa, m0 + rs, m0 + rs < M, fs, ss);
-        share_rows<ED>(fs, ss, lane, f, stype);
-        const bool ok[2] = {m0 + r < M, m0 + r + 8 < M};
-        float d[64];
-        edge_tile_mainloop<ED>(d, smem, full, empty, it, lane, ok, sW, f, stype);
-        mbar_arrive(main_done);
-        bar_consumers();                       // both warpgroups' main loops retired: the hand-over may overwrite stages 0-1
-        drain_msg(d, smem, g, wt, bias, C + (size_t)m0 * 128, M - m0);
-        fence_async_smem();
-        bar_wg(g);                             // the chained GEMM of warpgroup g reads its own hand-over rows only
-        float d2[64];
-#pragma unroll
-        for (int i = 0; i < 64; ++i) d2[i] = 0.f;
-        for (int kb2 = 0; kb2 < 4; ++kb2) {
-            const uint32_t j2 = tc_ * 4 + kb2, slot = j2 & 1, use = j2 >> 1;
-            mbar_wait(&b2_full[slot], use & 1);
-            wg_fence();
-            chain_kblock(d2, smem, g, kb2, slot);
-            wg_commit();
-            wg_wait<0>();
-            mbar_arrive(&b2_empty[slot]);
-        }
-        float q[2][1];
-        frag_relu_dot<1>(d2, ch.bias_g, ch.avec, 1, 1, wt, q);
-        if ((lane & 3) == 0) {
-            const int rr = m0 + 64 * g + frag_row0(wt);
-            if (rr < M) ch.logits[rr] = q[0][0] + ch.cst[0];
-            if (rr + 8 < M) ch.logits[rr + 8] = q[1][0] + ch.cst[0];
-        }
-        mbar_arrive(t2f);
-    }
-}
-
-constexpr int PROD_SMEM = STAGES * STG + 256 + L1_FLOATS * 4 + 1024;
-
-// MSG[e, :128] = relu-layer-1(edge e) @ W23 + b23: edge_l1 producer + folded message GEMM (K = 256, N = 128), with the
-// gate layer (K = N = 128, weights gate_Bt_*) and its folded gate vector chained in the same kernel: the logits are
-// written to chain.logits.
-inline int32_t launch_edge_msg(const gcbf_env_desc* d, const float* W1, const float* b1, const GraphRefs& g,
-                               int clip_all, const float* Bt_hi, const float* Bt_lo, const float* bias, float* msg,
-                               cudaStream_t st, const float* gate_Bt_hi, const float* gate_Bt_lo,
-                               const ChainArgs& chain) {
-    if (!g.counters) {
-        set_error("launch_edge_msg: the chained gate GEMM needs the device edge counter");
-        return -1;
-    }
-    ProdArgs pa;
-    memset(&pa, 0, sizeof(pa));
-    pa.d = *d;
-    pa.W1 = W1; pa.b1 = b1; pa.agent = g.agent; pa.goal = g.goal; pa.hits = g.hits;
-    pa.edge_recv = g.edge_recv; pa.edge_src = g.edge_src; pa.clip_all = clip_all;
-    const int K = 256, N = 128;
-    CUtensorMap tmB, tmBl, tmG, tmGl;
-    if (int32_t r = make_map(&tmB, Bt_hi, N, K, N)) return r;
-    if (int32_t r = make_map(&tmBl, Bt_lo, N, K, N)) return r;
-    if (int32_t r = make_map(&tmG, gate_Bt_hi, 128, 128, 128)) return r;
-    if (int32_t r = make_map(&tmGl, gate_Bt_lo, 128, 128, 128)) return r;
-    const int grid = min((d->edge_cap + BM - 1) / BM, sm_count());
-    GCBF_DISPATCH_ENV(d->env_kind, {
-        auto kern = edge_chain_kernel<KIND>;
-        static bool attr_done = false;
-        if (!attr_done) {
-            cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, PROD_SMEM);
-            attr_done = true;
-        }
-        kern<<<grid, THREADS_NN, PROD_SMEM, st>>>(tmB, tmBl, tmG, tmGl, pa, bias, msg, g.counters, d->edge_cap, chain);
-        count_launch();
-        return check_launch("edge_chain_kernel");
-    });
-    return -1;
 }
 
 }  // namespace tc

@@ -1,8 +1,9 @@
-// geometry_dev.cuh -- device functions shared by geometry.cu, rollout_persist.cu and train.cu: obstacle primitives
-// (Rectangle / Sphere inside + ray cast), the stable 32-key warp sort of the LiDAR returns, u_ref, the Euler step,
-// their state Jacobians (the CBF-condition gradient of falsify.cuh), the policy tail and reward / cost terms of an env
-// step, and the per-warp pieces of the graph build (2-D LiDAR,
-// active hits, neighbour scan, edge-row fill).  The 5-launch rollout step and the persistent rollout kernel run these
+// geometry_dev.cuh -- device functions shared by geometry.cu, rollout_persist.cu, train.cu, qp.cu, refine.cu and
+// falsify.cu: obstacle primitives (Rectangle / Sphere inside + ray cast), the stable 32-key warp sort of the LiDAR
+// returns, u_ref, the Euler step, their state Jacobians (the CBF-condition gradient of falsify.cu), the chain of the
+// train step's and the refinement's backward through the Euler step (dyn_chain_dev), the policy tail and reward / cost
+// terms of an env step, and the per-warp pieces of the graph build (2-D LiDAR, active hits, neighbour scan, edge-row
+// fill).  The 5-launch rollout step and the persistent rollout kernel run these
 // same functions, which is what keeps the two paths bit-identical.
 // Every including unit is compiled with -fmad=false: every arithmetic step keeps the reference's
 // one-rounding-per-op semantics (bit-exact index sets / hit ordering / masks against the CPU oracle).
@@ -373,6 +374,66 @@ __device__ __forceinline__ void euler_vjp_dev(const gcbf_env_desc& d, const floa
             for (int r = 0; r < SD; ++r) s += dxn[r] * d.B[r * NU + c];
             du[c] = s * d.dt;
         }
+    }
+}
+
+// d_es (edge-state grads of x') -> d a.   x' = clip_state(x + xdot(x, u) dt), u = clip_action(a)
+// (gcbf_plus.py:386-391; double_integrator.py:128-143,340-354 and twins): the chain edge state -> state ->
+// clip_state -> Euler -> clip_action of agent `a`, shared by the train step and the policy refinement.
+template <int KIND>
+__device__ __forceinline__ void dyn_chain_dev(const gcbf_env_desc& d, const float* agent, const float* goal,
+                                              const float* action, const float* xnext, const float* d_es, const int a,
+                                              float* g) {
+    using T = EnvTraits<KIND>;
+    constexpr int SD = T::SD, NU = T::NU, ED = T::ED;
+    float dx[SD], xn[SD], de[ED];
+#pragma unroll
+    for (int c = 0; c < ED; ++c) de[c] = d_es[(size_t)a * ED + c];
+#pragma unroll
+    for (int c = 0; c < SD; ++c) xn[c] = xnext[(size_t)a * SD + c];
+    if (KIND == GCBF_ENV_DUBINS_CAR) {  // es = (x, y, v cos th, v sin th)
+        const float th = xn[2], v = xn[3];
+        dx[0] = de[0];
+        dx[1] = de[1];
+        dx[2] = de[2] * (-v * sinf(th)) + de[3] * (v * cosf(th));
+        dx[3] = de[2] * cosf(th) + de[3] * sinf(th);
+    } else {
+#pragma unroll
+        for (int c = 0; c < SD; ++c) dx[c] = de[c];
+    }
+    // clip_state: zero gradient on clipped velocity components
+#pragma unroll
+    for (int c = 0; c < SD; ++c) {
+        const bool limited = (KIND == GCBF_ENV_DOUBLE_INTEGRATOR && c >= 2) || (KIND == GCBF_ENV_DUBINS_CAR && c == 3) ||
+                             (KIND == GCBF_ENV_LINEAR_DRONE && c >= 3);
+        if (limited && !(xn[c] > -d.v_lim && xn[c] < d.v_lim)) dx[c] = 0.f;
+    }
+    float du[NU];
+    if (KIND == GCBF_ENV_SINGLE_INTEGRATOR) {
+        du[0] = dx[0] * d.dt;
+        du[1] = dx[1] * d.dt;
+    } else if (KIND == GCBF_ENV_DOUBLE_INTEGRATOR) {
+        du[0] = dx[2] * d.dt / d.mass;
+        du[1] = dx[3] * d.dt / d.mass;
+    } else if (KIND == GCBF_ENV_DUBINS_CAR) {
+        const float ddx = agent[(size_t)a * SD + 0] - goal[(size_t)a * SD + 0];
+        const float ddy = agent[(size_t)a * SD + 1] - goal[(size_t)a * SD + 1];
+        const float keep = (sqrtf(ddx * ddx + ddy * ddy) < d.half_r) ? 0.f : 1.f;
+        du[0] = dx[2] * 20.f * d.dt * keep;
+        du[1] = dx[3] * d.dt * keep;
+    } else {
+#pragma unroll
+        for (int c = 0; c < NU; ++c) {
+            float s = 0.f;
+#pragma unroll
+            for (int r = 0; r < SD; ++r) s += dx[r] * d.B[r * NU + c];
+            du[c] = s * d.dt;
+        }
+    }
+#pragma unroll
+    for (int c = 0; c < NU; ++c) {
+        const float act = action[(size_t)a * NU + c];
+        g[c] = (act > -d.u_lim && act < d.u_lim) ? du[c] : 0.f;  // clip_action
     }
 }
 

@@ -1,4 +1,6 @@
-// gnn.cu -- GNN forward for one network (CBF h(x) or policy pi(x)) over a swarm batch.
+// gnn.cu -- GNN forward for one network (CBF h(x) or policy pi(x)) over a swarm batch: the non-GEMM layer kernels
+// (edge features + first message layer, attention softmax + aggregation, output head), the edge-message GEMM with the
+// chained gate GEMM, the folded and the unfolded forward, and the rollout step.
 #include "gemm.cuh"
 #include "gemm_tc.cuh"
 #include "gnn.cuh"
@@ -9,78 +11,374 @@
 
 using namespace gcbf;
 
-// ---- building blocks exported for unit tests and for bench.py's isolated kernel timing ----
-extern "C" __attribute__((visibility("default"))) int32_t gcbf_gemm_nn(int32_t epi, int32_t accum, const float* A,
-                                                                       const float* B, const float* bias,
-                                                                       const float* bias2, float* C, const float* aux,
-                                                                       const int32_t* m_ptr, int32_t m_fixed,
-                                                                       int32_t m_cap, int32_t K, int32_t N,
-                                                                       void* stream) {
-    GCBF_REQUIRE(A && B && C, "gcbf_gemm_nn: NULL pointer");
-    GCBF_REQUIRE((epi != EPI_BIAS && epi != EPI_BIAS_RELU) || bias, "gcbf_gemm_nn: bias required");
-    GCBF_REQUIRE(epi != EPI_RELU_MASK || aux, "gcbf_gemm_nn: aux required");
-    return launch_gemm_nn(epi, accum != 0, A, B, bias, bias2, C, aux, RowCount{m_ptr, m_fixed, m_cap}, K, N,
-                          (cudaStream_t)stream);
+namespace gcbf {
+
+// ---- edge features + message layer 1: X1 = relu(feat @ W1[:ed] + W1[ed + sender_type] + W1[ed+3+2] + b1)
+// one warp per edge (grid-stride); lane owns 8 output columns.
+template <int KIND>
+__global__ void __launch_bounds__(256)
+edge_l1_kernel(const gcbf_env_desc d, const float* __restrict__ W1, const float* __restrict__ b1,
+               const float* __restrict__ agent, const float* __restrict__ goal, const float* __restrict__ hits,
+               const int32_t* __restrict__ edge_recv, const int32_t* __restrict__ edge_src,
+               const int32_t* __restrict__ counters, const int clip_all, float* __restrict__ feat_out,
+               float* __restrict__ X1) {
+    using T = EnvTraits<KIND>;
+    constexpr int ED = T::ED, SD = T::SD;
+    __shared__ __align__(16) float sW[ED][256];
+    __shared__ __align__(16) float sB[3][256];  // [hit, goal, agent] sender one-hot rows + receiver row + bias
+    for (int i = threadIdx.x; i < ED * 256; i += blockDim.x) sW[i / 256][i % 256] = W1[i];
+    for (int i = threadIdx.x; i < 3 * 256; i += blockDim.x) {
+        const int t = i / 256, c = i % 256;
+        sB[t][c] = W1[(ED + t) * 256 + c] + W1[(ED + 3 + 2) * 256 + c] + b1[c];
+    }
+    __syncthreads();
+    const int nE = min(counters[0], d.edge_cap);
+    const int A = d.n_graphs * d.n_agents;
+    const int lane = threadIdx.x & 31;
+    const int warps_total = (gridDim.x * blockDim.x) >> 5;
+    for (int e = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; e < nE; e += warps_total) {
+        const int a = min(max(edge_recv[e], 0), A - 1);
+        int code = edge_src[e];
+        code = min(code, A - 1);
+        float er[ED], es[ED], f[ED], coef, nrm;
+        edge_state_dev<KIND>(agent + (size_t)a * SD, er);
+        sender_state_dev<KIND>(code, a, d.n_hits, agent, goal, hits, es);
+        edge_feat_dev<KIND>(er, es, clip_all || code == -1, d.comm_radius, f, &coef, &nrm);
+        const int t = (code >= 0) ? 2 : ((code == -1) ? 1 : 0);
+        if (lane < ED) feat_out[(size_t)e * FEAT_LD + lane] = f[lane];
+        float y[8];
+#pragma unroll
+        for (int j = 0; j < 8; ++j) y[j] = sB[t][lane * 8 + j];
+#pragma unroll
+        for (int c = 0; c < ED; ++c) {
+#pragma unroll
+            for (int j = 0; j < 8; ++j) y[j] = fmaf(f[c], sW[c][lane * 8 + j], y[j]);
+        }
+        float4* dst = reinterpret_cast<float4*>(X1 + (size_t)e * 256 + lane * 8);
+        dst[0] = make_float4(fmaxf(y[0], 0.f), fmaxf(y[1], 0.f), fmaxf(y[2], 0.f), fmaxf(y[3], 0.f));
+        dst[1] = make_float4(fmaxf(y[4], 0.f), fmaxf(y[5], 0.f), fmaxf(y[6], 0.f), fmaxf(y[7], 0.f));
+    }
 }
 
-extern "C" __attribute__((visibility("default"))) int32_t gcbf_gemm_tn(const float* X, int32_t ldx, const float* dY,
-                                                                       float* C, const float* roww,
-                                                                       const int32_t* row2agent, const int32_t* m_ptr,
-                                                                       int32_t m_fixed, int32_t m_cap, int32_t K1,
-                                                                       int32_t N, int32_t n_agents_total, void* stream) {
-    GCBF_REQUIRE(X && dY && C, "gcbf_gemm_tn: NULL pointer");
-    return launch_gemm_tn(X, ldx, dY, C, roww, row2agent, RowCount{m_ptr, m_fixed, m_cap}, K1, N, n_agents_total,
-                          (cudaStream_t)stream);
+// ---- gate logit + segment softmax + weighted aggregation (gnn.py:64-72); warp per receiver.
+// gate = G2 @ a3 + ba3 ; att = softmax over the receiver's edges ; AG[a] = sum att * MSG.
+static __global__ void __launch_bounds__(256)
+attn_aggregate_kernel(const int A, const int edge_cap, const float* __restrict__ G2, const float* __restrict__ MSG,
+                      const float* __restrict__ a3, const float* __restrict__ ba3,
+                      const int32_t* __restrict__ row_start, const int32_t* __restrict__ row_deg,
+                      float* __restrict__ ATT, float* __restrict__ AG, int32_t* __restrict__ zero_counter = nullptr) {
+    // G2 == nullptr (inference): ATT already holds the gate logits (written by tc::edge_chain_kernel) and is
+    // left as it is.  Otherwise (training) the gate logits are computed here and ATT receives the attention weights
+    // that the backward pass reads.
+    // zero_counter (rollout step): edge counter of the NEXT graph, cleared here so that no memset node sits in the
+    // per-step kernel chain (the graph build two kernels later accumulates into it)
+    if (zero_counter && blockIdx.x == 0 && threadIdx.x == 0) zero_counter[0] = 0;
+    const int lane = threadIdx.x & 31;
+    const int warps_total = (gridDim.x * blockDim.x) >> 5;
+    const float4 w = G2 ? *reinterpret_cast<const float4*>(a3 + lane * 4) : make_float4(0.f, 0.f, 0.f, 0.f);
+    const float bias = G2 ? ba3[0] : 0.f;
+    for (int a = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; a < A; a += warps_total) {
+        const int rs = row_start[a];
+        int rd = row_deg[a];
+        if (rs < 0 || rs + rd > edge_cap) rd = 0;
+        if (!G2) {
+            *reinterpret_cast<float4*>(AG + (size_t)a * 128 + lane * 4) = aggregate_logits(rs, rd, ATT, MSG, lane);
+            continue;
+        }
+        if (rd <= 4) {
+            // training fast path: the gate rows and the message rows of all (<= 4) edges are requested up front and the
+            // 4 dot products are reduced together; same arithmetic order as the general path below
+            float sg[4];
+            float4 mv[4];
+#pragma unroll
+            for (int q = 0; q < 4; ++q) {
+                const int e = rs + min(q, max(rd - 1, 0));
+                const bool on = q < rd;
+                const float4 g = on ? *reinterpret_cast<const float4*>(G2 + (size_t)e * 128 + lane * 4)
+                                    : make_float4(0.f, 0.f, 0.f, 0.f);
+                mv[q] = on ? *reinterpret_cast<const float4*>(MSG + (size_t)e * 128 + lane * 4)
+                           : make_float4(0.f, 0.f, 0.f, 0.f);
+                sg[q] = g.x * w.x + g.y * w.y + g.z * w.z + g.w * w.w;
+            }
+#pragma unroll
+            for (int off = 16; off > 0; off >>= 1)
+#pragma unroll
+                for (int q = 0; q < 4; ++q) sg[q] += __shfl_xor_sync(0xffffffffu, sg[q], off);
+            float mx = -INFINITY;
+#pragma unroll
+            for (int q = 0; q < 4; ++q) {
+                sg[q] = (q < rd) ? sg[q] + bias : -INFINITY;
+                mx = fmaxf(mx, sg[q]);
+            }
+            float den = 0.f;
+#pragma unroll
+            for (int q = 0; q < 4; ++q)
+                if (q < rd) den += expf(sg[q] - mx);
+            float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+            for (int q = 0; q < 4; ++q) {
+                if (q < rd) {
+                    const float att = expf(sg[q] - mx) / den;
+                    acc.x = fmaf(att, mv[q].x, acc.x);
+                    acc.y = fmaf(att, mv[q].y, acc.y);
+                    acc.z = fmaf(att, mv[q].z, acc.z);
+                    acc.w = fmaf(att, mv[q].w, acc.w);
+                    if (lane == 0) ATT[rs + q] = att;
+                }
+            }
+            *reinterpret_cast<float4*>(AG + (size_t)a * 128 + lane * 4) = acc;
+            continue;
+        }
+        float mx = -INFINITY;
+        for (int e = rs; e < rs + rd; ++e) {
+            const float4 g = *reinterpret_cast<const float4*>(G2 + (size_t)e * 128 + lane * 4);
+            float s = g.x * w.x + g.y * w.y + g.z * w.z + g.w * w.w;
+            s = warp_sum(s) + bias;
+            if (lane == 0) ATT[e] = s;
+            mx = fmaxf(mx, s);
+        }
+        __syncwarp();
+        float den = 0.f;
+        for (int e = rs; e < rs + rd; ++e) den += expf(ATT[e] - mx);
+        float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+        for (int e = rs; e < rs + rd; ++e) {
+            const float att = expf(ATT[e] - mx) / den;
+            const float4 m = *reinterpret_cast<const float4*>(MSG + (size_t)e * 128 + lane * 4);
+            acc.x = fmaf(att, m.x, acc.x);
+            acc.y = fmaf(att, m.y, acc.y);
+            acc.z = fmaf(att, m.z, acc.z);
+            acc.w = fmaf(att, m.w, acc.w);
+            __syncwarp();
+            if (lane == 0) ATT[e] = att;
+        }
+        *reinterpret_cast<float4*>(AG + (size_t)a * 128 + lane * 4) = acc;
+    }
 }
 
-extern "C" __attribute__((visibility("default"))) int32_t gcbf_colsum(const float* dY, float* db, const float* roww,
-                                                                      const int32_t* row2agent, const int32_t* m_ptr,
-                                                                      int32_t m_fixed, int32_t m_cap, int32_t N,
-                                                                      int32_t n_agents_total, void* stream) {
-    GCBF_REQUIRE(dY && db, "gcbf_colsum: NULL pointer");
-    return launch_colsum(dY, db, roww, row2agent, RowCount{m_ptr, m_fixed, m_cap}, N, n_agents_total,
-                         (cudaStream_t)stream);
+// ---- output layer pre-activations z[a][0..3] = H @ W[256, nout] (no bias / tanh): SIMT-path producer of the
+// policy tail's input (the tensor-core path gets it from the EPI_RELU_DOTN epilogue).  Warp per agent.
+static __global__ void __launch_bounds__(256)
+head_z_kernel(const int A, const int nout, const float* __restrict__ H, const float* __restrict__ W,
+              float* __restrict__ z) {
+    const int lane = threadIdx.x & 31;
+    const int warps_total = (gridDim.x * blockDim.x) >> 5;
+    for (int a = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; a < A; a += warps_total) {
+        const float4 h0 = *reinterpret_cast<const float4*>(H + (size_t)a * 256 + lane * 8);
+        const float4 h1 = *reinterpret_cast<const float4*>(H + (size_t)a * 256 + lane * 8 + 4);
+        const float hv[8] = {h0.x, h0.y, h0.z, h0.w, h1.x, h1.y, h1.z, h1.w};
+        float out[4] = {0.f, 0.f, 0.f, 0.f};
+        for (int j = 0; j < nout; ++j) {
+            float s = 0.f;
+#pragma unroll
+            for (int k = 0; k < 8; ++k) s = fmaf(hv[k], W[(lane * 8 + k) * nout + j], s);
+            out[j] = warp_sum(s);
+        }
+        if (lane == 0) *reinterpret_cast<float4*>(z + (size_t)a * 4) = make_float4(out[0], out[1], out[2], out[3]);
+    }
 }
 
-// ---- tensor-core (wgmma 3xTF32) variant of gcbf_gemm_nn: C = epi(A[M,K] @ Bt[N,K]^T) ----
-extern "C" __attribute__((visibility("default"))) int32_t gcbf_gemm_tc(int32_t epi, int32_t accum, const float* A,
-                                                                       const float* Bt_hi, const float* Bt_lo,
-                                                                       const float* bias,
-                                                                       const float* bias2, float* C, const float* aux,
-                                                                       const int32_t* m_ptr, int32_t m_fixed,
-                                                                       int32_t m_cap, int32_t K, int32_t N,
-                                                                       int32_t ndot, void* stream) {
-    GCBF_REQUIRE(A && Bt_hi && Bt_lo && C, "gcbf_gemm_tc: NULL pointer");
-    GCBF_REQUIRE(epi != EPI_RELU_DOTN || (bias && aux), "gcbf_gemm_tc: bias and aux required");
-    GCBF_REQUIRE(epi != EPI_RELU_DOTN || (ndot >= 1 && ndot <= 4), "gcbf_gemm_tc: ndot must be in [1, 4]");
-    GCBF_REQUIRE((epi != EPI_BIAS && epi != EPI_BIAS_RELU) || bias, "gcbf_gemm_tc: bias required");
-    GCBF_REQUIRE(epi != EPI_RELU_MASK || aux, "gcbf_gemm_tc: aux required");
-    GCBF_REQUIRE((((uintptr_t)A | (uintptr_t)Bt_hi | (uintptr_t)Bt_lo | (uintptr_t)C) & 15) == 0,
-                 "gcbf_gemm_tc: 16-byte alignment required");
-    return gcbf::tc::launch_gemm_tc(epi, accum != 0, A, Bt_hi, Bt_lo, bias, bias2, C, aux,
-                                    RowCount{m_ptr, m_fixed, m_cap}, K, N, (cudaStream_t)stream, ndot);
+// ---- output head: out = tanh(H2 @ W[256, nout] + b); warp per agent.
+static __global__ void __launch_bounds__(256)
+head_out_kernel(const int A, const int nout, const float* __restrict__ H2, const float* __restrict__ W,
+                const float* __restrict__ b, float* __restrict__ out) {
+    const int lane = threadIdx.x & 31;
+    const int warps_total = (gridDim.x * blockDim.x) >> 5;
+    float wl[8][4];
+#pragma unroll
+    for (int k = 0; k < 8; ++k)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) wl[k][j] = (j < nout) ? W[(lane * 8 + k) * nout + j] : 0.f;
+    // four agents per iteration: all eight row loads are in flight before the first reduction (latency-bound loop)
+    for (int a0 = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; a0 < A; a0 += 4 * warps_total) {
+        float4 hq[4][2];
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+            const int a = min(a0 + q * warps_total, A - 1);
+            hq[q][0] = *reinterpret_cast<const float4*>(H2 + (size_t)a * 256 + lane * 8);
+            hq[q][1] = *reinterpret_cast<const float4*>(H2 + (size_t)a * 256 + lane * 8 + 4);
+        }
+        float sv[4][4];
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+            const float hv[8] = {hq[q][0].x, hq[q][0].y, hq[q][0].z, hq[q][0].w, hq[q][1].x, hq[q][1].y, hq[q][1].z, hq[q][1].w};
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                float s = 0.f;
+#pragma unroll
+                for (int k = 0; k < 8; ++k) s = fmaf(hv[k], wl[k][j], s);
+                sv[q][j] = s;
+            }
+        }
+#pragma unroll
+        for (int off = 16; off > 0; off >>= 1)
+#pragma unroll
+            for (int q = 0; q < 4; ++q)
+#pragma unroll
+                for (int j = 0; j < 4; ++j) sv[q][j] += __shfl_xor_sync(0xffffffffu, sv[q][j], off);
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+            const int a = a0 + q * warps_total;
+            if (a < A && lane < nout) {
+                float s = sv[q][0];
+                if (lane == 1) s = sv[q][1];
+                if (lane == 2) s = sv[q][2];
+                if (lane == 3) s = sv[q][3];
+                out[(size_t)a * nout + lane] = tanhf(s + b[lane]);
+            }
+        }
+    }
 }
 
-extern "C" __attribute__((visibility("default"))) int32_t gcbf_split_tf32(const float* in, float* hi, float* lo, int32_t n,
-                                                                          void* stream) {
-    GCBF_REQUIRE(in && hi && lo && n > 0, "gcbf_split_tf32: bad argument");
-    gcbf::tc::split_tf32_kernel<<<min((n + 255) / 256, 4 * sm_count()), 256, 0, (cudaStream_t)stream>>>(in, hi, lo, n);
-    count_launch();
-    return check_launch("split_tf32_kernel");
+namespace tc {
+
+// edge message GEMM + chained gate GEMM (see ChainArgs).  Barriers: full / empty = the 3-stage ring of W23 planes;
+// main_done = both warpgroups' main-loop MMAs retired (stage 2 free for the gate weights); b2_full / b2_empty = the two
+// gate-weight slots; t2f = the chained GEMM retired (the stages may be refilled for the next tile).
+template <int KIND>
+__global__ void __launch_bounds__(THREADS_NN, 1)
+edge_chain_kernel(const __grid_constant__ CUtensorMap tmBh, const __grid_constant__ CUtensorMap tmBl,
+                  const __grid_constant__ CUtensorMap tmB2h, const __grid_constant__ CUtensorMap tmB2l,
+                  const __grid_constant__ ProdArgs pa, const float* __restrict__ bias, float* __restrict__ C,
+                  const int32_t* __restrict__ m_ptr, const int m_cap, const ChainArgs ch) {
+    constexpr int ED = EnvTraits<KIND>::ED;
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = smem_align1024(smem_raw);
+    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * STG);
+    uint64_t* full = bars;                 // [3]
+    uint64_t* empty = bars + 3;            // [3]
+    uint64_t* b2_full = bars + 6;          // [2]
+    uint64_t* b2_empty = bars + 8;         // [2]
+    uint64_t* main_done = bars + 10;
+    uint64_t* t2f = bars + 11;
+    float* sW = reinterpret_cast<float*>(smem + STAGES * STG + 256);
+
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    if (threadIdx.x == 0) {
+        for (int s = 0; s < 3; ++s) {
+            mbar_init(&full[s], 1);
+            mbar_init(&empty[s], CONSUMERS);
+        }
+        for (int i = 0; i < 2; ++i) {
+            mbar_init(&b2_full[i], 1);
+            mbar_init(&b2_empty[i], CONSUMERS);
+        }
+        mbar_init(main_done, CONSUMERS);
+        mbar_init(t2f, CONSUMERS);
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    load_l1_table<ED>(sW, pa.W1, pa.b1, threadIdx.x, blockDim.x);
+    __syncthreads();
+    const int M = min(*m_ptr, m_cap);
+    const int n_tiles = (M + BM - 1) / BM;
+
+    if (warp == 8) {
+        if (lane == 0) {
+            uint32_t it = 0, tc_ = 0;
+            for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++tc_) {
+                if (tc_ > 0) mbar_wait(t2f, (tc_ - 1) & 1);       // the previous tile's chained GEMM still reads the stages
+                for (int kb = 0; kb < 8; ++kb, ++it) {
+                    const int s = it % STAGES;
+                    mbar_wait(&empty[s], ((it / STAGES) & 1) ^ 1);
+                    uint8_t* st = smem + s * STG;
+                    mbar_expect_tx(&full[s], 2 * PLANE);
+                    tma_load_2d(st + 2 * PLANE, &tmBh, &full[s], kb * BK, 0);
+                    tma_load_2d(st + 3 * PLANE, &tmBl, &full[s], kb * BK, 0);
+                }
+                mbar_wait(main_done, tc_ & 1);                    // main-loop MMAs retired: stage 2 is free
+                for (int kb2 = 0; kb2 < 4; ++kb2) {
+                    const uint32_t j2 = tc_ * 4 + kb2, slot = j2 & 1, use = j2 >> 1;
+                    mbar_wait(&b2_empty[slot], (use & 1) ^ 1);
+                    uint8_t* sl = smem + 2 * STG + slot * 32768;
+                    mbar_expect_tx(&b2_full[slot], 32768);
+                    tma_load_2d(sl, &tmB2h, &b2_full[slot], kb2 * BK, 0);
+                    tma_load_2d(sl + 16384, &tmB2l, &b2_full[slot], kb2 * BK, 0);
+                }
+            }
+        }
+        return;
+    }
+    const int g = warp >> 2, wt = threadIdx.x & 127;
+    const int r = 64 * g + frag_row0(wt);      // the thread's fragment rows r, r + 8 of the tile
+    const int rs = r + 8 * setup_row(lane);    // ... and the one it sets up
+    uint32_t it = 0, tc_ = 0;
+    for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++tc_) {
+        const int m0 = tile * BM;
+        float fs[ED], f[2][ED];
+        int ss, stype[2];
+        edge_row_setup<KIND>(pa, m0 + rs, m0 + rs < M, fs, ss);
+        share_rows<ED>(fs, ss, lane, f, stype);
+        const bool ok[2] = {m0 + r < M, m0 + r + 8 < M};
+        float d[64];
+        edge_tile_mainloop<ED>(d, smem, full, empty, it, lane, ok, sW, f, stype);
+        mbar_arrive(main_done);
+        bar_consumers();                       // both warpgroups' main loops retired: the hand-over may overwrite stages 0-1
+        drain_msg(d, smem, g, wt, bias, C + (size_t)m0 * 128, M - m0);
+        fence_async_smem();
+        bar_wg(g);                             // the chained GEMM of warpgroup g reads its own hand-over rows only
+        float d2[64];
+#pragma unroll
+        for (int i = 0; i < 64; ++i) d2[i] = 0.f;
+        for (int kb2 = 0; kb2 < 4; ++kb2) {
+            const uint32_t j2 = tc_ * 4 + kb2, slot = j2 & 1, use = j2 >> 1;
+            mbar_wait(&b2_full[slot], use & 1);
+            wg_fence();
+            chain_kblock(d2, smem, g, kb2, slot);
+            wg_commit();
+            wg_wait<0>();
+            mbar_arrive(&b2_empty[slot]);
+        }
+        float q[2][1];
+        frag_relu_dot<1>(d2, ch.bias_g, ch.avec, 1, 1, wt, q);
+        if ((lane & 3) == 0) {
+            const int rr = m0 + 64 * g + frag_row0(wt);
+            if (rr < M) ch.logits[rr] = q[0][0] + ch.cst[0];
+            if (rr + 8 < M) ch.logits[rr + 8] = q[1][0] + ch.cst[0];
+        }
+        mbar_arrive(t2f);
+    }
 }
-extern "C" __attribute__((visibility("default"))) int32_t gcbf_gemm_tn_tc(const float* X, int32_t ldx, const float* dY,
-                                                                          float* C, const float* roww,
-                                                                          const int32_t* row2agent,
-                                                                          const int32_t* m_ptr, int32_t m_fixed,
-                                                                          int32_t m_cap, int32_t K1, int32_t N,
-                                                                          int32_t n_agents_total, float* cs1, float* cs2,
-                                                                          void* stream) {
-    GCBF_REQUIRE(X && dY && C, "gcbf_gemm_tn_tc: NULL pointer");
-    GCBF_REQUIRE(cs1 || !cs2, "gcbf_gemm_tn_tc: cs2 without cs1");
-    GCBF_REQUIRE((((uintptr_t)X | (uintptr_t)dY | (uintptr_t)C) & 15) == 0, "gcbf_gemm_tn_tc: 16-byte alignment required");
-    return gcbf::tc::launch_gemm_tn_tc(X, ldx, dY, C, roww, row2agent, RowCount{m_ptr, m_fixed, m_cap}, K1, N,
-                                       n_agents_total, (cudaStream_t)stream, cs1, cs2);
+
+constexpr int PROD_SMEM = STAGES * STG + 256 + L1_FLOATS * 4 + 1024;
+
+// MSG[e, :128] = relu-layer-1(edge e) @ W23 + b23: edge_l1 producer + folded message GEMM (K = 256, N = 128), with the
+// gate layer (K = N = 128, weights gate_Bt_*) and its folded gate vector chained in the same kernel: the logits are
+// written to chain.logits.
+static int32_t launch_edge_msg(const gcbf_env_desc* d, const float* W1, const float* b1, const GraphRefs& g,
+                               int clip_all, const float* Bt_hi, const float* Bt_lo, const float* bias, float* msg,
+                               cudaStream_t st, const float* gate_Bt_hi, const float* gate_Bt_lo,
+                               const ChainArgs& chain) {
+    if (!g.counters) {
+        set_error("launch_edge_msg: the chained gate GEMM needs the device edge counter");
+        return -1;
+    }
+    ProdArgs pa;
+    memset(&pa, 0, sizeof(pa));
+    pa.d = *d;
+    pa.W1 = W1; pa.b1 = b1; pa.agent = g.agent; pa.goal = g.goal; pa.hits = g.hits;
+    pa.edge_recv = g.edge_recv; pa.edge_src = g.edge_src; pa.clip_all = clip_all;
+    const int K = 256, N = 128;
+    CUtensorMap tmB, tmBl, tmG, tmGl;
+    if (int32_t r = make_map(&tmB, Bt_hi, N, K, N)) return r;
+    if (int32_t r = make_map(&tmBl, Bt_lo, N, K, N)) return r;
+    if (int32_t r = make_map(&tmG, gate_Bt_hi, 128, 128, 128)) return r;
+    if (int32_t r = make_map(&tmGl, gate_Bt_lo, 128, 128, 128)) return r;
+    const int grid = min((d->edge_cap + BM - 1) / BM, sm_count());
+    GCBF_DISPATCH_ENV(d->env_kind, {
+        auto kern = edge_chain_kernel<KIND>;
+        static bool attr_done = false;
+        if (!attr_done) {
+            cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, PROD_SMEM);
+            attr_done = true;
+        }
+        kern<<<grid, THREADS_NN, PROD_SMEM, st>>>(tmB, tmBl, tmG, tmGl, pa, bias, msg, g.counters, d->edge_cap, chain);
+        count_launch();
+        return check_launch("edge_chain_kernel");
+    });
+    return -1;
 }
+
+}  // namespace tc
+}  // namespace gcbf
 
 // =====================================================================================================
 // Inference path with folded weights.  Every MLP block of the GNN ends in two linear layers with no

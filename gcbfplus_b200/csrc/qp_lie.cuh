@@ -1,5 +1,5 @@
 // qp_lie.cuh -- Lie derivatives of a scalar function of the edge states along the control-affine dynamics
-// (env.control_affine_dyn).  Shared by the GCBF+ QP labels (qp.cuh) and the CBF-QP baselines (cbfqp.cu).
+// (env.control_affine_dyn).  Shared by the GCBF+ QP labels (qp.cu) and the CBF-QP baselines (cbfqp.cu).
 #pragma once
 
 #include "common.cuh"

@@ -5,15 +5,14 @@
 // workspace, then partial_sum_kernel; per-edge input gradients gathered per agent), so the step is bit-identical from
 // run to run for the same inputs on the same GPU model.  On the tensor-core path the step runs on the folded
 // network (gnn_backward_folded / unfold_jobs below: 4 GEMMs per pass and direction instead of
-// 9-10, same gradient); the strict-fp32 SIMT path runs the layer-by-layer step.  The same pieces serve the online
-// policy refinement (refine.cuh) and the CBF condition with its gradient wrt the agent states (falsify.cuh), both
-// included at the end of this unit.
+// 9-10, same gradient); the strict-fp32 SIMT path runs the layer-by-layer step.  The same pieces serve the QP labels
+// (qp.cu), the online policy refinement (refine.cu) and the CBF condition with its gradient wrt the agent states
+// (falsify.cu), through internal.cuh.
 //
 // Replaces gcbfplus/algo/gcbf_plus.py:354-447 (update_inner / get_loss / value_and_grad),
 // trainer/utils.py:62-75 (compute_norm_and_clip), optax.adamw + optax.apply_if_finite
 // (gcbf_plus.py:109-110,127-128) and gcbf_plus.py:188-191 (update_tgt).
 #include "gemm.cuh"
-#include "gemm_tc.cuh"
 #include "geometry_dev.cuh"
 #include "gnn.cuh"
 #include "translayout.cuh"
@@ -46,6 +45,16 @@ __global__ void act_dyn_kernel(const gcbf_env_desc d, const float* __restrict__ 
     step_agent<KIND>(d, x, gl, act, ur, true, xn);
 #pragma unroll
     for (int c = 0; c < SD; ++c) xnext[(size_t)a * SD + c] = xn[c];
+}
+
+int32_t launch_act_dyn(const gcbf_env_desc* d, const float* agent, const float* goal, const float* pi, float* action,
+                       float* xnext, cudaStream_t st) {
+    const int A = d->n_graphs * d->n_agents;
+    GCBF_DISPATCH_ENV(d->env_kind, {
+        act_dyn_kernel<KIND><<<(A + 127) / 128, 128, 0, st>>>(*d, agent, goal, pi, action, xnext);
+    });
+    count_launch();
+    return check_launch("act_dyn_kernel");
 }
 
 // ------------------------------------------------------------------------------------ losses (gcbf_plus.py:362-431)
@@ -515,66 +524,6 @@ edge_grad_gather_kernel(const int A, const int edge_cap, const int32_t* __restri
     for (int c = 0; c < ED; ++c) d_es[(size_t)a * ED + c] = s[c];
 }
 
-// d_es (edge-state grads of x') -> d a.   x' = clip_state(x + xdot(x, u) dt), u = clip_action(a)
-// (gcbf_plus.py:386-391; double_integrator.py:128-143,340-354 and twins): the chain edge state -> state ->
-// clip_state -> Euler -> clip_action of agent `a`, shared by the train step and the policy refinement.
-template <int KIND>
-__device__ __forceinline__ void dyn_chain_dev(const gcbf_env_desc& d, const float* agent, const float* goal,
-                                              const float* action, const float* xnext, const float* d_es, const int a,
-                                              float* g) {
-    using T = EnvTraits<KIND>;
-    constexpr int SD = T::SD, NU = T::NU, ED = T::ED;
-    float dx[SD], xn[SD], de[ED];
-#pragma unroll
-    for (int c = 0; c < ED; ++c) de[c] = d_es[(size_t)a * ED + c];
-#pragma unroll
-    for (int c = 0; c < SD; ++c) xn[c] = xnext[(size_t)a * SD + c];
-    if (KIND == GCBF_ENV_DUBINS_CAR) {  // es = (x, y, v cos th, v sin th)
-        const float th = xn[2], v = xn[3];
-        dx[0] = de[0];
-        dx[1] = de[1];
-        dx[2] = de[2] * (-v * sinf(th)) + de[3] * (v * cosf(th));
-        dx[3] = de[2] * cosf(th) + de[3] * sinf(th);
-    } else {
-#pragma unroll
-        for (int c = 0; c < SD; ++c) dx[c] = de[c];
-    }
-    // clip_state: zero gradient on clipped velocity components
-#pragma unroll
-    for (int c = 0; c < SD; ++c) {
-        const bool limited = (KIND == GCBF_ENV_DOUBLE_INTEGRATOR && c >= 2) || (KIND == GCBF_ENV_DUBINS_CAR && c == 3) ||
-                             (KIND == GCBF_ENV_LINEAR_DRONE && c >= 3);
-        if (limited && !(xn[c] > -d.v_lim && xn[c] < d.v_lim)) dx[c] = 0.f;
-    }
-    float du[NU];
-    if (KIND == GCBF_ENV_SINGLE_INTEGRATOR) {
-        du[0] = dx[0] * d.dt;
-        du[1] = dx[1] * d.dt;
-    } else if (KIND == GCBF_ENV_DOUBLE_INTEGRATOR) {
-        du[0] = dx[2] * d.dt / d.mass;
-        du[1] = dx[3] * d.dt / d.mass;
-    } else if (KIND == GCBF_ENV_DUBINS_CAR) {
-        const float ddx = agent[(size_t)a * SD + 0] - goal[(size_t)a * SD + 0];
-        const float ddy = agent[(size_t)a * SD + 1] - goal[(size_t)a * SD + 1];
-        const float keep = (sqrtf(ddx * ddx + ddy * ddy) < d.half_r) ? 0.f : 1.f;
-        du[0] = dx[2] * 20.f * d.dt * keep;
-        du[1] = dx[3] * d.dt * keep;
-    } else {
-#pragma unroll
-        for (int c = 0; c < NU; ++c) {
-            float s = 0.f;
-#pragma unroll
-            for (int r = 0; r < SD; ++r) s += dx[r] * d.B[r * NU + c];
-            du[c] = s * d.dt;
-        }
-    }
-#pragma unroll
-    for (int c = 0; c < NU; ++c) {
-        const float act = action[(size_t)a * NU + c];
-        g[c] = (act > -d.u_lim && act < d.u_lim) ? du[c] : 0.f;  // clip_action
-    }
-}
-
 // train step: a = 2 pi + u_ref, so d_pi = 2 (da_dyn + da_direct).
 template <int KIND>
 __global__ void dyn_bwd_kernel(const gcbf_env_desc d, const float* __restrict__ agent, const float* __restrict__ goal,
@@ -591,30 +540,7 @@ __global__ void dyn_bwd_kernel(const gcbf_env_desc d, const float* __restrict__ 
 }
 
 // ------------------------------------------------------------------------------------ one network backward
-// Built by aggregate initialisation, in this order.
-struct BwdArgs {
-    const gcbf_env_desc* d;
-    GraphRefs g;           // the graph of the forward pass
-    float* gw;             // gradient workspace (make_ws layout)
-    float* part;           // PART_FLOATS: per-CTA partials of the weight-gradient reductions (when G is set)
-    int use_tc;            // 1: backward-data GEMMs on the wgmma path
-    int out_dim;
-    const float* P;        // parameters
-    const float* PT;       // backward-data B operands (prepare_bwd_operands)
-    const float* fw;       // forward workspace (saved activations)
-    const float* out;      // network output (tanh applied) [A, out_dim]
-    const float* d_out;    // upstream gradient wrt the output [A, out_dim]
-    const float* roww;     // optional per-agent weights applied to every dW / db contribution
-    float* G;              // parameter gradient (accumulated); nullptr: data-only backward
-    int clip_all;
-    float* d_es;           // optional [A, ED] (written): gradient wrt the agents' edge states, gathered from `je`
-    float* je;             // [cap, 8] when d_es is wanted or the per-edge blocks are the result: d out[recv] / d feat_e
-    const int32_t* agent_rows = nullptr;   // optional device row count of the agent-row GEMMs (default: every agent)
-};
-
-// Backward-data B operands of a one-layer network: the straight tf32 planes (build_planes) on the tensor-core path,
-// W^T (TransLayout) on the SIMT path.
-static int32_t prepare_bwd_operands(int ed, int out_dim, int use_tc, const float* P, float* PT, cudaStream_t st) {
+int32_t prepare_bwd_operands(int ed, int out_dim, int use_tc, const float* P, float* PT, cudaStream_t st) {
     if (use_tc) return build_planes(ed, out_dim, 1, P, PT, st);
     const ParamLayout L = make_layout(ed, out_dim);
     return build_transposes(L, make_trans_layout(L), P, PT, st);
@@ -709,7 +635,7 @@ static int32_t dense_bwd_data(const BwdArgs& b, const ParamLayout& L, const int*
     return launch_gemm_nn(epi, accum, dY, B, nullptr, nullptr, dX, aux, rc, K, N, st);
 }
 
-static int32_t gnn_backward_impl(const BwdArgs& b, cudaStream_t st) {
+int32_t gnn_backward_impl(const BwdArgs& b, cudaStream_t st) {
     const gcbf_env_desc* d = b.d;
     const int ed = env_ed(d->env_kind);
     const ParamLayout L = make_layout(ed, b.out_dim);
@@ -943,42 +869,6 @@ __global__ void polyak_kernel(float* __restrict__ tgt, const float* __restrict__
         tgt[i] = tau * src[i] + (1.f - tau) * tgt[i];
 }
 
-}  // namespace gcbf
-#include "qp.cuh"
-#include "refine.cuh"
-#include "falsify.cuh"
-namespace gcbf {
-
-// ------------------------------------------------------------------------------------ QP label workspace layout
-struct QpWs {
-    int64_t ws0, gws, pt_cbf, h, ones, je, qb, qs, qe, ur, qsc, rev, total;
-};
-static QpWs make_qp_ws(const gcbf_env_desc* d) {
-    const int ed = env_ed(d->env_kind);
-    const int64_t A = (int64_t)d->n_graphs * d->n_agents, cap = d->edge_cap;
-    const GnnWs W = make_ws(d->edge_cap, A);
-    QpWs t;
-    WsSlots S{8};   // 32-byte slots: 256-bit epilogue stores
-    t.ws0 = S.take(W.total);
-    t.gws = S.take(W.total);
-    t.pt_cbf = S.take(make_plane_layout(make_deep_layout(ed, 1, 1), ed).total);   // also holds the SIMT TransLayout
-    t.h = S.take(A);
-    t.ones = S.take(A);
-    t.je = S.take(cap * 8);
-    t.qb = S.take(A);
-    t.qs = S.take(A * 4);
-    t.qe = S.take(cap * 4);
-    t.ur = S.take(A * 4);
-    t.qsc = S.take(A);
-    t.rev = S.take(cap);
-    t.total = S.off;
-    return t;
-}
-
-__global__ void fill_kernel(float* __restrict__ p, const int n, const float v) {
-    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) p[i] = v;
-}
-
 // ------------------------------------------------------------------------------------ train workspace layout
 // One parameter region per network, holding what the step of its GEMM path needs: the SIMT step the transposed
 // weights (TransLayout, at `pt`), the folded tensor-core step [folded blob (InferLayout) at `pt` | gradient of the
@@ -1122,11 +1012,7 @@ extern "C" __attribute__((visibility("default"))) int32_t gcbf_train_step(
     };
     RC(forward(1, cbf_params, blob_c, g, 0, ws + TW.h, ws + TW.ws0));
     RC(forward(nu, actor_params, blob_a, g, 0, ws + TW.pi, ws + TW.ws1));
-    GCBF_DISPATCH_ENV(d->env_kind, {
-        act_dyn_kernel<KIND><<<(A + 127) / 128, 128, 0, st>>>(*d, agent, goal, ws + TW.pi, ws + TW.act, ws + TW.xn);
-    });
-    count_launch();
-    RC(check_launch("act_dyn_kernel"));
+    RC(launch_act_dyn(d, agent, goal, ws + TW.pi, ws + TW.act, ws + TW.xn, st));
     RC(forward(1, cbf_params, blob_c, gn, 1, ws + TW.hn, ws + TW.ws2));
     // ---- losses and their derivatives wrt h, h', a
     {
@@ -1207,304 +1093,4 @@ extern "C" __attribute__((visibility("default"))) int32_t gcbf_polyak(float* tgt
     polyak_kernel<<<min((n + 1023) / 1024, 2 * sm_count()), 256, 0, (cudaStream_t)stream>>>(tgt, src, n, tau);
     count_launch();
     return check_launch("polyak_kernel");
-}
-
-// ------------------------------------------------------------------------------------ QP action labels
-extern "C" __attribute__((visibility("default"))) int64_t gcbf_qp_workspace_floats(const gcbf_env_desc* desc) {
-    return graph_desc_ok(desc) ? make_qp_ws(desc).total : -1;
-}
-
-extern "C" __attribute__((visibility("default"))) int32_t gcbf_qp_workspace_layout(const gcbf_env_desc* desc,
-                                                                                   int64_t* offsets8_host) {
-    GCBF_REQUIRE(offsets8_host, "gcbf_qp_workspace_layout: bad argument");
-    if (int32_t rc = check_graph_desc(desc, "gcbf_qp_workspace_layout")) return rc;
-    const QpWs Q = make_qp_ws(desc);
-    const int64_t o[8] = {Q.h, Q.je, Q.qb, Q.qs, Q.qe, Q.ur, Q.qsc, Q.rev};
-    for (int i = 0; i < 8; ++i) offsets8_host[i] = o[i];
-    return 0;
-}
-
-// The QP of the labels with the nominal action u_nom in place of u_ref (u_nom == NULL: u_ref, the labels themselves).
-static int32_t qp_solve(const char* name, const gcbf_env_desc* desc, float alpha, int32_t use_tensor_cores,
-                        int32_t max_iter, float tol, const float* cbf_params, const float* agent, const float* goal,
-                        const float* hits, const int32_t* row_start, const int32_t* row_deg, const int32_t* edge_recv,
-                        const int32_t* edge_src, const int32_t* counters, const float* u_nom, float* u_qp, float* aux,
-                        int32_t* iters, float* workspace, int64_t workspace_floats, void* stream) {
-    GCBF_REQUIRE(desc && cbf_params && agent && goal && hits && row_start && row_deg && edge_recv && edge_src &&
-                     counters && u_qp && workspace, "%s: NULL pointer argument", name);
-    if (int32_t rc = check_graph_desc(desc, name)) return rc;
-    GCBF_REQUIRE(desc->n_agents <= QP_MAX_AGENTS, "%s: n_agents %d > %d not supported", name, desc->n_agents,
-                 QP_MAX_AGENTS);
-    GCBF_REQUIRE(max_iter > 0 && tol >= 0.f, "%s: bad solver settings", name);
-    const QpWs Q = make_qp_ws(desc);
-    GCBF_REQUIRE(workspace_floats >= Q.total, "qp workspace too small: %lld < %lld floats", (long long)workspace_floats,
-                 (long long)Q.total);
-    GCBF_REQUIRE(((uintptr_t)workspace & 15) == 0 && ((uintptr_t)cbf_params & 15) == 0, "buffers must be 16-byte aligned");
-    cudaStream_t st = (cudaStream_t)stream;
-    const gcbf_env_desc* d = desc;
-    const int ed = env_ed(d->env_kind), nu = env_nu(d->env_kind);
-    const int A = d->n_graphs * d->n_agents, N = d->n_agents;
-    float* ws = workspace;
-    const GraphRefs g{agent, goal, hits, row_start, row_deg, edge_recv, edge_src, counters};
-    int32_t rc;
-#define RC(x) do { if ((rc = (x))) return rc; } while (0)
-    RC(prepare_bwd_operands(ed, 1, use_tensor_cores, cbf_params, ws + Q.pt_cbf, st));
-    // h = cbf(add_edge_feats(graph, x)): every edge feature norm-clipped (gcbf_plus.py:310-316)
-    RC(gnn_forward(d, 1, 1, cbf_params, use_tensor_cores ? ws + Q.pt_cbf : nullptr, g, 1, ws + Q.h, nullptr, ws + Q.ws0,
-                   st));
-    fill_kernel<<<min((A + 255) / 256, 2 * sm_count()), 256, 0, st>>>(ws + Q.ones, A, 1.f);
-    count_launch();
-    RC(check_launch("fill_kernel"));
-    // Jacobian: data-only backward with upstream 1, kept per edge
-    RC(gnn_backward_impl({d, g, ws + Q.gws, nullptr, use_tensor_cores, 1, cbf_params, ws + Q.pt_cbf, ws + Q.ws0, ws + Q.h,
-                          ws + Q.ones, nullptr, nullptr, 1, nullptr, ws + Q.je}, st));
-    int32_t* rev = reinterpret_cast<int32_t*>(ws + Q.rev);
-    GCBF_DISPATCH_ENV(d->env_kind, {
-        qp_assemble_kernel<KIND><<<(A + 127) / 128, 128, 0, st>>>(*d, alpha, agent, goal, ws + Q.h, ws + Q.je, row_start,
-                                                                  row_deg, edge_src, u_nom, ws + Q.qb, ws + Q.qs,
-                                                                  ws + Q.qe, ws + Q.ur, ws + Q.qsc, rev);
-    });
-    count_launch();
-    RC(check_launch("qp_assemble_kernel"));
-    const int nt = min(1024, (N + 31) / 32 * 32);
-    // compacted agent-agent blocks per graph kept in shared memory: N (N - 1) at most, 24 per agent is generous for
-    // radius graphs, and whatever fits under the 227 KB limit; denser graphs iterate on the global edge list.
-    int nbr_cap = (int)min((int64_t)N * (N - 1), (int64_t)24 * N);
-    const size_t smem_base = qp_solve_smem(N, nu, 0), entry = sizeof(int) + 2 * nu * sizeof(float);
-    const size_t smem_max = 200 * 1024;
-    if (smem_base + (size_t)nbr_cap * entry > smem_max) nbr_cap = (int)((smem_max - smem_base) / entry);
-    nbr_cap = max(nbr_cap, 1);
-    const size_t smem = qp_solve_smem(N, nu, nbr_cap);
-    cudaError_t e;
-#define QP_LAUNCH(NUv)                                                                                                  \
-    do {                                                                                                                \
-        if ((e = cudaFuncSetAttribute(qp_solve_kernel<NUv>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)) !=  \
-            cudaSuccess) {                                                                                              \
-            set_error("cudaFuncSetAttribute(qp_solve_kernel): %s", cudaGetErrorString(e));                              \
-            return (int32_t)e;                                                                                          \
-        }                                                                                                               \
-        qp_solve_kernel<NUv><<<d->n_graphs, nt, smem, st>>>(N, d->edge_cap, nbr_cap, d->u_lim, max_iter, tol, ws + Q.qb,  \
-                                                            ws + Q.qs, ws + Q.qe, ws + Q.ur, ws + Q.qsc, rev, row_start, \
-                                                            row_deg, edge_src, u_qp, aux, iters);                       \
-    } while (0)
-    if (nu == 2) QP_LAUNCH(2);
-    else QP_LAUNCH(3);
-#undef QP_LAUNCH
-    count_launch();
-    RC(check_launch("qp_solve_kernel"));
-#undef RC
-    return 0;
-}
-
-extern "C" __attribute__((visibility("default"))) int32_t gcbf_qp_labels(
-    const gcbf_env_desc* desc, float alpha, int32_t use_tensor_cores, int32_t max_iter, float tol,
-    const float* cbf_params, const float* agent, const float* goal, const float* hits, const int32_t* row_start,
-    const int32_t* row_deg, const int32_t* edge_recv, const int32_t* edge_src, const int32_t* counters, float* u_qp,
-    float* aux, int32_t* iters, float* workspace, int64_t workspace_floats, void* stream) {
-    return qp_solve("gcbf_qp_labels", desc, alpha, use_tensor_cores, max_iter, tol, cbf_params, agent, goal, hits,
-                    row_start, row_deg, edge_recv, edge_src, counters, nullptr, u_qp, aux, iters, workspace,
-                    workspace_floats, stream);
-}
-
-extern "C" __attribute__((visibility("default"))) int32_t gcbf_qp_filter(
-    const gcbf_env_desc* desc, float alpha, int32_t use_tensor_cores, int32_t max_iter, float tol,
-    const float* cbf_params, const float* agent, const float* goal, const float* hits, const int32_t* row_start,
-    const int32_t* row_deg, const int32_t* edge_recv, const int32_t* edge_src, const int32_t* counters,
-    const float* u_nom, float* u, float* aux, int32_t* iters, float* workspace, int64_t workspace_floats,
-    void* stream) {
-    return qp_solve("gcbf_qp_filter", desc, alpha, use_tensor_cores, max_iter, tol, cbf_params, agent, goal, hits,
-                    row_start, row_deg, edge_recv, edge_src, counters, u_nom, u, aux, iters, workspace,
-                    workspace_floats, stream);
-}
-
-// ------------------------------------------------------------------------------------ online policy refinement
-extern "C" __attribute__((visibility("default"))) int32_t gcbf_refine_prepare(int32_t edge_dim, int32_t use_tensor_cores,
-                                                                              const float* cbf_params, float* prepared,
-                                                                              void* stream) {
-    GCBF_REQUIRE(cbf_params && prepared && (edge_dim == 2 || edge_dim == 4 || edge_dim == 6),
-                 "gcbf_refine_prepare: bad argument");
-    GCBF_REQUIRE((((uintptr_t)cbf_params | (uintptr_t)prepared) & 15) == 0, "buffers must be 16-byte aligned");
-    return prepare_bwd_operands(edge_dim, 1, use_tensor_cores, cbf_params, prepared, (cudaStream_t)stream);
-}
-
-extern "C" __attribute__((visibility("default"))) int64_t gcbf_refine_workspace_floats(const gcbf_env_desc* desc) {
-    return graph_desc_ok(desc) ? make_refine_ws(desc).total : -1;
-}
-
-extern "C" __attribute__((visibility("default"))) int32_t gcbf_refine_actions(
-    const gcbf_env_desc* desc, float alpha, float lr, int32_t max_iter, int32_t use_tensor_cores,
-    const float* cbf_params, const float* cbf_prepared, const float* pi, const float* agent, const float* goal,
-    const float* hits, const int32_t* row_start, const int32_t* row_deg, const int32_t* edge_recv,
-    const int32_t* edge_src, const int32_t* counters, float* action, float* value, int32_t* iters, float* workspace,
-    int64_t workspace_floats, void* stream) {
-    GCBF_REQUIRE(desc && cbf_params && cbf_prepared && pi && agent && goal && hits && row_start && row_deg &&
-                     edge_recv && edge_src && counters && action && workspace, "gcbf_refine_actions: NULL pointer argument");
-    if (int32_t rc = check_graph_desc(desc, "gcbf_refine_actions")) return rc;
-    GCBF_REQUIRE(desc->dt > 0.f, "gcbf_refine_actions: bad descriptor (dt %g)", (double)desc->dt);
-    GCBF_REQUIRE(max_iter > 0 && isfinite(lr) && isfinite(alpha), "gcbf_refine_actions: bad settings (max_iter %d)",
-                 max_iter);
-    const RefineWs R = make_refine_ws(desc);
-    GCBF_REQUIRE(workspace_floats >= R.total, "refine workspace too small: %lld < %lld floats",
-                 (long long)workspace_floats, (long long)R.total);
-    GCBF_REQUIRE((((uintptr_t)workspace | (uintptr_t)cbf_params | (uintptr_t)cbf_prepared) & 15) == 0,
-                 "buffers must be 16-byte aligned");
-    cudaStream_t st = (cudaStream_t)stream;
-    const gcbf_env_desc* d = desc;
-    const int nu = env_nu(d->env_kind);
-    const int G = d->n_graphs, N = d->n_agents, A = G * N;
-    const int blocks = (A + 127) / 128;
-    float* ws = workspace;
-    int32_t* active = reinterpret_cast<int32_t*>(ws + R.active);
-    int32_t* upd = reinterpret_cast<int32_t*>(ws + R.upd);
-    int32_t* rows = reinterpret_cast<int32_t*>(ws + R.rows);
-    const float* PT = cbf_prepared;
-    int32_t rc;
-#define RC(x) do { if ((rc = (x))) return rc; } while (0)
-    // g: the graph; gn: its edges over the next states x'; gr: the same with the refinement steps' device edge count
-    const GraphRefs g{agent, goal, hits, row_start, row_deg, edge_recv, edge_src, counters};
-    const GraphRefs gn = g.with_agent(ws + R.xn);
-    GraphRefs gr = gn;
-    gr.counters = rows;
-    auto forward = [&](const GraphRefs& on, int clip_all, const int32_t* arows, float* out) -> int32_t {
-        return gnn_forward(d, 1, 1, cbf_params, use_tensor_cores ? PT : nullptr, on, clip_all, out, nullptr, ws + R.fw,
-                           st, arows);
-    };
-    // 1. h = cbf(g) on the graph's own edge features
-    RC(forward(g, 0, nullptr, ws + R.h));
-    // 2. h(g'(u_ref)), every edge feature recomputed and norm-clipped (forward_graph)
-    GCBF_DISPATCH_ENV(d->env_kind, {
-        refine_next_state_kernel<KIND><<<blocks, 128, 0, st>>>(*d, nullptr, agent, goal, nullptr, ws + R.ur, ws + R.xn);
-    });
-    count_launch();
-    RC(check_launch("refine_next_state_kernel"));
-    RC(forward(gn, 1, nullptr, ws + R.hn));
-    // 3. per-agent selection of the starting action; every graph active
-    if (nu == 2)
-        refine_init_kernel<2><<<blocks, 128, 0, st>>>(G, A, alpha, d->dt, ws + R.h, ws + R.hn, ws + R.ur, pi, counters,
-                                                      action, active, rows);
-    else
-        refine_init_kernel<3><<<blocks, 128, 0, st>>>(G, A, alpha, d->dt, ws + R.h, ws + R.hn, ws + R.ur, pi, counters,
-                                                      action, active, rows);
-    count_launch();
-    RC(check_launch("refine_init_kernel"));
-    // 4. the refinement steps: data-only backward of h' into the edge-state gradient of x' (same as the QP labels'
-    //    Jacobian pass, gathered per agent), then the chain into the action
-    const BwdArgs b{d, gr, ws + R.gw, nullptr, use_tensor_cores, 1, cbf_params, PT, ws + R.fw, ws + R.hn, ws + R.dhn,
-                    nullptr, nullptr, 1, ws + R.d_es, ws + R.je, rows + 1};
-    for (int it = 0; it < max_iter; ++it) {
-        GCBF_DISPATCH_ENV(d->env_kind, {
-            refine_next_state_kernel<KIND><<<blocks, 128, 0, st>>>(*d, rows, agent, goal, action, nullptr, ws + R.xn);
-        });
-        count_launch();
-        RC(check_launch("refine_next_state_kernel"));
-        RC(forward(gr, 1, rows + 1, ws + R.hn));
-        refine_value_kernel<<<G, REFINE_VALUE_THREADS, 0, st>>>(N, env_sd(d->env_kind), alpha, d->dt, it, max_iter,
-                                                                ws + R.h, ws + R.hn, ws + R.xn, ws + R.dhn, active,
-                                                                upd, value, iters);
-        count_launch();
-        RC(check_launch("refine_value_kernel"));
-        RC(gnn_backward_impl(b, st));
-        GCBF_DISPATCH_ENV(d->env_kind, {
-            refine_update_kernel<KIND><<<blocks, 128, 0, st>>>(*d, lr, agent, goal, ws + R.xn, ws + R.d_es, active, upd,
-                                                               counters, rows, action);
-        });
-        count_launch();
-        RC(check_launch("refine_update_kernel"));
-    }
-#undef RC
-    return 0;
-}
-
-// ------------------------------------------------------------------------------------ CBF condition + state gradient
-extern "C" __attribute__((visibility("default"))) int32_t gcbf_cbf_condition_prepare(int32_t edge_dim, int32_t out_dim,
-                                                                                     int32_t use_tensor_cores,
-                                                                                     const float* params,
-                                                                                     float* prepared,
-                                                                                     int64_t prepared_floats,
-                                                                                     void* stream) {
-    GCBF_REQUIRE(params && prepared && (edge_dim == 2 || edge_dim == 4 || edge_dim == 6) && out_dim >= 1 && out_dim <= 3,
-                 "gcbf_cbf_condition_prepare: bad argument");
-    GCBF_REQUIRE((((uintptr_t)params | (uintptr_t)prepared) & 15) == 0, "buffers must be 16-byte aligned");
-    const ParamLayout L = make_layout(edge_dim, out_dim);
-    const int64_t need = use_tensor_cores ? make_plane_layout(make_deep_layout(edge_dim, out_dim, 1), edge_dim).total
-                                          : make_trans_layout(L).total;
-    GCBF_REQUIRE(prepared_floats >= need, "gcbf_cbf_condition_prepare: buffer too small: %lld < %lld floats",
-                 (long long)prepared_floats, (long long)need);
-    return prepare_bwd_operands(edge_dim, out_dim, use_tensor_cores, params, prepared, (cudaStream_t)stream);
-}
-
-extern "C" __attribute__((visibility("default"))) int64_t gcbf_cbf_condition_workspace_floats(const gcbf_env_desc* desc) {
-    return graph_desc_ok(desc) ? make_falsify_ws(desc).total : -1;
-}
-
-extern "C" __attribute__((visibility("default"))) int32_t gcbf_cbf_condition(
-    const gcbf_env_desc* desc, float alpha, int32_t use_tensor_cores, const float* cbf_params, const float* cbf_planes,
-    const float* actor_params, const float* actor_planes, const float* agent, const float* goal, const float* hits,
-    const int32_t* row_start, const int32_t* row_deg, const int32_t* edge_recv, const int32_t* edge_src,
-    const int32_t* counters, float* h, float* term, int32_t* worst, float* grad_x, float* workspace,
-    int64_t workspace_floats, void* stream) {
-    GCBF_REQUIRE(desc && cbf_params && cbf_planes && actor_params && actor_planes && agent && goal && hits &&
-                     row_start && row_deg && edge_recv && edge_src && counters && h && term && worst && workspace,
-                 "gcbf_cbf_condition: NULL pointer argument");
-    if (int32_t rc = check_graph_desc(desc, "gcbf_cbf_condition")) return rc;
-    GCBF_REQUIRE(desc->dt > 0.f && isfinite(alpha), "gcbf_cbf_condition: bad settings (dt %g, alpha %g)",
-                 (double)desc->dt, (double)alpha);
-    const FalsifyWs F = make_falsify_ws(desc);
-    GCBF_REQUIRE(workspace_floats >= F.total, "cbf condition workspace too small: %lld < %lld floats",
-                 (long long)workspace_floats, (long long)F.total);
-    GCBF_REQUIRE((((uintptr_t)workspace | (uintptr_t)cbf_params | (uintptr_t)cbf_planes | (uintptr_t)actor_params |
-                   (uintptr_t)actor_planes) & 15) == 0, "buffers must be 16-byte aligned");
-    cudaStream_t st = (cudaStream_t)stream;
-    const gcbf_env_desc* d = desc;
-    const int nu = env_nu(d->env_kind);
-    const int G = d->n_graphs, N = d->n_agents, A = G * N;
-    const int blocks = (A + 127) / 128;
-    float* ws = workspace;
-    int32_t rc;
-#define RC(x) do { if ((rc = (x))) return rc; } while (0)
-    // g: the graph; gn: its edges over the next states x' (forward_graph: every feature norm-clipped)
-    const GraphRefs g{agent, goal, hits, row_start, row_deg, edge_recv, edge_src, counters};
-    const GraphRefs gn = g.with_agent(ws + F.xn);
-    auto forward = [&](int out_dim, const float* P, const float* PT, const GraphRefs& on, int clip_all, float* out,
-                       float* fws) -> int32_t {
-        return gnn_forward(d, out_dim, 1, P, use_tensor_cores ? PT : nullptr, on, clip_all, out, nullptr, fws, st);
-    };
-    // 1. forwards: h = cbf(g), pi = actor(g), a = 2 pi + u_ref and x' (act_dyn_kernel), h' = cbf(g')
-    RC(forward(1, cbf_params, cbf_planes, g, 0, h, ws + F.fw_h));
-    RC(forward(nu, actor_params, actor_planes, g, 0, ws + F.pi, ws + F.fw_pi));
-    GCBF_DISPATCH_ENV(d->env_kind, {
-        act_dyn_kernel<KIND><<<blocks, 128, 0, st>>>(*d, agent, goal, ws + F.pi, ws + F.act, ws + F.xn);
-    });
-    count_launch();
-    RC(check_launch("act_dyn_kernel"));
-    RC(forward(1, cbf_params, cbf_planes, gn, 1, ws + F.hn, ws + F.fw_hn));
-    // 2. terms, worst agent per graph, upstream gradients of J wrt h and h'
-    falsify_select_kernel<<<G, FALSIFY_SELECT_THREADS, 0, st>>>(N, env_sd(d->env_kind), alpha, d->dt, h, ws + F.hn,
-                                                                ws + F.xn, term, worst, ws + F.dh, ws + F.dhn);
-    count_launch();
-    RC(check_launch("falsify_select_kernel"));
-    if (!grad_x) return 0;
-    // 3. data-only backward of cbf(g') -> d_es'
-    RC(gnn_backward_impl({d, gn, ws + F.gw, nullptr, use_tensor_cores, 1, cbf_params, cbf_planes, ws + F.fw_hn,
-                          ws + F.hn, ws + F.dhn, nullptr, nullptr, 1, ws + F.des_n, ws + F.je}, st));
-    // 4. through x' = Euler(x, clip_action(2 pi + u_ref(x))): dpi and the direct / u_ref parts of d J / dx
-    GCBF_DISPATCH_ENV(d->env_kind, {
-        falsify_dyn_kernel<KIND><<<blocks, 128, 0, st>>>(*d, agent, goal, ws + F.act, ws + F.xn, ws + F.des_n,
-                                                         ws + F.dpi, ws + F.gx);
-    });
-    count_launch();
-    RC(check_launch("falsify_dyn_kernel"));
-    // 5. data-only backwards on g: the actor with upstream dpi, the CBF with upstream dh
-    RC(gnn_backward_impl({d, g, ws + F.gw, nullptr, use_tensor_cores, nu, actor_params, actor_planes, ws + F.fw_pi,
-                          ws + F.pi, ws + F.dpi, nullptr, nullptr, 0, ws + F.des_a, ws + F.je}, st));
-    RC(gnn_backward_impl({d, g, ws + F.gw, nullptr, use_tensor_cores, 1, cbf_params, cbf_planes, ws + F.fw_h, h,
-                          ws + F.dh, nullptr, nullptr, 0, ws + F.des_c, ws + F.je}, st));
-    // 6. edge-state gradients -> states, plus the Euler / u_ref part
-    GCBF_DISPATCH_ENV(d->env_kind, {
-        falsify_grad_kernel<KIND><<<blocks, 128, 0, st>>>(*d, agent, ws + F.des_a, ws + F.des_c, ws + F.gx, grad_x);
-    });
-    count_launch();
-    RC(check_launch("falsify_grad_kernel"));
-#undef RC
-    return 0;
 }

@@ -1,37 +1,17 @@
 // translayout.cuh -- the GEMM weights of a network in the layouts the GEMMs read: transposed fp32 copies (TransLayout,
-// the backward-data operands of the SIMT path) and tf32 hi / lo planes (PlaneLayout, the tensor-core path).
+// the backward-data operands of the SIMT path) and tf32 hi / lo planes (PlaneLayout, the tensor-core path).  They are
+// built by build_transposes (dense.cu) and build_planes (gnn.cu).
 #pragma once
 #include "common.cuh"
 
 namespace gcbf {
-
-static __global__ void transpose_kernel(const float* __restrict__ in, float* __restrict__ out, int rows, int cols) {
-    __shared__ float tile[32][33];
-    const int c0 = blockIdx.x * 32, r0 = blockIdx.y * 32;
-    for (int i = threadIdx.y; i < 32; i += blockDim.y) {
-        const int r = r0 + i, c = c0 + threadIdx.x;
-        if (r < rows && c < cols) tile[i][threadIdx.x] = in[(size_t)r * cols + c];
-    }
-    __syncthreads();
-    for (int i = threadIdx.y; i < 32; i += blockDim.y) {
-        const int c = c0 + i, r = r0 + threadIdx.x;
-        if (r < rows && c < cols) out[(size_t)c * rows + r] = tile[threadIdx.x][i];
-    }
-}
-
-static int32_t launch_transpose(const float* in, float* out, int rows, int cols, cudaStream_t st) {
-    dim3 grid((cols + 31) / 32, (rows + 31) / 32), block(32, 8);
-    transpose_kernel<<<grid, block, 0, st>>>(in, out, rows, cols);
-    count_launch();
-    return check_launch("transpose_kernel");
-}
 
 // Transposed copies of the GEMM weights of one network (backward-data operands).
 struct TransLayout {
     int w[12];
     int total;
 };
-static TransLayout make_trans_layout(const ParamLayout& L) {
+inline TransLayout make_trans_layout(const ParamLayout& L) {
     TransLayout T;
     int off = 0;
     for (int i = 0; i < 12; ++i) {
@@ -43,15 +23,6 @@ static TransLayout make_trans_layout(const ParamLayout& L) {
     }
     T.total = off;
     return T;
-}
-static int32_t build_transposes(const ParamLayout& L, const TransLayout& T, const float* P, float* PT, cudaStream_t st) {
-    for (int i = 0; i < 12; ++i) {
-        if (T.w[i] < 0) continue;
-        const float* src = P + L.w[i] + (i == L_UPD0 ? 3 * 256 : 0);
-        const int rows = (i == L_UPD0) ? 128 : L.in[i];
-        if (int32_t rc = launch_transpose(src, PT + T.w[i], rows, L.out[i], st)) return rc;
-    }
-    return 0;
 }
 
 // tf32 hi / lo planes of the GEMM weights of an n_layers-deep network (gcbf_prepare_params_l): the one prepared-weights
