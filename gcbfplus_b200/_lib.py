@@ -153,6 +153,17 @@ def ptr(t) -> int:
     return t.data_ptr()
 
 
+#: Bit 30 of an iteration word (`iters` of the device QPs and of the refinement): the bits below it count iterations.
+#: What the bit flags depends on the entry point (include/gcbf_b200.h): the dense-graph path for gcbf_qp_labels and
+#: gcbf_qp_filter, a solve that hit its cap for gcbf_cbfqp_* and gcbf_refine_actions.
+ITER_FLAG = 1 << 30
+
+
+def split_iters(iters):
+    """(iteration counts, flag bits set) of a tensor or array of iteration words."""
+    return iters & (ITER_FLAG - 1), (iters & ITER_FLAG) != 0
+
+
 def f32(v: float) -> float:
     """Round a python double to fp32 (where JAX's weak typing rounds a python scalar)."""
     return float(np.float32(v))

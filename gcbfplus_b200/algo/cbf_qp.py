@@ -22,15 +22,16 @@ K_NEAREST = 3
 #: default iteration cap and stopping threshold (projected dual-gradient residual) of the device QP solves
 QP_MAX_ITER = 10000
 QP_TOL = 1e-8
-CAPPED_BIT = 1 << 30
 
 
-def iter_stats(iters: torch.Tensor) -> dict:
-    """Median / max iterations and the number of capped solves of an iteration record (gcbf_cbfqp_* `iters`)."""
-    v = iters.reshape(-1).to(torch.int64).cpu().numpy()
-    n = v & (CAPPED_BIT - 1)
-    return {"solves": int(v.size), "iters_median": float(np.median(n)) if v.size else 0.0,
-            "iters_max": int(n.max()) if v.size else 0, "capped": int(((v & CAPPED_BIT) != 0).sum())}
+def iter_stats(iters: torch.Tensor, cap: Optional[int] = None) -> dict:
+    """Median / max iterations and the number of capped solves of an iteration record (`iters` of gcbf_cbfqp_* or
+    gcbf_refine_actions, whose bit 30 marks a capped solve).  For gcbf_qp_labels / gcbf_qp_filter, whose bit 30 marks
+    the dense-graph path instead, pass their iteration cap: a solve then counts as capped when it ran `cap` iterations."""
+    n, flag = _lib.split_iters(iters.reshape(-1).to(torch.int64).cpu().numpy())
+    capped = flag if cap is None else n >= cap
+    return {"solves": int(n.size), "iters_median": float(np.median(n)) if n.size else 0.0,
+            "iters_max": int(n.max()) if n.size else 0, "capped": int(capped.sum())}
 
 
 class _PairwiseCBFQP(MultiAgentController):
@@ -43,7 +44,7 @@ class _PairwiseCBFQP(MultiAgentController):
         self.k = K_NEAREST
         self.max_iter = int(max_iter)
         self.tol = float(tol)
-        #: iteration record of the last get_qp_action (one entry per solve, bit 30 = capped)
+        #: iteration record of the last get_qp_action (one entry per solve, bit 30 = capped: _lib.split_iters)
         self.last_iters: Optional[torch.Tensor] = None
 
     @property

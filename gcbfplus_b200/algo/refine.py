@@ -14,7 +14,6 @@ from .params import NetParams
 
 REFINE_LR = 0.1
 REFINE_MAX_ITER = 30
-CAPPED_BIT = 1 << 30
 
 
 def require_one_layer_refine(params: NetParams, what: str) -> None:

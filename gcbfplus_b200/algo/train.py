@@ -393,9 +393,9 @@ def qp_labels(algo, graph: SwarmGraph, params=None, with_aux: bool = False, max_
         u_nom = u_nom.to(device=env.device, dtype=torch.float32).contiguous()
         _lib.check(lib.gcbf_qp_filter(*head, _lib.ptr(u_nom), *tail), "gcbf_qp_filter")
     if with_aux:
-        return u_qp, aux, iters & 0x3FFFFFFF      # bit 30 flags the global-memory fallback of dense graphs
+        return u_qp, aux, _lib.split_iters(iters)[0]      # bit 30 flags the dense-graph path, not a cap
     if with_iters:
-        return u_qp, iters & 0x3FFFFFFF
+        return u_qp, _lib.split_iters(iters)[0]
     return u_qp
 
 

@@ -16,11 +16,9 @@
 // constant distance and dp = dv = 0, so its gradient is exactly 0.  Lie terms along env.control_affine_dyn
 // (qp_lie.cuh): Lf_h = dh/dx_i f(x_i) + dh/dx_j f(x_j), Lg_self = dh/dx_i g(x_i), Lg_other = dh/dx_j g(x_j).
 //
-// Both controllers solve   min 1/2 |u|^2 - u_ref.u + 5 |r|^2 + 1000 sum r   s.t.  -Lg u - r <= b,  |u| <= u_lim,
-// r >= 0 (H = diag(1.., 10..), H > 0: the minimiser is unique).  The reference hands it to JaxProxQP with
-// max_iter = 100; here it is solved exactly on the dual, as qp.cu does for the GCBF+ labels: with multipliers
-// lam >= 0 the inner minimisers are closed-form, u(lam) = clip(u_ref + Lg^T lam), r(lam) = max(0, (lam - 1000) / 10),
-// and an accelerated projected-gradient ascent with gradient restart runs on the row-scaled dual in fp64.
+// Both controllers solve the QP of dual_qp.cuh, which the reference hands to JaxProxQP with max_iter = 100, exactly
+// on its dual with the momentum scalar in fp64.  A NaN u_ref component (u_ref is NaN exactly at the goal) takes part
+// as 0 and comes out NaN, as it passes through the reference's solve.
 //   DecShareCBF: one 3-row problem per agent (own Lg block only), b = resp (Lf_h + alpha h), resp = 1 for an
 //     obstacle pick, 0.5 for an agent pick.  Thread per agent.
 //   CentralizedCBF: one 3N-row problem per graph, row (i, k) touching u_i and, for an agent pick, u_j;
@@ -28,6 +26,7 @@
 #include <math.h>
 
 #include "common.cuh"
+#include "dual_qp.cuh"
 #include "geometry_dev.cuh"
 #include "qp_lie.cuh"
 
@@ -35,8 +34,6 @@ namespace gcbf {
 
 constexpr int CBF_K = 3;
 constexpr float CBF_SELF_DIST = 1e2f;      // utils.py: o_dist_sq.at[agent_idx].set(1e2)
-constexpr double CBF_RELAX_PENALTY = 1e3;  // dec_share_cbf.py:103 relax_penalty
-constexpr double CBF_RELAX_WEIGHT = 10.0;  // H[-k:, -k:] = 10
 constexpr int CBF_WARPS = 8;               // agents (warps) per CTA of the pairwise kernel
 constexpr int CBF_CENTRAL_THREADS = 512;
 
@@ -193,6 +190,7 @@ cbf_pairwise_kernel(const gcbf_env_desc d, const float* __restrict__ agent, cons
 // ------------------------------------------------------------------------------------------------------------------
 // DecShareCBF: one 3-multiplier dual per agent, thread per agent
 // ------------------------------------------------------------------------------------------------------------------
+// The steps of dual_cta_solve on a thread-local problem held in registers (no block reduction).
 // iters[a] = iterations | (1 << 30) when the cap was hit before the stopping test passed
 template <int KIND>
 __global__ void __launch_bounds__(128)
@@ -211,7 +209,7 @@ cbf_dec_share_kernel(const gcbf_env_desc d, const float alpha, const int max_ite
         gl[c] = goal[(size_t)a * SD + c];
     }
     u_ref_dev<KIND>(d, x, gl, urf);
-    double L[K][NU], b[K], s[K], ur[NU];
+    double L[K][NU], b[K], s[K], ur[NU], mu[K], y[K];
     const double ul = (double)d.u_lim;
     double fro = 0.0, s2max = 0.0;
 #pragma unroll
@@ -221,29 +219,21 @@ cbf_dec_share_kernel(const gcbf_env_desc d, const float alpha, const int max_ite
         const size_t o = (size_t)a * K + k;
         const float resp = pw.isobs[o] ? 1.0f : 0.5f;
         b[k] = (double)(resp * (pw.lf[o] + alpha * pw.h[o]));
-        double sq = 0.0;
+        double sq = 0.0, rs = 0.0;
 #pragma unroll
         for (int c = 0; c < NU; ++c) {
             L[k][c] = (double)pw.lg_self[o * NU + c];
             sq += L[k][c] * L[k][c];
+            rs += fabs(L[k][c]);
         }
-        s[k] = 1.0 / sqrt(sq + 1.0 / CBF_RELAX_WEIGHT);
+        s[k] = 1.0 / sqrt(sq + 1.0 / QP_RELAX_WEIGHT);
         fro += s[k] * s[k] * sq;
         s2max = fmax(s2max, s[k] * s[k]);
-    }
-    // step 1 / lip with lip = |S Lg|_F^2 + max(s^2) / 10 >= |S Lg|_2^2 + max(s^2) / 10
-    const double lip = fro + s2max / CBF_RELAX_WEIGHT, step = 1.0 / lip;
-    double mu[K], y[K];
-#pragma unroll
-    for (int k = 0; k < K; ++k) {
-        // a row no admissible u satisfies is relaxed at the optimum with r >= its violation: start there
-        double rs = 0.0;
-#pragma unroll
-        for (int c = 0; c < NU; ++c) rs += fabs(L[k][c]);
-        const double vmin = -rs * ul - b[k];
-        mu[k] = vmin > 0.0 ? (CBF_RELAX_PENALTY + CBF_RELAX_WEIGHT * vmin) / s[k] : 0.0;
+        mu[k] = dual_warm_start(-rs * ul - b[k], s[k]);
         y[k] = mu[k];
     }
+    // step 1 / lip with |S Lg|_F^2 >= |S Lg|_2^2
+    const double lip = dual_lipschitz(fro, s2max), step = 1.0 / lip;
     double t = 1.0;
     int it = 0;
     bool conv = false;
@@ -254,7 +244,7 @@ cbf_dec_share_kernel(const gcbf_env_desc d, const float alpha, const int max_ite
             double v = ur[c];
 #pragma unroll
             for (int k = 0; k < K; ++k) v = fma(L[k][c], s[k] * y[k], v);
-            u[c] = isnan(v) ? 0.0 : fmin(fmax(v, -ul), ul);   // NaN u_ref (agent exactly at its goal): see below
+            u[c] = isnan(v) ? 0.0 : fmin(fmax(v, -ul), ul);   // NaN u_ref: as 0 here, NaN in the result
         }
         double res = 0.0, dotp = 0.0, mn[K];
 #pragma unroll
@@ -262,22 +252,15 @@ cbf_dec_share_kernel(const gcbf_env_desc d, const float alpha, const int max_ite
             double lgu = 0.0;
 #pragma unroll
             for (int c = 0; c < NU; ++c) lgu = fma(L[k][c], u[c], lgu);
-            const double r = fmax(0.0, (s[k] * y[k] - CBF_RELAX_PENALTY) / CBF_RELAX_WEIGHT);
-            const double grad = s[k] * (-lgu - r - b[k]);
-            mn[k] = fmax(0.0, fma(step, grad, y[k]));
-            res = fmax(res, fabs(mn[k] - y[k]));
-            dotp = fma(grad, mn[k] - mu[k], dotp);
+            mn[k] = dual_row_step(k, s[k] * y[k], s, b, y, mu, lgu, step, res, dotp);
         }
-        const bool restart = dotp < 0.0;
-        const double t_new = restart ? 1.0 : 0.5 * (1.0 + sqrt(1.0 + 4.0 * t * t));
-        const double beta = restart ? 0.0 : (t - 1.0) / t_new;
+        const double beta = dual_momentum(dotp, t);
 #pragma unroll
         for (int k = 0; k < K; ++k) {
-            y[k] = fma(beta, mn[k] - mu[k], mn[k]);
+            y[k] = dual_extrapolate(beta, mn[k], mu[k]);
             mu[k] = mn[k];
         }
-        t = t_new;
-        if (res * lip < tol) { conv = true; break; }
+        if (dual_converged(res, lip, tol)) { conv = true; break; }
     }
 #pragma unroll
     for (int c = 0; c < NU; ++c) {
@@ -289,7 +272,7 @@ cbf_dec_share_kernel(const gcbf_env_desc d, const float alpha, const int max_ite
     if (out_r) {
 #pragma unroll
         for (int k = 0; k < K; ++k)
-            out_r[(size_t)a * K + k] = (float)fmax(0.0, (s[k] * mu[k] - CBF_RELAX_PENALTY) / CBF_RELAX_WEIGHT);
+            out_r[(size_t)a * K + k] = (float)dual_relax(s[k] * mu[k]);
     }
     if (iters) iters[a] = min(it, max_iter) | (conv ? 0 : (1 << 30));
 }
@@ -297,20 +280,49 @@ cbf_dec_share_kernel(const gcbf_env_desc d, const float alpha, const int max_ite
 // ------------------------------------------------------------------------------------------------------------------
 // CentralizedCBF: one 3N-row dual per graph, one CTA per graph
 // ------------------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void cbf_block_max_sum(double& a, double& b, double* red) {
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = (blockDim.x + 31) >> 5;
+// The problem of dual_cta_solve: row (i, k) = self block ls of agent i plus, for an agent pick j, other block lo of
+// agent j.  u is fp64, and a NaN u_ref component takes part as 0 until the returned iterate, which keeps the NaN.
+template <int NU>
+struct CentralRows {
+    const float* ls; const float* lo; const float* ur;   // [M, NU], [M, NU], [N, NU]
+    const int* oth; const int* toff; const int* trow;   // other agent of each row; transposed index
+    double* u;                                          // [N, NU]
+    int N;
+    double ul;
+    // u = clip(u_ref + Lg^T lam): own rows (self block) + the transposed list (other block)
+    __device__ __forceinline__ void primal(const double* lam, const bool last) const {
+        for (int j = threadIdx.x; j < N; j += blockDim.x) {
+            double v[NU];
 #pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-        a = fmax(a, __shfl_xor_sync(0xffffffffu, a, o));
-        b += __shfl_xor_sync(0xffffffffu, b, o);
+            for (int q = 0; q < NU; ++q) v[q] = (double)ur[j * NU + q];
+            for (int k = 0; k < CBF_K; ++k) {
+                const double l = lam[j * CBF_K + k];
+#pragma unroll
+                for (int q = 0; q < NU; ++q) v[q] = fma((double)ls[(j * CBF_K + k) * NU + q], l, v[q]);
+            }
+            for (int w = toff[j]; w < toff[j + 1]; ++w) {
+                const int r = trow[w];
+                const double l = lam[r];
+#pragma unroll
+                for (int q = 0; q < NU; ++q) v[q] = fma((double)lo[r * NU + q], l, v[q]);
+            }
+#pragma unroll
+            for (int q = 0; q < NU; ++q)
+                u[j * NU + q] = isnan(v[q]) ? (last ? NAN : 0.0) : fmin(fmax(v[q], -ul), ul);
+        }
     }
-    __syncthreads();
-    if (lane == 0) { red[warp] = a; red[32 + warp] = b; }
-    __syncthreads();
-    a = red[0];
-    b = red[32];
-    for (int w = 1; w < nw; ++w) { a = fmax(a, red[w]); b += red[32 + w]; }
-}
+    __device__ __forceinline__ double row_dot(const int r) const {
+        const int i = r / CBF_K, j = oth[r];
+        double lgu = 0.0;
+#pragma unroll
+        for (int q = 0; q < NU; ++q) lgu = fma((double)ls[r * NU + q], u[i * NU + q], lgu);
+        if (j >= 0) {
+#pragma unroll
+            for (int q = 0; q < NU; ++q) lgu = fma((double)lo[r * NU + q], u[j * NU + q], lgu);
+        }
+        return lgu;
+    }
+};
 
 // Shared memory, M = 3N rows: mu, y, lam [M] fp64 | u [N, NU] fp64 | red [64] fp64 | s, b [M] | lg_self, lg_other
 // [M, NU] | u_ref [N, NU] | other [M] int (agent j of the row or -1) | toff [N + 1] int | trow [M] int (transposed
@@ -364,9 +376,7 @@ cbf_central_kernel(const gcbf_env_desc d, const float alpha, const int max_iter,
             lo[r * NU + q] = pw.lg_other[o * NU + q];
             sq += ls[r * NU + q] * ls[r * NU + q] + lo[r * NU + q] * lo[r * NU + q];
         }
-        sc[r] = rsqrtf(sq + (float)(1.0 / CBF_RELAX_WEIGHT));
-        mu[r] = 0.0;
-        y[r] = 0.0;
+        sc[r] = rsqrtf(sq + (float)(1.0 / QP_RELAX_WEIGHT));
         if (j >= 0) atomicAdd(&toff[j + 1], 1);
     }
     for (int j = tid; j < N; j += nt) {
@@ -394,19 +404,16 @@ cbf_central_kernel(const gcbf_env_desc d, const float alpha, const int max_iter,
     __syncthreads();
 
     // ---- step bound L = |S Lg|_1 |S Lg|_inf + max(s^2) / 10 and the relaxed-row warm start
-    double rowmax = 0.0, colmax = 0.0, s2max = 0.0, dummy = 0.0;
+    double rowmax = 0.0, colmax = 0.0, s2max = 0.0;
     for (int r = tid; r < M; r += nt) {
         double rs = 0.0;
 #pragma unroll
         for (int q = 0; q < NU; ++q) rs += fabs((double)ls[r * NU + q]) + fabs((double)lo[r * NU + q]);
         rowmax = fmax(rowmax, (double)sc[r] * rs);
         s2max = fmax(s2max, (double)sc[r] * (double)sc[r]);
-        const double vmin = -rs * ul - (double)bb[r];
-        if (vmin > 0.0) {
-            const double m0 = (CBF_RELAX_PENALTY + CBF_RELAX_WEIGHT * vmin) / (double)sc[r];
-            mu[r] = m0;
-            y[r] = m0;
-        }
+        const double m0 = dual_warm_start(-rs * ul - (double)bb[r], (double)sc[r]);
+        mu[r] = m0;
+        y[r] = m0;
     }
     for (int j = tid; j < N; j += nt) {
 #pragma unroll
@@ -417,91 +424,24 @@ cbf_central_kernel(const gcbf_env_desc d, const float alpha, const int max_iter,
             colmax = fmax(colmax, cs);
         }
     }
-    cbf_block_max_sum(rowmax, dummy, red);
-    dummy = 0.0;
-    cbf_block_max_sum(colmax, dummy, red);
-    dummy = 0.0;
-    cbf_block_max_sum(s2max, dummy, red);
-    const double lip = rowmax * colmax + s2max / CBF_RELAX_WEIGHT, step = 1.0 / lip;
+    rowmax = block_max(rowmax, red);
+    colmax = block_max(colmax, red);
+    s2max = block_max(s2max, red);
+    const double lip = dual_lipschitz(rowmax * colmax, s2max);
     __syncthreads();
 
-    // u = clip(u_ref + Lg^T lam): own rows (self block) + the transposed list (other block)
-    // a NaN u_ref component (u_ref is NaN exactly at the goal) takes part as 0 and comes out NaN, as it passes
-    // through the reference's solve
-    auto primal = [&](const bool last) {
-        for (int j = tid; j < N; j += nt) {
-            double v[NU];
-#pragma unroll
-            for (int q = 0; q < NU; ++q) v[q] = (double)ur[j * NU + q];
-            for (int k = 0; k < K; ++k) {
-                const double l = lam[j * K + k];
-#pragma unroll
-                for (int q = 0; q < NU; ++q) v[q] = fma((double)ls[(j * K + k) * NU + q], l, v[q]);
-            }
-            for (int w = toff[j]; w < toff[j + 1]; ++w) {
-                const int r = trow[w];
-                const double l = lam[r];
-#pragma unroll
-                for (int q = 0; q < NU; ++q) v[q] = fma((double)lo[r * NU + q], l, v[q]);
-            }
-#pragma unroll
-            for (int q = 0; q < NU; ++q)
-                u[j * NU + q] = isnan(v[q]) ? (last ? NAN : 0.0) : fmin(fmax(v[q], -ul), ul);
-        }
-    };
-    for (int r = tid; r < M; r += nt) lam[r] = (double)sc[r] * y[r];
-    __syncthreads();
-    double t = 1.0;
-    int it;
-    bool conv = false;
-    for (it = 1; it <= max_iter; ++it) {
-        primal(false);
-        __syncthreads();
-        double res = 0.0, dotp = 0.0;
-        for (int r = tid; r < M; r += nt) {
-            const int i = r / K, j = oth[r];
-            double lgu = 0.0;
-#pragma unroll
-            for (int q = 0; q < NU; ++q) lgu = fma((double)ls[r * NU + q], u[i * NU + q], lgu);
-            if (j >= 0) {
-#pragma unroll
-                for (int q = 0; q < NU; ++q) lgu = fma((double)lo[r * NU + q], u[j * NU + q], lgu);
-            }
-            const double rr = fmax(0.0, (lam[r] - CBF_RELAX_PENALTY) / CBF_RELAX_WEIGHT);
-            const double grad = (double)sc[r] * (-lgu - rr - (double)bb[r]);
-            const double mn = fmax(0.0, fma(step, grad, y[r]));
-            res = fmax(res, fabs(mn - y[r]));
-            dotp = fma(grad, mn - mu[r], dotp);
-            lam[r] = mn;   // carries mu_new until the momentum update (u is already formed)
-        }
-        cbf_block_max_sum(res, dotp, red);
-        const bool restart = dotp < 0.0;
-        const double t_new = restart ? 1.0 : 0.5 * (1.0 + sqrt(1.0 + 4.0 * t * t));
-        const double beta = restart ? 0.0 : (t - 1.0) / t_new;
-        for (int r = tid; r < M; r += nt) {
-            const double mn = lam[r];
-            const double yn = fma(beta, mn - mu[r], mn);
-            y[r] = yn;
-            mu[r] = mn;
-            lam[r] = (double)sc[r] * yn;
-        }
-        t = t_new;
-        __syncthreads();
-        if (res * lip < tol) { conv = true; break; }
-    }
-    for (int r = tid; r < M; r += nt) lam[r] = (double)sc[r] * mu[r];
-    __syncthreads();
-    primal(true);
-    __syncthreads();
+    CentralRows<NU> P{ls, lo, ur, oth, toff, trow, u, N, ul};
+    bool conv;
+    const int it = dual_cta_solve<double>(P, M, max_iter, tol, lip, mu, y, lam, sc, bb, red, conv);
     for (int j = tid; j < N; j += nt) {
 #pragma unroll
         for (int q = 0; q < NU; ++q) out_u[(base + j) * NU + q] = (float)u[j * NU + q];
     }
     if (out_r) {
         for (int r = tid; r < M; r += nt)
-            out_r[base * K + r] = (float)fmax(0.0, (lam[r] - CBF_RELAX_PENALTY) / CBF_RELAX_WEIGHT);
+            out_r[base * K + r] = (float)dual_relax(lam[r]);
     }
-    if (iters && tid == 0) iters[g] = min(it, max_iter) | (conv ? 0 : (1 << 30));
+    if (iters && tid == 0) iters[g] = it | (conv ? 0 : (1 << 30));
 }
 
 // ------------------------------------------------------------------------------------------------------------------

@@ -1,18 +1,15 @@
 // qp.cu -- CBF-QP action labels u_qp (gcbfplus/algo/gcbf_plus.py:299-352 get_qp_action, :193-211 get_b_u_qp).
 // Uses u_ref_dev of geometry_dev.cuh and, from the train step (internal.cuh), the data-only mode of gnn_backward_impl.
 //
-// Per graph with N agents, x = [u | r]:
-//     min 1/2 |u|^2 - u_ref.u + 5 |r|^2 + 1000 sum r   s.t.  -Lg_h u - r <= Lf_h + 0.1 alpha h,  |u| <= u_lim,  r >= 0
-// The safety filter (gcbf_qp_filter) solves the same QP with a given nominal action u_nom in place of u_ref.
-// The reference hands the dense [N, N nu] problem to JaxProxQP.  Here:
+// Per graph with N agents, the QP of dual_qp.cuh with b = Lf_h + 0.1 alpha h (one row per agent).  The safety filter
+// (gcbf_qp_filter) solves it with a given nominal action u_nom in place of u_ref.  The reference hands the dense
+// [N, N nu] problem to JaxProxQP; the minimiser is unique, so any exact method returns its label up to tolerance.
 //   * h(x) is a ONE-layer GNN, so row i of dh/dx is non-zero only at i and at i's agent neighbours: the
 //     Jacobian is one data-only backward pass with upstream 1 (every receiver's gradient stays on its own
 //     edges), kept per edge -- Lg_h is stored on the edge list (self block + one nu-block per agent edge);
-//   * H is diagonal, so the dual is a box-projected concave problem in N multipliers whose inner minimisers
-//     are closed-form: u(lam) = clip(u_ref + Lg^T lam), r(lam) = max(0, (lam - 1000) / 10).  One CTA per graph
-//     runs an accelerated projected-gradient ascent with gradient restart on the row-scaled dual, everything
-//     in shared memory; Lg^T lam uses the symmetric radius graph (edge j->i has the mirror edge i->j).
-// The minimiser is unique (H > 0), so any exact method returns the reference's label up to solver tolerance.
+//   * one CTA per graph runs dual_cta_solve, everything in shared memory; Lg^T lam uses the symmetric radius graph
+//     (edge j->i has the mirror edge i->j).
+#include "dual_qp.cuh"
 #include "geometry_dev.cuh"
 #include "gnn.cuh"
 #include "internal.cuh"
@@ -20,8 +17,6 @@
 
 namespace gcbf {
 
-constexpr float QP_RELAX_PENALTY = 1e3f;   // gcbf_plus.py:302
-constexpr float QP_RELAX_WEIGHT = 10.f;    // gcbf_plus.py:331
 constexpr float QP_H_SCALE = 0.1f;         // gcbf_plus.py:334
 constexpr int QP_MAX_AGENTS = 2048;
 
@@ -105,43 +100,20 @@ qp_assemble_kernel(const gcbf_env_desc d, const float alpha, const float* __rest
         sq = fmaf(lg[c], lg[c], sq);
     }
     QB[i] = lf_sum + alpha * QP_H_SCALE * h[i];
-    QSC[i] = rsqrtf(sq + 1.f / QP_RELAX_WEIGHT);
-}
-
-__device__ __forceinline__ float qp_block_max(float v, float* red) {
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = (blockDim.x + 31) >> 5;
-    v = warp_max(v);
-    __syncthreads();
-    if (lane == 0) red[warp] = v;
-    __syncthreads();
-    float r = red[0];
-    for (int w = 1; w < nw; ++w) r = fmaxf(r, red[w]);
-    return r;
-}
-// (max of a, sum of b) over the block in one round trip; the sum runs in a fixed order (deterministic).
-__device__ __forceinline__ void qp_block_max_sum(double& a, double& b, double* red) {
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = (blockDim.x + 31) >> 5;
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-        a = fmax(a, __shfl_xor_sync(0xffffffffu, a, o));
-        b += __shfl_xor_sync(0xffffffffu, b, o);
-    }
-    __syncthreads();
-    if (lane == 0) { red[warp] = a; red[32 + warp] = b; }
-    __syncthreads();
-    a = red[0];
-    b = red[32];
-    for (int w = 1; w < nw; ++w) { a = fmax(a, red[w]); b += red[32 + w]; }
+    QSC[i] = rsqrtf(sq + (float)(1.0 / QP_RELAX_WEIGHT));
 }
 
 // Neighbour access of the dual iteration.  SM: the graph's agent-agent blocks compacted into shared memory
 // (CSR: off / nj / lg / lgt); otherwise straight from the edge list in global memory (graphs too dense to fit).
+// The problem of dual_cta_solve: u is fp32, and a NaN u_ref component clips to -u_lim (fmax drops the NaN).
 template <int NU, bool SM>
 struct QpRows {
     const int* off; const int* nj; const float* lg; const float* lgt;           // shared CSR
     const int32_t* row_start; const int32_t* row_deg; const int32_t* edge_src;  // global edge list
     const float* QE; const int32_t* REV;
+    const float* ls; const float* ur; float* u;                                 // Lg_self, u_ref, u [N, NU] (shared)
     int base, N, edge_cap;
+    float u_lim;
     __device__ __forceinline__ void range(int i, int& beg, int& end) const {
         if (SM) { beg = off[i]; end = off[i + 1]; return; }
         beg = row_start[base + i];
@@ -160,94 +132,49 @@ struct QpRows {
         col_blk = QE + (size_t)rv * 4;
         return code - base;
     }
-};
-
-template <int NU, bool SM>
-__device__ __forceinline__ void qp_primal_u(const QpRows<NU, SM>& R, const int N, const float u_lim, const double* lam,
-                                            const float* ls, const float* ur, float* u) {
     // u = clip(u_ref + Lg^T lam): column block j collects Lg[i, j] lam_i over j's neighbours i (mirror edges)
-    for (int j = threadIdx.x; j < N; j += blockDim.x) {
-        int beg, end;
-        R.range(j, beg, end);
-        const double lj = lam[j];
-        double v[NU];
-#pragma unroll
-        for (int c = 0; c < NU; ++c) v[c] = fma((double)ls[j * NU + c], lj, (double)ur[j * NU + c]);
-        for (int k = beg; k < end; ++k) {
-            const float *rb, *cb;
-            const int i = R.nbr(k, rb, cb);
-            if (i < 0) continue;
-            const double li = lam[i];
-#pragma unroll
-            for (int c = 0; c < NU; ++c) v[c] = fma((double)cb[c], li, v[c]);
-        }
-#pragma unroll
-        for (int c = 0; c < NU; ++c) u[j * NU + c] = (float)fmin(fmax(v[c], -(double)u_lim), (double)u_lim);
-    }
-}
-
-template <int NU, bool SM>
-__device__ __forceinline__ int qp_iterate(const QpRows<NU, SM>& R, const int N, const float u_lim, const int max_iter,
-                                          const double tol, const double lip, double* mu, double* y, double* lam,
-                                          const float* sc, const float* bb, const float* ls, const float* ur, float* u,
-                                          double* red) {
-    const int tid = threadIdx.x, nt = blockDim.x;
-    const double step = 1.0 / lip;
-    float t = 1.f;                                  // momentum schedule: fp32 is ample (only beta depends on it)
-    int it;
-    for (int i = tid; i < N; i += nt) lam[i] = (double)sc[i] * y[i];
-    __syncthreads();
-    for (it = 1; it <= max_iter; ++it) {            // 4 block barriers per iteration
-        qp_primal_u<NU, SM>(R, N, u_lim, lam, ls, ur, u);
-        __syncthreads();
-        // dual gradient s (-Lg u - r - b), projected step, restart test
-        double res = 0.0, dotp = 0.0;
-        for (int i = tid; i < N; i += nt) {
+    __device__ __forceinline__ void primal(const double* lam, bool) const {
+        for (int j = threadIdx.x; j < N; j += blockDim.x) {
             int beg, end;
-            R.range(i, beg, end);
-            double lgu = 0.0;
+            range(j, beg, end);
+            const double lj = lam[j];
+            double v[NU];
 #pragma unroll
-            for (int c = 0; c < NU; ++c) lgu = fma((double)ls[i * NU + c], (double)u[i * NU + c], lgu);
+            for (int c = 0; c < NU; ++c) v[c] = fma((double)ls[j * NU + c], lj, (double)ur[j * NU + c]);
             for (int k = beg; k < end; ++k) {
                 const float *rb, *cb;
-                const int j = R.nbr(k, rb, cb);
-                if (j < 0) continue;
+                const int i = nbr(k, rb, cb);
+                if (i < 0) continue;
+                const double li = lam[i];
 #pragma unroll
-                for (int c = 0; c < NU; ++c) lgu = fma((double)rb[c], (double)u[j * NU + c], lgu);
+                for (int c = 0; c < NU; ++c) v[c] = fma((double)cb[c], li, v[c]);
             }
-            const double r = fmax(0.0, (lam[i] - (double)QP_RELAX_PENALTY) / (double)QP_RELAX_WEIGHT);
-            const double grad = (double)sc[i] * (-lgu - r - (double)bb[i]);
-            const double mn = fmax(0.0, fma(step, grad, y[i]));
-            res = fmax(res, fabs(mn - y[i]));
-            dotp = fma(grad, mn - mu[i], dotp);
-            lam[i] = mn;   // lam carries mu_new until the momentum update below (u is already formed)
+#pragma unroll
+            for (int c = 0; c < NU; ++c) u[j * NU + c] = (float)fmin(fmax(v[c], -(double)u_lim), (double)u_lim);
         }
-        qp_block_max_sum(res, dotp, red);
-        const bool restart = dotp < 0.0;
-        const float t_new = restart ? 1.f : 0.5f * (1.f + sqrtf(1.f + 4.f * t * t));
-        const double beta = restart ? 0.0 : (double)((t - 1.f) / t_new);
-        for (int i = tid; i < N; i += nt) {
-            const double mn = lam[i];
-            const double yn = fma(beta, mn - mu[i], mn);
-            y[i] = yn;
-            mu[i] = mn;
-            lam[i] = (double)sc[i] * yn;            // multipliers of the next iterate (read by every thread after the barrier)
-        }
-        t = t_new;
-        __syncthreads();
-        if (res * lip < tol) break;
     }
-    for (int i = tid; i < N; i += nt) lam[i] = (double)sc[i] * mu[i];
-    __syncthreads();
-    qp_primal_u<NU, SM>(R, N, u_lim, lam, ls, ur, u);
-    __syncthreads();
-    return min(it, max_iter);
-}
+    // (Lg u)_i: self block + row i's agent-agent blocks
+    __device__ __forceinline__ double row_dot(int i) const {
+        int beg, end;
+        range(i, beg, end);
+        double lgu = 0.0;
+#pragma unroll
+        for (int c = 0; c < NU; ++c) lgu = fma((double)ls[i * NU + c], (double)u[i * NU + c], lgu);
+        for (int k = beg; k < end; ++k) {
+            const float *rb, *cb;
+            const int j = nbr(k, rb, cb);
+            if (j < 0) continue;
+#pragma unroll
+            for (int c = 0; c < NU; ++c) lgu = fma((double)rb[c], (double)u[j * NU + c], lgu);
+        }
+        return lgu;
+    }
+};
 
-// One CTA per graph.  Dual variables mu = lam / s (row-scaled), FISTA with gradient restart, step 1 / L with the
-// guaranteed bound L = |S Lg|_1 |S Lg|_inf + max(s^2) / 10 >= |S Lg|_2^2 + max(s^2) / 10.
+// One CTA per graph runs dual_cta_solve (dual_qp.cuh) with the momentum scalar in fp32 (only beta depends on it) and
+// the guaranteed bound L = |S Lg|_1 |S Lg|_inf + max(s^2) / 10 >= |S Lg|_2^2 + max(s^2) / 10.
 // The multipliers are iterated in fp64: a relaxed row sits at lam ~ 1e3 while its fixed point is decided at the
-// 1e-6 level (fp32 stalls ~600 ulp short: measured primal residual 3.7e-3); the matrix entries stay fp32.
+// 1e-6 level (fp32 stalls ~600 ulp short: measured primal residual 3.7e-3); the matrix entries and u stay fp32.
 // Shared memory: per agent mu, y, lam (fp64), s, b, u[NU], u_ref[NU], Lg_self[NU]; then the compacted agent-agent
 // blocks of the graph (nbr_cap entries; graphs with more fall back to the global edge list).
 // out_u [A, NU] clipped label; optional out_aux [A, 2] = (lam, r); optional out_iters [G].
@@ -276,26 +203,23 @@ qp_solve_kernel(const int N, const int edge_cap, const int nbr_cap, const float 
     const int g = blockIdx.x;
     const int base = g * N;
     const int tid = threadIdx.x, nt = blockDim.x;
+    const QpRows<NU, false> E{off, nj, lg, lgt, row_start, row_deg, edge_src, QE, REV, ls, ur, u, base, N, edge_cap, u_lim};
 
     // ---- load rows, count agent-agent blocks
     for (int i = tid; i < N; i += nt) {
         const int a = base + i;
         sc[i] = QSC[a];
         bb[i] = QB[a];
-        mu[i] = 0.0;
-        y[i] = 0.0;
 #pragma unroll
         for (int c = 0; c < NU; ++c) {
             ur[i * NU + c] = UR[(size_t)a * 4 + c];
             ls[i * NU + c] = QS[(size_t)a * 4 + c];
         }
-        const int rs = row_start[a];
-        int rd = row_deg[a];
-        if (rs < 0 || rs + rd > edge_cap) rd = 0;
-        int cnt = 0;
-        for (int e = rs; e < rs + rd; ++e) {
-            const int code = edge_src[e];
-            cnt += (code >= base && code < base + N && REV[e] >= 0) ? 1 : 0;
+        int beg, end, cnt = 0;
+        E.range(i, beg, end);
+        for (int e = beg; e < end; ++e) {
+            const float *rb, *cb;
+            cnt += E.nbr(e, rb, cb) >= 0 ? 1 : 0;
         }
         off[i + 1] = cnt;
     }
@@ -311,10 +235,8 @@ qp_solve_kernel(const int N, const int edge_cap, const int nbr_cap, const float 
     // ---- norms for the step size (+ fill of the shared CSR)
     float rowmax = 0.f, colmax = 0.f, s2max = 0.f;
     for (int i = tid; i < N; i += nt) {
-        const int a = base + i;
-        const int rs = row_start[a];
-        int rd = row_deg[a];
-        if (rs < 0 || rs + rd > edge_cap) rd = 0;
+        int beg, end;
+        E.range(i, beg, end);
         const float s = sc[i];
         float rsum = 0.f, csum[NU];
 #pragma unroll
@@ -323,19 +245,17 @@ qp_solve_kernel(const int N, const int edge_cap, const int nbr_cap, const float 
             csum[c] = s * fabsf(ls[i * NU + c]);
         }
         int k = in_smem ? off[i] : 0;
-        for (int e = rs; e < rs + rd; ++e) {
-            const int code = edge_src[e];
-            if (code < base || code >= base + N) continue;
-            const int rv = REV[e];
-            if (rv < 0) continue;
-            const float sj = sc[code - base];
-            if (in_smem) nj[k] = code - base;
+        for (int e = beg; e < end; ++e) {
+            const float *vr, *vc;
+            const int j = E.nbr(e, vr, vc);
+            if (j < 0) continue;
+            const float sj = sc[j];
+            if (in_smem) nj[k] = j;
 #pragma unroll
             for (int c = 0; c < NU; ++c) {
-                const float vr = QE[(size_t)e * 4 + c], vc = QE[(size_t)rv * 4 + c];
-                rsum += fabsf(vr);
-                csum[c] += sj * fabsf(vc);
-                if (in_smem) { lg[(size_t)k * NU + c] = vr; lgt[(size_t)k * NU + c] = vc; }
+                rsum += fabsf(vr[c]);
+                csum[c] += sj * fabsf(vc[c]);
+                if (in_smem) { lg[(size_t)k * NU + c] = vr[c]; lgt[(size_t)k * NU + c] = vc[c]; }
             }
             ++k;
         }
@@ -343,30 +263,26 @@ qp_solve_kernel(const int N, const int edge_cap, const int nbr_cap, const float 
 #pragma unroll
         for (int c = 0; c < NU; ++c) colmax = fmaxf(colmax, csum[c]);
         s2max = fmaxf(s2max, s * s);
-        // A row that no admissible u can satisfy (violation >= vmin > 0 over the whole box) is relaxed at the
-        // optimum with r_i >= vmin, i.e. lam_i >= 1000 + 10 vmin: start there instead of climbing from 0
-        // (the climb costs ~sqrt(1000 / (step * violation)) accelerated steps).
+        // warm start of a row no admissible u satisfies (violation >= vmin over the whole box)
         const float vmin = -rsum * u_lim - bb[i];
-        if (vmin > 0.f) {
-            const double m0 = ((double)QP_RELAX_PENALTY + (double)QP_RELAX_WEIGHT * (double)vmin) / (double)s;
-            mu[i] = m0;
-            y[i] = m0;
-        }
+        const double m0 = dual_warm_start((double)vmin, (double)s);
+        mu[i] = m0;
+        y[i] = m0;
     }
     float* redf = reinterpret_cast<float*>(red);
-    rowmax = qp_block_max(rowmax, redf);
-    colmax = qp_block_max(colmax, redf);
-    s2max = qp_block_max(s2max, redf);
-    const double lip = (double)rowmax * (double)colmax + (double)s2max / (double)QP_RELAX_WEIGHT;
+    rowmax = block_max(rowmax, redf);
+    colmax = block_max(colmax, redf);
+    s2max = block_max(s2max, redf);
+    const double lip = dual_lipschitz((double)rowmax * (double)colmax, (double)s2max);
     __syncthreads();
 
     int it;
+    bool conv;
     if (in_smem) {
-        QpRows<NU, true> R{off, nj, lg, lgt, row_start, row_deg, edge_src, QE, REV, base, N, edge_cap};
-        it = qp_iterate<NU, true>(R, N, u_lim, max_iter, (double)tol, lip, mu, y, lam, sc, bb, ls, ur, u, red);
+        const QpRows<NU, true> S{off, nj, lg, lgt, row_start, row_deg, edge_src, QE, REV, ls, ur, u, base, N, edge_cap, u_lim};
+        it = dual_cta_solve<float>(S, N, max_iter, (double)tol, lip, mu, y, lam, sc, bb, red, conv);
     } else {
-        QpRows<NU, false> R{off, nj, lg, lgt, row_start, row_deg, edge_src, QE, REV, base, N, edge_cap};
-        it = qp_iterate<NU, false>(R, N, u_lim, max_iter, (double)tol, lip, mu, y, lam, sc, bb, ls, ur, u, red);
+        it = dual_cta_solve<float>(E, N, max_iter, (double)tol, lip, mu, y, lam, sc, bb, red, conv);
     }
     for (int j = tid; j < N; j += nt) {
         const int a = base + j;
@@ -375,10 +291,10 @@ qp_solve_kernel(const int N, const int edge_cap, const int nbr_cap, const float 
         if (out_aux) {
             const double lj = lam[j];
             out_aux[(size_t)a * 2 + 0] = (float)lj;
-            out_aux[(size_t)a * 2 + 1] = (float)fmax(0.0, (lj - (double)QP_RELAX_PENALTY) / (double)QP_RELAX_WEIGHT);
+            out_aux[(size_t)a * 2 + 1] = (float)dual_relax(lj);
         }
     }
-    if (out_iters && tid == 0) out_iters[g] = it | (in_smem ? 0 : (1 << 30));
+    if (out_iters && tid == 0) out_iters[g] = it | (in_smem ? 0 : (1 << 30));   // bit 30: dense-graph fallback, not a cap
 }
 
 // shared-memory bytes of qp_solve_kernel for N agents and nbr_cap compacted blocks

@@ -34,7 +34,7 @@ import torch
 from .. import _lib
 from ..algo.cbf_qp import BASELINES, iter_stats
 from ..algo.params import NetParams
-from ..algo.refine import (CAPPED_BIT, REFINE_LR, REFINE_MAX_ITER, launch_refine, planes_buffer, prepare_planes,
+from ..algo.refine import (REFINE_LR, REFINE_MAX_ITER, launch_refine, planes_buffer, prepare_planes,
                            refine_workspace, require_one_layer_refine)
 from ..algo.train import QP_MAX_ITER, QP_TOL, require_one_layer
 from ..utils.graph import SwarmGraph
@@ -564,8 +564,7 @@ class RolloutEngine:
         condition was relaxed (r > 0, `relaxed_frac`); a solve counts as capped when it ran QP_MAX_ITER iterations."""
         ch = self.chains[0]
         if self.policy in QP_FILTER_POLICIES:
-            n = ch.qp_iters & (CAPPED_BIT - 1)          # bit 30 of the QP's count marks the dense-graph path, not a cap
-            st = iter_stats(torch.where(n >= QP_MAX_ITER, n | CAPPED_BIT, n))
+            st = iter_stats(ch.qp_iters, cap=QP_MAX_ITER)   # bit 30 marks the dense-graph path, not a cap
             st["mean_correction"] = float(torch.linalg.vector_norm(self.actions - ch.qp_nominal, dim=-1).mean())
             st["relaxed_frac"] = float((ch.qp_aux[..., 1] > 0).float().mean())
             return st

@@ -141,6 +141,23 @@ def _as_result(res):
                          res.dones.transpose(0, 1), {})
 
 
+def test_nan_u_ref_at_goal():
+    """An agent exactly at its goal has a NaN u_ref (its normalised goal error is 0 / 0).  Both baselines carry it
+    through the solve as 0 and return NaN exactly in that agent's NaN u_ref components, as the reference's solve does;
+    every other agent's action stays finite."""
+    env_id, N, G, area, n_obs = "DoubleIntegrator", 8, 2, 1.5, 4
+    env = product_env(env_id, N, area, n_obs)
+    agent, goal, obs = random_scene(env_id, N, G, area, n_obs, seed=11)
+    agent[0, 3] = goal[0, 3]
+    g = env.get_graph(torch.from_numpy(agent).cuda(), torch.from_numpy(goal).cuda(), product_obstacles(env_id, obs))
+    nan_ref = torch.isnan(env.u_ref(g)).cpu()
+    assert nan_ref[0, 3].all() and int(nan_ref.sum()) == nan_ref[0, 3].numel()
+    for algo in ALGOS:
+        u = _controller(env, algo).get_qp_action(g)[0].cpu()
+        assert torch.equal(torch.isnan(u), nan_ref), algo
+        assert bool(torch.isfinite(u[~nan_ref]).all()), algo
+
+
 @pytest.mark.parametrize("algo", ALGOS)
 @pytest.mark.parametrize("env_id", ["SingleIntegrator", "DoubleIntegrator", "DubinsCar"])
 def test_closed_loop_matches_oracle(env_id, algo):

@@ -37,7 +37,6 @@ def run(args, N: int) -> dict:
     import torch
     from gcbfplus_b200 import _lib
     from gcbfplus_b200.algo import make_algo
-    from gcbfplus_b200.algo.cbf_qp import CAPPED_BIT
     from gcbfplus_b200.algo.train import QP_MAX_ITER, QP_TOL
     from gcbfplus_b200.env import make_env
     from gcbfplus_b200.trainer.rollout import RolloutEngine
@@ -94,10 +93,10 @@ def run(args, N: int) -> dict:
         if policy == "actor_refine":
             row["refine"] = eng.refine_stats()
         elif policy != "actor":
-            it = eng.chains[0].qp_iters.reshape(-1).to(torch.int64).cpu().numpy() & (CAPPED_BIT - 1)
+            it, dense = _lib.split_iters(eng.chains[0].qp_iters.reshape(-1).to(torch.int64).cpu().numpy())
             row["qp"] = dict(eng.qp_stats(), iters_mean=float(it.mean()),
                              iters_p90=float(np.percentile(it, 90)), iters_p99=float(np.percentile(it, 99)),
-                             dense_fallback=int(((eng.chains[0].qp_iters.cpu().numpy() & CAPPED_BIT) != 0).sum()))
+                             dense_fallback=int(dense.sum()))
         out[policy] = row
     out["clocks"] = clocks
     out["gpu"] = _gpu()

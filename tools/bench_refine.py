@@ -51,7 +51,6 @@ def run(args, weights: str) -> dict:
     import torch
     from gcbfplus_b200 import _lib
     from gcbfplus_b200.algo import make_algo
-    from gcbfplus_b200.algo.cbf_qp import CAPPED_BIT
     from gcbfplus_b200.env import make_env
     from gcbfplus_b200.trainer.rollout import RolloutEngine
     if not torch.cuda.is_available():
@@ -89,8 +88,8 @@ def run(args, weights: str) -> dict:
                        "rollouts_per_window": n, "launches_per_env_step": eng.launches_per_run / T}
         if policy == "actor_refine":
             it = eng.chains[0].refine_iters.reshape(-1).to(torch.int64).cpu().numpy()   # last timed rollout
-            k = it & (CAPPED_BIT - 1)
-            out["refine"] = dict(eng.refine_stats(), capped_frac=float(((it & CAPPED_BIT) != 0).mean()),
+            k, capped = _lib.split_iters(it)
+            out["refine"] = dict(eng.refine_stats(), capped_frac=float(capped.mean()),
                                  iters_mean=float(k.mean()),
                                  iters_hist={int(a): int(b) for a, b in zip(*np.unique(k, return_counts=True))})
         del eng
@@ -126,7 +125,7 @@ def run(args, weights: str) -> dict:
         cg.replay()
         torch.cuda.synchronize()
         floor[f"max_iter_{mi}"] = {"ms_per_call": _timed(cg.replay, args.floor_calls, args.repeats, clocks),
-                                   "iters_max": int((its & (CAPPED_BIT - 1)).max()),
+                                   "iters_max": int(_lib.split_iters(its)[0].max()),
                                    "graphs_value_0": int((v == 0).sum())}
         del cg
     d = float(np.median(floor["max_iter_30"]["ms_per_call"]) - np.median(floor["max_iter_1"]["ms_per_call"]))
