@@ -38,6 +38,12 @@ def test_cbfqp_argument_errors_without_gpu():
     nb = lib.gcbf_cbfqp_workspace_floats(ctypes.byref(big))
     rc = lib.gcbf_cbfqp_centralized(ctypes.byref(big), 1.0, 10, 1e-7, p, p, p, p, None, None, p, nb, None)
     assert rc < 0 and b"1024" in lib.gcbf_last_error_string()
+    # LinearDrone (NU = 3): 999 agents take 232,284 B of shared memory, 1000 would take 232,516 > 227 KB
+    drone = _desc(kind=3, N=1000)
+    nd = lib.gcbf_cbfqp_workspace_floats(ctypes.byref(drone))
+    rc = lib.gcbf_cbfqp_centralized(ctypes.byref(drone), 1.0, 10, 1e-7, p, p, p, p, None, None, p, nd, None)
+    msg = lib.gcbf_last_error_string()
+    assert rc < 0 and b"1000 agents" in msg and b"LinearDrone 999" in msg, msg
     tiny = _desc(N=1, R=1)
     rc = lib.gcbf_cbf_pairwise(ctypes.byref(tiny), p, p, p, p, p, p, p, None, None)
     assert rc < 0 and b"candidates" in lib.gcbf_last_error_string()

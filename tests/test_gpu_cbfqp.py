@@ -99,12 +99,13 @@ def test_pairwise_and_actions_match_oracle(env_id, N):
 
 def test_centralized_at_scale():
     """DoubleIntegrator N = 512, one graph: the 1536-row QP against the exact float64 minimiser of the kernel's own
-    data; the number of capped solves is reported."""
+    data, with an iteration budget the solve must converge within."""
     env, g, area, n_obs = _graph("DoubleIntegrator", 512, 1, seed=7)
-    cen = _controller(env, "centralized_cbf")
+    cen = _controller(env, "centralized_cbf", max_iter=200000)
     u, r = cen.get_qp_action(g)
     st = cen.iter_stats()
     print(f"centralized_cbf DoubleIntegrator N=512: {st}")
+    assert st["capped"] == 0, st
     pw = {k: v.cpu().numpy() for k, v in cen.pairwise(g).items()}
     Lg = cq.central_from_blocks(pw["idx"][0], pw["lg_self"][0], pw["lg_other"][0])
     b = (pw["lf_h"][0] + np.float32(1.0) * pw["h"][0]).astype(np.float64).reshape(-1)
@@ -114,9 +115,8 @@ def test_centralized_at_scale():
     assert (lam > 1e-9).any()
     slack = -(Lg @ uo) - ro - b
     assert max(float(np.maximum(slack, 0).max()), float(np.abs(lam * slack).max())) <= 1e-8
-    if st["capped"] == 0:
-        np.testing.assert_allclose(u.cpu().numpy().reshape(-1), uo, atol=1e-5)
-        np.testing.assert_allclose(r.cpu().numpy().reshape(-1), ro, atol=1e-4)
+    np.testing.assert_allclose(u.cpu().numpy().reshape(-1), uo, atol=1e-5)
+    np.testing.assert_allclose(r.cpu().numpy().reshape(-1), ro, atol=1e-4)
 
 
 def test_qp_stats_reports_capped_solves():

@@ -31,10 +31,11 @@ CASES = [("SingleIntegrator", 8, 3, 0.9, 4, 3), ("DoubleIntegrator", 16, 3, 1.6,
          ("DubinsCar", 12, 2, 1.4, 6, 5), ("LinearDrone", 10, 2, 1.0, 4, 6)]
 
 
-def _dense_from_device(env, algo, graph, N, nu):
-    """Rebuild per-graph dense (b, Lg_h [N, N*nu], u_ref) from the workspace the library just filled."""
+def _qp_from_device(env, ws, graph, N, nu, sparse=False):
+    """Rebuild per-graph (h, b, Lg_h [N, N*nu], u_ref, row scale s) from the QP workspace `ws` the library just filled.
+    Lg_h is dense, or scipy CSR with sparse (cheap at N = 2048)."""
+    import scipy.sparse as sp
     from gcbfplus_b200 import _lib
-    ws = algo._qp_ws["ws"]
     d = env.desc(graph.n_graphs, 0, edge_cap=graph.edge_recv.numel())
     offs = (C.c_int64 * 8)()
     _lib.check(env.lib.gcbf_qp_workspace_layout(C.byref(d), offs), "layout")
@@ -45,22 +46,27 @@ def _dense_from_device(env, algo, graph, N, nu):
     qs = w[offs[3]: offs[3] + A * 4].reshape(A, 4)
     qe = w[offs[4]: offs[4] + cap * 4].reshape(cap, 4)
     ur = w[offs[5]: offs[5] + A * 4].reshape(A, 4)
+    qsc = w[offs[6]: offs[6] + A]
     rev = w[offs[7]: offs[7] + cap].view(np.int32)
     rs, rd = graph.row_start.cpu().numpy(), graph.row_deg.cpu().numpy()
     src = graph.edge_src.cpu().numpy()
+    # every stored edge of every receiver a, in row order
+    recv = np.repeat(np.arange(A), rd)
+    e = np.repeat(rs, rd) + np.arange(rd.sum()) - np.repeat(np.cumsum(rd) - rd, rd)
+    agent_edge = src[e] >= 0
+    recv, e = recv[agent_edge], e[agent_edge]
+    assert (rev[e] >= 0).all() and (src[rev[e]] == recv).all(), "mirror edge missing: radius graph not symmetric?"
+    ar = np.arange(nu)
     out = []
     for g in range(graph.n_graphs):
-        Lg = np.zeros((N, N * nu))
-        for i in range(N):
-            a = g * N + i
-            Lg[i, i * nu:(i + 1) * nu] = qs[a, :nu]
-            for e in range(rs[a], rs[a] + rd[a]):
-                if src[e] >= 0:
-                    j = src[e] - g * N
-                    Lg[i, j * nu:(j + 1) * nu] = qe[e, :nu]
-                    assert rev[e] >= 0 and src[rev[e]] == a, "mirror edge missing: radius graph not symmetric?"
-        out.append(dict(h=h[g * N:(g + 1) * N].astype(np.float64), b=qb[g * N:(g + 1) * N].astype(np.float64), Lg=Lg,
-                        u_ref=ur[g * N:(g + 1) * N, :nu].reshape(-1).astype(np.float64)))
+        lo, hi = g * N, (g + 1) * N
+        sel = (recv >= lo) & (recv < hi)
+        rows = np.concatenate([np.repeat(np.arange(N), nu), np.repeat(recv[sel] - lo, nu)])
+        cols = np.concatenate([(np.arange(N)[:, None] * nu + ar).ravel(), ((src[e[sel]] - lo)[:, None] * nu + ar).ravel()])
+        vals = np.concatenate([qs[lo:hi, :nu].ravel(), qe[e[sel], :nu].ravel()]).astype(np.float64)
+        Lg = sp.csr_matrix((vals, (rows, cols)), shape=(N, N * nu))
+        out.append(dict(h=h[lo:hi].astype(np.float64), b=qb[lo:hi].astype(np.float64), Lg=Lg if sparse else Lg.toarray(),
+                        u_ref=ur[lo:hi, :nu].reshape(-1).astype(np.float64), s=qsc[lo:hi].astype(np.float64)))
     return out
 
 
@@ -119,7 +125,7 @@ def test_qp_labels_match_oracle(env_id, N, G, area, n_obs, seed, gemm_path):
     torch.cuda.synchronize()
     graph.check_overflow()
     nu = env.action_dim
-    dev = _dense_from_device(env, algo, graph, N, nu)
+    dev = _qp_from_device(env, algo._qp_ws["ws"], graph, N, nu)
     u_dev = u_dev.cpu().numpy().astype(np.float64)
     aux = aux.cpu().numpy().astype(np.float64)
     packed = pobs.packed.cpu().numpy()
@@ -159,7 +165,7 @@ def test_qp_labels_kkt_at_scale(gemm_path):
     u_dev, aux, iters = qp_labels(algo, graph, params=algo.cbf_params, with_aux=True)
     torch.cuda.synchronize()
     graph.check_overflow()
-    dev = _dense_from_device(env, algo, graph, N, env.action_dim)
+    dev = _qp_from_device(env, algo._qp_ws["ws"], graph, N, env.action_dim)
     u_dev = u_dev.cpu().numpy().astype(np.float64)
     aux = aux.cpu().numpy().astype(np.float64)
     packed = pobs.packed.cpu().numpy()
@@ -191,7 +197,7 @@ def test_qp_labels_dense_graph_fallback():
     torch.cuda.synchronize()
     graph.check_overflow()
     assert int(graph.row_deg.min()) > 25
-    dev = _dense_from_device(env, algo, graph, N, env.action_dim)
+    dev = _qp_from_device(env, algo._qp_ws["ws"], graph, N, env.action_dim)
     for g in range(G):
         ud = u_dev[g].cpu().numpy().astype(np.float64).reshape(-1)
         ax = aux[g].cpu().numpy().astype(np.float64)

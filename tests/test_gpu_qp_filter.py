@@ -82,7 +82,7 @@ def test_null_nominal_is_the_labels(env_id, N, G, area, n_obs, seed, gemm_path):
 @pytest.mark.parametrize("env_id,N,G,area,n_obs,seed", CASES)
 def test_random_nominals_match_oracle(env_id, N, G, area, n_obs, seed, gemm_path):
     from oracle import qp
-    from test_gpu_qp import _dense_from_device
+    from test_gpu_qp import _qp_from_device
     env, algo, graph, _ = _scene(env_id, N, G, area, n_obs, seed)
     nu = env.action_dim
     u_lim = float(env.action_lim()[1][0])
@@ -94,7 +94,7 @@ def test_random_nominals_match_oracle(env_id, N, G, area, n_obs, seed, gemm_path
     torch.cuda.synchronize()
     graph.check_overflow()
     assert int(iters.max()) < 20000, "dual iteration did not reach its tolerance"
-    dev = _dense_from_device(env, algo, graph, N, nu)
+    dev = _qp_from_device(env, algo._qp_ws["ws"], graph, N, nu)
     u_dev = u_dev.cpu().numpy().astype(np.float64)
     r_dev = r_dev.cpu().numpy().astype(np.float64)
     n_active = n_moved = n_box = 0
