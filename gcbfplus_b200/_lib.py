@@ -107,7 +107,14 @@ _SIGNATURES = {
                              [C.c_int64, _P]),
     "gcbf_cbfqp_centralized": (C.c_int32, [C.POINTER(EnvDesc), C.c_float, C.c_int32, C.c_float] + [_P] * 7 +
                                [C.c_int64, _P]),
+    "gcbf_perturb_observation": (C.c_int32, [C.POINTER(EnvDesc), _P, C.c_int64, C.c_int64] + [_P] * 5),
+    "gcbf_perturb_action": (C.c_int32, [C.POINTER(EnvDesc), _P, C.c_int64, C.c_int64, _P, _P]),
+    "gcbf_normal_draws": (C.c_int32, [C.c_uint64, C.c_int32, _P, C.c_int64, _P, _P]),
 }
+
+#: floats of the noise buffer of gcbf_perturb_observation / gcbf_perturb_action (GCBF_NOISE_FLOATS) and its layout:
+#: the uint64 seed in words 0-1, sigma_x from word 2, sigma_l at word 8, sigma_u from word 9
+NOISE_FLOATS, NOISE_SIGMA_X, NOISE_SIGMA_L, NOISE_SIGMA_U = 16, 2, 8, 9
 
 
 def lib_path() -> str:

@@ -28,6 +28,7 @@ UNITS = {  # translation unit -> extra flags
     "falsify.cu": ["-fmad=false"],
     "geometry.cu": ["-fmad=false"],
     "gnn.cu": ["-fmad=false"],
+    "noise.cu": ["-fmad=false"],
     "qp.cu": ["-fmad=false"],
     "refine.cu": ["-fmad=false"],
     "rollout_persist.cu": ["-fmad=false"],

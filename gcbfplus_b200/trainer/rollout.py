@@ -22,12 +22,19 @@ g // (n_envs // n_nets).  Where the persistent kernel applies, ONE gcbf_rollout_
 network, each cluster reading its own network's weights, so every network's environments get the bits a solo persistent
 rollout of that network gives them.  Otherwise (LinearDrone, n > 512, deeper actors, persistent=False or not chosen by
 default) the engine runs one solo engine per network, one after another, and gathers their records.
+Observation and actuation noise (a Perturbation; DESIGN.md 4.11) runs on the step-by-step path for every policy: per
+step the observed states and LiDAR hits of the true graph (gcbf_perturb_observation), the policy on them, the action
+noise (gcbf_perturb_action), env.step of the TRUE state with the applied action, and the graph build of the next true
+state.  The `actor` policy then runs the modular sequence (policy forward with every edge feature norm-clipped,
+gcbf_act, the noise, gcbf_env_step mode 1) instead of the fused gcbf_rollout_step_l, which feeds one state array to the
+network and to the integrator.
 """
 from __future__ import annotations
 
 import ctypes as C
+import math
 import os
-from typing import Optional
+from typing import Optional, Sequence, Union
 
 import torch
 
@@ -42,6 +49,62 @@ from .data import Rollout
 
 #: the CBF-QP safety-filter policies: the nominal action of each, filtered by the learned CBF
 QP_FILTER_POLICIES = ("actor_qp", "u_ref_qp")
+
+
+def _sigmas(value, name: str) -> tuple:
+    vals = tuple(float(v) for v in value) if hasattr(value, "__len__") else (float(value),)
+    if not vals:
+        raise ValueError(f"{name} is empty")
+    bad = [v for v in vals if not math.isfinite(v) or v < 0]
+    if bad:
+        raise ValueError(f"{name} must be finite and >= 0, got {bad[0]}")
+    return vals
+
+
+class Perturbation:
+    """Observation and actuation noise of a rollout (DESIGN.md 4.11), every sigma absolute, in the environment's units:
+    x_hat = x + state_sigma z per state component, h_hat = h + lidar_sigma z per LiDAR hit coordinate (rays that hit
+    nothing stay as they are), a = a_cmd + action_sigma z per action component, z ~ N(0, 1).
+    state_sigma / action_sigma: one value for every component or one per component (state_dim / action_dim values).
+    seed: the generator key, an int in [0, 2**64).  env_offset: the episode index of the engine's environment 0; the draws
+    of episode k depend on (seed, k, t) only, so an episode gets the same noise in any batch it runs in."""
+
+    def __init__(self, state_sigma: Union[float, Sequence[float]], lidar_sigma: float,
+                 action_sigma: Union[float, Sequence[float]], seed: int, env_offset: int = 0):
+        self.state_sigma = _sigmas(state_sigma, "state_sigma")
+        lidar = _sigmas(lidar_sigma, "lidar_sigma")
+        if len(lidar) != 1:
+            raise ValueError(f"lidar_sigma is one value, got {len(lidar)}")
+        self.lidar_sigma = lidar[0]
+        self.action_sigma = _sigmas(action_sigma, "action_sigma")
+        if int(seed) != seed or not 0 <= int(seed) < 2 ** 64:
+            raise ValueError(f"seed must be an int in [0, 2**64), got {seed!r}")
+        if int(env_offset) != env_offset or int(env_offset) < 0:
+            raise ValueError(f"env_offset must be an int >= 0, got {env_offset!r}")
+        self.seed, self.env_offset = int(seed), int(env_offset)
+
+    @staticmethod
+    def _per_component(vals: tuple, n: int, name: str) -> list:
+        if len(vals) == 1:
+            return list(vals) * n
+        if len(vals) != n:
+            raise ValueError(f"{name} has {len(vals)} values; give one, or one per component ({n})")
+        return list(vals)
+
+    def sigmas(self, env) -> tuple:
+        """(state sigmas [state_dim], lidar sigma, action sigmas [action_dim]) for env; refuses a length mismatch."""
+        return (self._per_component(self.state_sigma, env.state_dim, "state_sigma"), self.lidar_sigma,
+                self._per_component(self.action_sigma, env.action_dim, "action_sigma"))
+
+    def pack(self, env) -> torch.Tensor:
+        """The noise buffer of gcbf_perturb_observation / gcbf_perturb_action (host, _lib.NOISE_FLOATS floats)."""
+        sx, sl, su = self.sigmas(env)
+        buf = torch.zeros(_lib.NOISE_FLOATS, dtype=torch.float32)
+        buf.view(torch.int64)[0] = self.seed - (1 << 64 if self.seed >= 1 << 63 else 0)
+        buf[_lib.NOISE_SIGMA_X:_lib.NOISE_SIGMA_X + len(sx)] = torch.tensor(sx)
+        buf[_lib.NOISE_SIGMA_L] = sl
+        buf[_lib.NOISE_SIGMA_U:_lib.NOISE_SIGMA_U + len(su)] = torch.tensor(su)
+        return buf
 
 
 class _Chain:
@@ -116,8 +179,12 @@ def check_nets(nets, n_nets: int) -> list:
 class RolloutEngine:
     def __init__(self, env, n_envs: int, T: Optional[int] = None, n_obs: Optional[int] = None,
                  use_cuda_graph: bool = True, policy: str = "actor", persistent: Optional[bool] = None,
-                 n_nets: int = 1, net_of_env=None):
-        """n_nets: number of actor networks (policy 'actor' only).  Environment g runs network net_of_env[g]; the
+                 n_nets: int = 1, net_of_env=None, perturbation: Optional[Perturbation] = None):
+        """perturbation: observation and actuation noise (a Perturbation; set_perturbation() changes it between runs).
+        It runs on the step-by-step path: persistent=True with a perturbation is refused, the default choice takes the
+        step path, and n_nets must be 1.  Every policy then acts on the observed states and LiDAR hits; the CBF-QP
+        baselines pick their nearest candidates from the observed states, so for them the topology is the observed one.
+        n_nets: number of actor networks (policy 'actor' only).  Environment g runs network net_of_env[g]; the
         default table gives each network n_envs // n_nets consecutive environments (n_envs % n_nets == 0).
         policy: 'actor' (a = 2 pi + u_ref, algo.step), 'actor_refine' (that action refined against the CBF,
         GCBFPlus.online_policy_refinement; set_cbf_params() gives the CBF), 'actor_qp' / 'u_ref_qp' (2 pi + u_ref or
@@ -153,6 +220,13 @@ class RolloutEngine:
         #: the network of every environment (host list) and each network's environments
         self.net_table = check_net_table(net_of_env, self.n_nets, n_envs)
         self.net_envs = [[g for g, k in enumerate(self.net_table) if k == j] for j in range(self.n_nets)]
+        if perturbation is not None:
+            if persistent:
+                raise ValueError("the persistent rollout has no noise model: a perturbation runs on the step-by-step "
+                                 "path (persistent=False or None)")
+            if self.n_nets > 1:
+                raise ValueError("a perturbation needs n_nets = 1")
+            persistent = False
         # actor_refine / actor_qp / u_ref_qp: a copy of the CBF, its prepared planes (actor_refine) and the settings
         # (set_cbf_params)
         self.cbf_params: Optional[NetParams] = None
@@ -171,6 +245,17 @@ class RolloutEngine:
         self.rewards = torch.zeros(T, E, dtype=f32, device=dev)
         self.costs = torch.zeros(T, E, dtype=f32, device=dev)
         self.chains = [_Chain(self)]   # a one-element list: bench.py reads eng.chains[0]
+        #: the perturbation, its device noise buffer, the record of the observed states [T, E, N, sd] and the observed
+        #: LiDAR hits of the current step (scratch: a record would be as large as `hits`)
+        self.perturbation: Optional[Perturbation] = None
+        self._noise: Optional[torch.Tensor] = None
+        self.obs_agent: Optional[torch.Tensor] = None
+        self._obs_hits: Optional[torch.Tensor] = None
+        if perturbation is not None:
+            self._noise = torch.zeros(_lib.NOISE_FLOATS, dtype=f32, device=dev)
+            self.obs_agent = torch.zeros(T, E, N, sd, dtype=f32, device=dev)
+            self._obs_hits = torch.zeros(E, N, R, pd, dtype=f32, device=dev)
+            self.set_perturbation(perturbation)
         self.desc = self.chains[0].desc
         self.params_buf = torch.zeros(_lib.param_count(env.edge_dim, nu), dtype=f32, device=dev)
         # folded inference weights (gcbf_prepare_infer), rebuilt by set_params()
@@ -256,17 +341,54 @@ class RolloutEngine:
                                       ch.counters[t].data_ptr(), self._build_flags, stream)
         _lib.check(rc, "gcbf_graph_build")
 
+    def _observe(self, ch: _Chain, t: int, stream: int) -> tuple:
+        """The agent states and LiDAR hits the policy acts on at step t: the true ones, or with a perturbation the
+        observed ones (enqueued here)."""
+        if self._noise is None:
+            return self.agent[t, ch.e0], self.hits[t, ch.e0]
+        rc = self.env.lib.gcbf_perturb_observation(C.byref(ch.desc), self._noise.data_ptr(), t,
+                                                   self.perturbation.env_offset, self.agent[t, ch.e0].data_ptr(),
+                                                   self.hits[t, ch.e0].data_ptr(), self.obs_agent[t].data_ptr(),
+                                                   self._obs_hits.data_ptr(), stream)
+        _lib.check(rc, "gcbf_perturb_observation")
+        return self.obs_agent[t], self._obs_hits
+
+    def _actuate(self, ch: _Chain, t: int, stream: int) -> None:
+        """With a perturbation, the action noise on the commanded actions[t] (in place: the record holds the applied
+        actions)."""
+        if self._noise is not None:
+            rc = self.env.lib.gcbf_perturb_action(C.byref(ch.desc), self._noise.data_ptr(), t,
+                                                  self.perturbation.env_offset, self.actions[t, ch.e0].data_ptr(), stream)
+            _lib.check(rc, "gcbf_perturb_action")
+
+    def _actor_forward(self, ch: _Chain, args: tuple, clip_all: int, stream: int) -> None:
+        """pi of the actor on the graph arrays `args` (agent, goal, hits, row_start, row_deg, edge_recv, edge_src,
+        counters) -> ch.pi."""
+        env, d = self.env, ch.desc
+        if self.n_layers > 1:
+            rc = env.lib.gcbf_gnn_forward_l(C.byref(d), _lib.NET_ACTOR, env.action_dim, self.n_layers,
+                                            self.params_buf.data_ptr(), self.infer_blob.data_ptr(),
+                                            *[_lib.ptr(x) for x in args], clip_all, ch.pi.data_ptr(), ch.ws.data_ptr(),
+                                            ch.ws.numel(), stream)
+            _lib.check(rc, "gcbf_gnn_forward_l")
+            return
+        rc = env.lib.gcbf_gnn_infer(C.byref(d), _lib.NET_ACTOR, env.action_dim, self.params_buf.data_ptr(),
+                                    self.infer_blob.data_ptr(), self.use_tc, *[_lib.ptr(x) for x in args], clip_all,
+                                    ch.pi.data_ptr(), ch.ws.data_ptr(), ch.ws.numel(), stream)
+        _lib.check(rc, "gcbf_gnn_infer")
+
     def _step(self, ch: _Chain, t: int, stream: int) -> None:
         env, d = self.env, ch.desc
         obs = self.obstacles[ch.e0].data_ptr() if self.O > 0 else None
         b = t % 2
+        x, h = self._observe(ch, t, stream)
         if self.policy == "actor_refine":
-            self._step_refine(ch, t, stream)
+            self._step_refine(ch, t, x, h, stream)
             return
         if self.policy in QP_FILTER_POLICIES:
-            self._step_qp_filter(ch, t, stream)
+            self._step_qp_filter(ch, t, x, h, stream)
             return
-        if self.policy == "actor":      # algo.step + env.step + get_graph(next) in one call
+        if self.policy == "actor" and self._noise is None:      # algo.step + env.step + get_graph(next) in one call
             rc = env.lib.gcbf_rollout_step_l(
                 C.byref(d), self.n_layers, self.params_buf.data_ptr(), self.infer_blob.data_ptr(), self.use_tc,
                 self.agent[t, ch.e0].data_ptr(), self.goal[ch.e0].data_ptr(), obs, env.ray_table.data_ptr(),
@@ -282,12 +404,22 @@ class RolloutEngine:
         mode = 2                        # u_ref policy
         if self.controller is not None:  # CBF-QP action, then env.step with it as input
             c = self.controller
-            rc = getattr(env.lib, c._ENTRY)(C.byref(d), c.alpha, c.max_iter, c.tol, self.agent[t, ch.e0].data_ptr(),
-                                            self.goal[ch.e0].data_ptr(), self.hits[t, ch.e0].data_ptr(),
+            rc = getattr(env.lib, c._ENTRY)(C.byref(d), c.alpha, c.max_iter, c.tol, x.data_ptr(),
+                                            self.goal[ch.e0].data_ptr(), h.data_ptr(),
                                             self.actions[t, ch.e0].data_ptr(), ch.qp_r.data_ptr(),
                                             ch.qp_iters[t].data_ptr(), ch.qp_ws.data_ptr(), ch.qp_ws.numel(), stream)
             _lib.check(rc, c._ENTRY)
             mode = env.action_step_mode
+        elif self._noise is not None:   # actor / u_ref from the observation: 2 pi + u_ref(x_hat) or u_ref(x_hat)
+            pi = None
+            if self.policy == "actor":
+                self._actor_forward(ch, (x, self.goal[ch.e0], h, ch.row_start[b], ch.row_deg[b], ch.edge_recv[b],
+                                         ch.edge_src[b], ch.counters[t]), 1, stream)
+                pi = ch.pi.data_ptr()
+            _lib.check(env.lib.gcbf_act(C.byref(d), x.data_ptr(), self.goal[ch.e0].data_ptr(), pi,
+                                        self.actions[t, ch.e0].data_ptr(), stream), "gcbf_act")
+            mode = 1
+        self._actuate(ch, t, stream)
         rc = env.lib.gcbf_env_step(C.byref(d), self.agent[t, ch.e0].data_ptr(), self.goal[ch.e0].data_ptr(), obs,
                                    None, ch.row_start[b].data_ptr(), ch.row_deg[b].data_ptr(), ch.edge_src[b].data_ptr(),
                                    self.actions[t, ch.e0].data_ptr(), self.agent[t + 1, ch.e0].data_ptr(),
@@ -295,22 +427,19 @@ class RolloutEngine:
         _lib.check(rc, "gcbf_env_step")
         self._build(ch, t + 1, stream)
 
-    def _step_refine(self, ch: _Chain, t: int, stream: int) -> None:
-        """policy forward -> refined action (gcbf_refine_actions, iterations recorded per graph) -> env.step with it as
-        input -> graph build of the next state."""
+    def _step_refine(self, ch: _Chain, t: int, x: torch.Tensor, h: torch.Tensor, stream: int) -> None:
+        """policy forward on (x, h) -> refined action (gcbf_refine_actions, iterations recorded per graph) -> env.step
+        with it as input -> graph build of the next state."""
         env, d = self.env, ch.desc
         if self.cbf_params is None:
             raise RuntimeError("the actor_refine policy needs the CBF: call set_cbf_params() before run()")
         b = t % 2
-        args = (self.agent[t, ch.e0], self.goal[ch.e0], self.hits[t, ch.e0], ch.row_start[b], ch.row_deg[b],
-                ch.edge_recv[b], ch.edge_src[b], ch.counters[t])
-        rc = env.lib.gcbf_gnn_infer(C.byref(d), _lib.NET_ACTOR, env.action_dim, self.params_buf.data_ptr(),
-                                    self.infer_blob.data_ptr(), self.use_tc, *[_lib.ptr(x) for x in args], 0,
-                                    ch.pi.data_ptr(), ch.ws.data_ptr(), ch.ws.numel(), stream)
-        _lib.check(rc, "gcbf_gnn_infer")
+        args = (x, self.goal[ch.e0], h, ch.row_start[b], ch.row_deg[b], ch.edge_recv[b], ch.edge_src[b], ch.counters[t])
+        self._actor_forward(ch, args, 0, stream)
         launch_refine(env, d, self.refine_alpha, self.refine_lr, self.refine_max_iter, self.use_tc, self.cbf_params,
                       self._refine_planes, ch.pi, *args, self.actions[t, ch.e0], None,
                       ch.refine_iters[t], ch.refine_ws, stream)
+        self._actuate(ch, t, stream)
         obs = self.obstacles[ch.e0].data_ptr() if self.O > 0 else None
         rc = env.lib.gcbf_env_step(C.byref(d), self.agent[t, ch.e0].data_ptr(), self.goal[ch.e0].data_ptr(), obs,
                                    None, ch.row_start[b].data_ptr(), ch.row_deg[b].data_ptr(), ch.edge_src[b].data_ptr(),
@@ -319,22 +448,18 @@ class RolloutEngine:
         _lib.check(rc, "gcbf_env_step")
         self._build(ch, t + 1, stream)
 
-    def _step_qp_filter(self, ch: _Chain, t: int, stream: int) -> None:
-        """nominal action (actor_qp: policy forward and 2 pi + u_ref; u_ref_qp: u_ref) -> the CBF-QP nearest to it
-        (gcbf_qp_filter; iterations, nominal and (lam, r) recorded) -> env.step with the filtered action as input ->
-        graph build of the next state."""
+    def _step_qp_filter(self, ch: _Chain, t: int, x: torch.Tensor, h: torch.Tensor, stream: int) -> None:
+        """nominal action on (x, h) (actor_qp: policy forward and 2 pi + u_ref; u_ref_qp: u_ref) -> the CBF-QP nearest
+        to it (gcbf_qp_filter; iterations, nominal and (lam, r) recorded) -> env.step with the filtered action as
+        input -> graph build of the next state."""
         env, d = self.env, ch.desc
         if self.cbf_params is None:
             raise RuntimeError(f"the {self.policy} policy needs the CBF: call set_cbf_params() before run()")
         b = t % 2
-        args = (self.agent[t, ch.e0], self.goal[ch.e0], self.hits[t, ch.e0], ch.row_start[b], ch.row_deg[b],
-                ch.edge_recv[b], ch.edge_src[b], ch.counters[t])
+        args = (x, self.goal[ch.e0], h, ch.row_start[b], ch.row_deg[b], ch.edge_recv[b], ch.edge_src[b], ch.counters[t])
         pi = None
         if self.policy == "actor_qp":
-            rc = env.lib.gcbf_gnn_infer(C.byref(d), _lib.NET_ACTOR, env.action_dim, self.params_buf.data_ptr(),
-                                        self.infer_blob.data_ptr(), self.use_tc, *[_lib.ptr(x) for x in args], 0,
-                                        ch.pi.data_ptr(), ch.ws.data_ptr(), ch.ws.numel(), stream)
-            _lib.check(rc, "gcbf_gnn_infer")
+            self._actor_forward(ch, args, 0, stream)
             pi = ch.pi.data_ptr()
         nominal = ch.qp_nominal[t]
         _lib.check(env.lib.gcbf_act(C.byref(d), _lib.ptr(args[0]), _lib.ptr(args[1]), pi, nominal.data_ptr(), stream),
@@ -346,6 +471,7 @@ class RolloutEngine:
                                     self.actions[t, ch.e0].data_ptr(), ch.qp_aux[t].data_ptr(),
                                     ch.qp_iters[t].data_ptr(), ch.qp_ws.data_ptr(), ch.qp_ws.numel(), stream)
         _lib.check(rc, "gcbf_qp_filter")
+        self._actuate(ch, t, stream)
         obs = self.obstacles[ch.e0].data_ptr() if self.O > 0 else None
         rc = env.lib.gcbf_env_step(C.byref(d), self.agent[t, ch.e0].data_ptr(), self.goal[ch.e0].data_ptr(), obs,
                                    None, ch.row_start[b].data_ptr(), ch.row_deg[b].data_ptr(), ch.edge_src[b].data_ptr(),
@@ -547,6 +673,20 @@ class RolloutEngine:
         if settings != (self.refine_alpha, self.refine_lr, self.refine_max_iter):
             self._graph = None      # the settings are baked into the captured launches
         self.refine_alpha, self.refine_lr, self.refine_max_iter = settings
+
+    def set_perturbation(self, perturbation: Perturbation) -> None:
+        """Change the noise of an engine built with a perturbation.  The seed and the sigmas live in a device buffer, so
+        a captured rollout keeps its CUDA graph; a new env_offset is a launch parameter and the next run() re-captures."""
+        if self._noise is None:
+            raise RuntimeError("set_perturbation() needs an engine built with a perturbation "
+                               "(RolloutEngine(..., perturbation=...)): the noiseless engine may take the persistent path")
+        if not isinstance(perturbation, Perturbation):
+            raise TypeError(f"set_perturbation takes a Perturbation, got {type(perturbation).__name__}")
+        buf = perturbation.pack(self.env)
+        if self.perturbation is not None and perturbation.env_offset != self.perturbation.env_offset:
+            self._graph = None
+        self._noise.copy_(buf)      # synchronous: buf is pageable host memory
+        self.perturbation = perturbation
 
     def refine_stats(self) -> dict:
         """actor_refine: median / max refinement iterations and the graph-steps that stopped at the cap, over every

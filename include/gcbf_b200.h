@@ -481,6 +481,33 @@ int32_t gcbf_cbfqp_centralized(const gcbf_env_desc* desc, float alpha, int32_t m
                                const float* agent, const float* goal, const float* hits, float* u, float* r,
                                int32_t* iters, float* workspace, int64_t workspace_floats, void* stream);
 
+/* ---------------------------------------------------------------- observation and actuation noise
+ * The perturbation model of the step-by-step rollout (DESIGN.md 4.11): every agent observes x_hat = x + sigma_x z of
+ * each agent state and h_hat = h + sigma_l z of each LiDAR hit position (the network sees the TRUE graph's edges with
+ * features recomputed from the observed states, gcbf_gnn_infer with clip_all = 1), and the applied action is
+ * a = a_cmd + sigma_u z.  z ~ N(0, 1) from Philox4x64-10 with key (seed, kind), kind 0 = state, 1 = LiDAR, 2 = action,
+ * and counter (t, env_offset + g, agent, block): one call gives the 64-bit words w0..w3, u_k = ((w_k >> 11) + 1/2) 2^-53
+ * in fp64, Box-Muller (fp64) z0, z1 from (u0, u1) and z2, z3 from (u2, u3), each rounded to fp32 once; block j holds
+ * components 4j .. 4j + 3 of the agent's flattened state [sd], LiDAR [R, pd] or action [nu] vector (draws past its end
+ * are discarded).  Then delta = sigma z and x + delta in fp32.  A component whose sigma is 0 is copied, so with every
+ * sigma 0 the outputs equal the inputs bit for bit; a hit farther than 2 comm_radius from its agent (the no-hit
+ * sentinel of a ray that hit nothing) is always copied.  The draws of an episode depend only on (seed, t, env_offset +
+ * g): not on the batch size or the number of calls.
+ *   noise [GCBF_NOISE_FLOATS] (device, 8-byte aligned): words 0-1 the uint64 seed (little-endian), 2-7 sigma_x (the first
+ *     sd used), 8 sigma_l, 9-11 sigma_u (the first nu used).  Read at run time: a captured launch sees new values.
+ *   t >= 0: the step; env_offset >= 0: the episode index of graph 0.
+ * gcbf_perturb_observation: agent [G,N,sd], hits [G,N,R,pd] (true) -> obs_agent, obs_hits (same shapes, must not alias
+ *   the inputs).  One thread per component, one launch.
+ * gcbf_perturb_action: action_inout [G,N,nu] += sigma_u z, in place.  One launch.
+ * gcbf_normal_draws: out [n, 4] <- the fp32 z of counters [n, 4] (uint64) under key (seed, kind); test hook of the
+ *   generator.  No launch when n == 0. */
+#define GCBF_NOISE_FLOATS 16
+int32_t gcbf_perturb_observation(const gcbf_env_desc* desc, const float* noise, int64_t t, int64_t env_offset,
+                                 const float* agent, const float* hits, float* obs_agent, float* obs_hits, void* stream);
+int32_t gcbf_perturb_action(const gcbf_env_desc* desc, const float* noise, int64_t t, int64_t env_offset,
+                            float* action_inout, void* stream);
+int32_t gcbf_normal_draws(uint64_t seed, int32_t kind, const uint64_t* counters, int64_t n, float* out, void* stream);
+
 /* ---------------------------------------------------------------- dense-layer building blocks
  * The fp32 GEMM family the MLPs are made of (flax nn.Dense, gcbfplus/nn/mlp.py:19-21, and its
  * autodiff transposes).  Exported so the kernels can be unit-tested against a plain fp32

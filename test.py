@@ -18,7 +18,13 @@ together (RolloutEngine with n_nets networks: one persistent launch where it app
 by success rate.  --log appends one row per network (step first, then test_log.csv's columns) to <run>/test_sweep.csv.
 --falsify ITERS (with --path) searches for states where the trained CBF's condition fails under the policy
 (GCBFPlus.falsify: ITERS normalised gradient-ascent iterations) from every recorded step of the evaluation episodes,
-prints one summary line and writes <path>/falsify/step<S>.npz."""
+prints one summary line and writes <path>/falsify/step<S>.npz.
+--state-noise S [S ...] (one value or state_dim values), --lidar-noise S and --action-noise S [S ...] evaluate the
+controller under observation and actuation noise (trainer/rollout.py Perturbation, DESIGN.md 4.11): every agent acts on
+x + S z of the agent states and on noisy LiDAR hits, and the applied action is the commanded one plus S z.  The draws
+come from --noise-seed (default: --seed) and each episode's index (--offset counts), so an episode gets the same noise
+in any batch.  One line reports the sigmas and the realised mean |x_hat - x|; --log writes to test_log_noise.csv, the
+sigmas and seed first."""
 import argparse
 import os
 
@@ -29,7 +35,7 @@ from gcbfplus_b200.algo import make_algo
 from gcbfplus_b200.algo.cbf_qp import BASELINES
 from gcbfplus_b200.algo.train import QP_MAX_ITER
 from gcbfplus_b200.env import make_env
-from gcbfplus_b200.trainer.rollout import RolloutEngine
+from gcbfplus_b200.trainer.rollout import Perturbation, RolloutEngine
 from gcbfplus_b200.trainer.utils import cbf_contours, test_rates
 
 
@@ -37,6 +43,7 @@ def test(args):
     print(f"> Running test.py {args}")
     if args.cpu:
         raise SystemExit("--cpu: gcbfplus_b200 is the sm_90a CUDA path only (no CPU fallback by design)")
+    perturbation = noise_perturbation(args)
     check_falsify_flags(args)
     if check_sweep_flags(args):
         test_sweep(args)
@@ -52,6 +59,11 @@ def test(args):
     num_agents = config.num_agents if args.num_agents is None else args.num_agents
     env = make_env(env_id=config.env if args.env is None else args.env, num_agents=num_agents, num_obs=args.obs,
                    area_size=args.area_size, max_step=args.max_step, max_travel=args.max_travel)
+    if perturbation is not None:
+        try:
+            perturbation.sigmas(env)
+        except ValueError as e:
+            raise SystemExit(f"noise flags: {e}")
     policy = "u_ref"
     algo = None
     baseline = args.algo in BASELINES and args.path is None and not args.u_ref
@@ -89,7 +101,7 @@ def test(args):
         path = os.path.join(f"./logs/{args.env}/nominal")
         os.makedirs(path, exist_ok=True)
     n_epi = args.epi - args.offset
-    eng = RolloutEngine(env, n_epi, T=env.max_episode_steps, policy=policy)
+    eng = RolloutEngine(env, n_epi, T=env.max_episode_steps, policy=policy, perturbation=perturbation)
     if algo is not None and not baseline:
         eng.set_params(algo.actor_params)
         if args.online_refine or args.qp_filter:
@@ -108,6 +120,11 @@ def test(args):
         print(f"epi: {i}, reward: {rewards[i]:.3f}, cost: {costs[i]:.3f}, safe rate: {rates[i, 0] * 100:.3f}%,"
               f"finish rate: {rates[i, 1] * 100:.3f}%, success rate: {rates[i, 2] * 100:.3f}%")
     print(summary["line"])
+    if perturbation is not None:
+        sx, sl, su = perturbation.sigmas(env)
+        err = float((eng.obs_agent - eng.agent[:-1]).abs().mean())
+        print(f"noise: state sigma {sx}, LiDAR sigma {sl}, action sigma {su}, seed {perturbation.seed}; "
+              f"realised mean |x_hat - x| {err:.6f}")
     if baseline or args.qp_filter:
         st = eng.qp_stats()
         print(f"QP iterations: median {st['iters_median']:.0f}, max {st['iters_max']}, "
@@ -126,7 +143,12 @@ def test(args):
         if st["capped"]:
             print(f"WARNING: {st['capped']} graph-step(s) hit the refinement cap ({eng.refine_max_iter} iterations) "
                   "with the CBF condition still violated; their actions are the capped iterates")
-    if args.log:
+    if args.log and perturbation is not None:
+        sx, sl, su = perturbation.sigmas(env)
+        with open(os.path.join(path, "test_log_noise.csv"), "a") as f:
+            f.write(f"{' '.join(map(str, sx))},{sl},{' '.join(map(str, su))},{perturbation.seed},"
+                    + log_row(env, args, summary) + "\n")
+    elif args.log:
         with open(os.path.join(path, "test_log.csv"), "a") as f:
             f.write(log_row(env, args, summary) + "\n")
     if getattr(args, "falsify", None) is not None:
@@ -323,6 +345,34 @@ def run_falsify(args, env, algo, eng, g0, path: str, step: int) -> None:
     print(f"falsify results: {f_out}")
 
 
+NOISE_FLAGS = (("--state-noise", "state_noise"), ("--lidar-noise", "lidar_noise"), ("--action-noise", "action_noise"))
+
+
+def noise_perturbation(args):
+    """The Perturbation of --state-noise / --lidar-noise / --action-noise (None without them): checked before any device
+    work.  Noisy evaluation runs one engine on the step-by-step path, so the sweeps and --falsify (which searches from
+    the noiseless states) are refused, naming the flag.  (A namespace parsed from FLAGS alone has none of the flags.)"""
+    given = [flag for flag, key in NOISE_FLAGS if getattr(args, key, None) is not None]
+    seed = getattr(args, "noise_seed", None)
+    if not given:
+        if seed is not None:
+            raise SystemExit("--noise-seed seeds the noise of --state-noise / --lidar-noise / --action-noise; give one "
+                             "of them")
+        return None
+    for flag, on in (("--paths", getattr(args, "paths", None) is not None),
+                     ("--all-steps", getattr(args, "all_steps", False)),
+                     ("--falsify", getattr(args, "falsify", None) is not None)):
+        if on:
+            raise SystemExit(f"{given[0]} evaluates one controller under noise; it cannot be combined with {flag}")
+    try:
+        return Perturbation(args.state_noise if args.state_noise is not None else 0.0,
+                            args.lidar_noise if args.lidar_noise is not None else 0.0,
+                            args.action_noise if args.action_noise is not None else 0.0,
+                            seed=args.seed if seed is None else seed, env_offset=args.offset)
+    except ValueError as e:
+        raise SystemExit(f"noise flags: {e}")
+
+
 def check_refine_flags(args) -> None:
     """--online-refine refines a trained GCBF+ policy: it needs --path and excludes --u-ref and the baselines."""
     if not args.online_refine:
@@ -363,11 +413,15 @@ FLAGS = [
 
 
 def build_test_parser():
-    """FLAGS plus the sweep flags (--paths takes several runs)."""
+    """FLAGS plus the sweep flags (--paths takes several runs) and the noise flags (the sigmas take one or more values)."""
     from train import build_parser
     parser = build_parser(FLAGS)
     parser.add_argument("--paths", type=str, nargs="+", default=None)
     parser.add_argument("--all-steps", action="store_true", default=False)
+    parser.add_argument("--state-noise", type=float, nargs="+", default=None)
+    parser.add_argument("--lidar-noise", type=float, default=None)
+    parser.add_argument("--action-noise", type=float, nargs="+", default=None)
+    parser.add_argument("--noise-seed", type=int, default=None)
     return parser
 
 
